@@ -12,6 +12,10 @@
  *   obca_check_parking        <- ParkingConstraints.jl:29-149  called from ParkingSignedDist.jl:253,278, ParkingDist.jl:259,277
  *   obca_parking_solve_mixed / obca_check_parking_mixed: the same two for a batch whose problems have different horizons
  *                                 (the Hybrid A* warm starts of main.jl:215-248 each come with their own N)
+ *   obca_quadcopter_solve_batch / obca_check_quadcopter  <- QuadcopterSignedDist.jl / QuadcopterDist.jl / constrSatisfaction.jl
+ *   obca_quadcopter_solve_mixed / obca_check_quadcopter_mixed: the same two for a batch whose problems have different
+ *                                 horizons and sampling times (the 3-D A* warm starts of mainQuadcopter.jl:122-137 each
+ *                                 come with their own N and Ts = round(Ts*80/N, 2))
  *
  * Conventions
  *   - every array is float64, COLUMN-MAJOR exactly as the Julia caller holds it; a batch of B problems is the B
@@ -155,6 +159,27 @@ int obca_quadcopter_solve_batch(int B, int N, const double* x0, const double* xF
 int obca_check_quadcopter(int B, int N, const double* x, const double* u, const double* timeScale, const double* x0,
                           const double* xF, double Ts, const double* lambda, const double* ob, double R,
                           const obca_opts* opts, int* feasible, double* worst);
+
+/* Batched QuadcopterSignedDist / QuadcopterDist over problems with different horizons and sampling times, in ONE solve.
+ * Problem b has horizon Nb[b], 2 <= Nb[b] <= Nmax, and sampling time Tsb[b] (finite, > 0).  Obstacles, R, the state
+ * bounds and timeWS are shared by the batch.  Every per-problem array has the shape it has in
+ * obca_quadcopter_solve_batch with N = Nmax (inputs xWS 12x(Nmax+1); outputs xp 12x(Nmax+1), up 4xNmax, ts Nmax+1,
+ * lp 30x(Nmax+1), slack 5x(Nmax+1)); problem b uses the first Nb[b]+1 stages and the first Nb[b] control columns of them.
+ * The solver never reads input entries past that point and never writes output entries past it.  Problem b's results
+ * (outputs over its own horizon, exitflag including the slack gate value 2, iters, kkt_err) are bit-identical to solving
+ * it with obca_quadcopter_solve_batch at N = Nb[b], Ts = Tsb[b] and the same options.  Nb or Tsb NULL, an Nb[b] outside
+ * [2, Nmax] or a Tsb[b] that is not a finite number > 0: OBCA_ERR_ARG (the index is in obca_last_error()), no output
+ * touched.  Nmax + 1 > 128 is answered like obca_quadcopter_solve_batch at N = Nmax. */
+int obca_quadcopter_solve_mixed(int B, const int* Nb, int Nmax, const double* x0, const double* xF, const double* Tsb,
+                                double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
+                                const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
+                                int* exitflag, int* iters, double* kkt_err, double* solve_seconds);
+
+/* obca_check_quadcopter over problems with different horizons and sampling times: Nb[b] in [2, Nmax], Tsb[b] finite > 0,
+ * arrays laid out for Nmax as in obca_quadcopter_solve_mixed; problem b is checked on its first Nb[b]+1 stages with Tsb[b]. */
+int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x, const double* u, const double* timeScale,
+                                const double* x0, const double* xF, const double* Tsb, const double* lambda,
+                                const double* ob, double R, const obca_opts* opts, int* feasible, double* worst);
 
 /* Device times of the last obca_parking_solve_batch[_dev] / obca_parking_solve_mixed on `device`: DualMultWS (0 when the caller passed lWS / nWS) and the
  * solve alone (= what solve_seconds reports; the reference's `time`, ParkingSignedDist.jl:297). */

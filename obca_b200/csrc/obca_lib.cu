@@ -10,7 +10,9 @@
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <string.h>
 
+#include <cmath>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -137,8 +139,12 @@ __global__ void k_check(const __grid_constant__ ParkProblem P, int B, const int*
 // ---------------------------------------------------------------------------------------------------------
 // quadcopter (obca_quad.cuh): persistent solver kernel + constrSatisfaction twin
 // ---------------------------------------------------------------------------------------------------------
+// Arrays laid out for the horizon c_qP.N.  Nb, Tsb (optional, together): per-problem horizons <= c_qP.N and sampling times;
+// when null, every problem has the horizon c_qP.N and the sampling time c_qP.Ts.
 struct QBatchPtrs {
   const double *x0, *xF, *xWS;
+  const int* Nb;
+  const double* Tsb;
   double timeWS;
   double *xp, *up, *ts, *lp, *slack;
   int *exitflag, *iters;
@@ -159,7 +165,7 @@ k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmO
   __shared__ double s_red[4 * 12];
   __shared__ int s_b;
   __shared__ double s_sum[4];
-  const int N = P.N, NS = N + 1;
+  const int N = P.N, NS = N + 1;      // the layout: strides of the per-problem arrays
   double* W = Wall + (size_t)blockIdx.x * L.total * L.NSP;
   for (;;) {
     if (threadIdx.x == 0) s_b = atomicAdd(counter, 1);
@@ -168,6 +174,7 @@ k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmO
     if (b >= bp.B) break;
     QCtx C;
     C.P = &P; C.O = &O; C.L = L; C.W = W; C.red_scratch = s_red; C.tile = s_kkt; C.S = &S;
+    C.N = bp.Nb ? bp.Nb[b] : c_qP.N; C.Ts = bp.Tsb ? bp.Tsb[b] : c_qP.Ts;      // this problem's horizon and sampling time
     C.in.x0 = bp.x0 + 12 * (size_t)b; C.in.xF = bp.xF + 12 * (size_t)b; C.in.xWS = bp.xWS + (size_t)12 * NS * b;
     C.in.timeWS = bp.timeWS;
     QOutputs out;
@@ -176,7 +183,8 @@ k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmO
     IpmDriver<QuadSolver<SDV> >::solve(C, 0);      // flag = 1 in the reference: a single attempt (QuadcopterSignedDist.jl:227-235)
     __syncthreads();
     double ssum = 0.0;
-    for (int k = threadIdx.x; k < NS; k += blockDim.x) {
+    const int Np = C.N;
+    for (int k = threadIdx.x; k <= Np; k += blockDim.x) {
       QuadSolver<SDV>::store_stage(C, k, out);
       if (SDV) for (int j = 0; j < QNOB; ++j) ssum += W[(size_t)(L.SLK + j) * L.NSP + k];
     }
@@ -185,7 +193,7 @@ k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmO
     __syncthreads();
     if (threadIdx.x == 0) {
       double tot = 0.0;
-      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += s_sum[w];
+      for (int w = 0; w < ((Np + 32) >> 5); ++w) tot += s_sum[w];      // the problem's own warps (see block_reduce)
       int ef = S.status == 1 ? 1 : 0;
       if (SDV && ef == 1 && tot > 1e-3) ef = 2;      // sum-slack gate, QuadcopterSignedDist.jl:283-288
       bp.exitflag[b] = ef; bp.iters[b] = S.iters; bp.kkt_err[b] = S.e0;
@@ -196,16 +204,20 @@ k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmO
   }
 }
 
-__global__ void k_quad_check(const __grid_constant__ QuadProblem P, int B, const double* __restrict__ x0,
-                             const double* __restrict__ xF, const double* __restrict__ x, const double* __restrict__ u,
-                             const double* __restrict__ ts, const double* __restrict__ lam, int* __restrict__ feasible,
-                             double* __restrict__ worst_out) {
+// Arrays laid out for the horizon P.N; Nb, Tsb (optional, together): problem b is checked on its stages 0..Nb[b] with the
+// sampling time Tsb[b].
+__global__ void k_quad_check(const __grid_constant__ QuadProblem P, int B, const int* __restrict__ Nb, const double* __restrict__ Tsb,
+                             const double* __restrict__ x0, const double* __restrict__ xF, const double* __restrict__ x,
+                             const double* __restrict__ u, const double* __restrict__ ts, const double* __restrict__ lam,
+                             int* __restrict__ feasible, double* __restrict__ worst_out) {
   __shared__ double s_w[4];
   const int N = P.N, NS = N + 1;
   for (int b = blockIdx.x; b < B; b += gridDim.x) {
+    const int Np = Nb ? Nb[b] : N;
+    const double Tsp = Tsb ? Tsb[b] : P.Ts;
     double w = 0.0;
-    for (int k = threadIdx.x; k < NS; k += blockDim.x)
-      w = fmax(w, quad_check_stage(P, k, x0 + 12 * (size_t)b, xF + 12 * (size_t)b, x + (size_t)12 * NS * b, u + (size_t)4 * N * b,
+    for (int k = threadIdx.x; k <= Np; k += blockDim.x)
+      w = fmax(w, quad_check_stage(P, Np, Tsp, k, x0 + 12 * (size_t)b, xF + 12 * (size_t)b, x + (size_t)12 * NS * b, u + (size_t)4 * N * b,
                                    ts + (size_t)NS * b, lam + (size_t)30 * NS * b));
     for (int off = 16; off > 0; off >>= 1) w = fmax(w, __shfl_down_sync(0xffffffffu, w, off));
     if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = w;
@@ -725,6 +737,117 @@ static int check_parking(int B, int N, const int* Nb, int nOb, const int* vOb, c
 }
 
 
+// The quadcopter solve behind the uniform and the mixed entries (host pointers, staged through one device buffer).  Every
+// per-problem array is laid out for the horizon N.  Nb, Tsb (host pointers, optional, together): per-problem horizons <= N
+// and sampling times; problem b uses the first Nb[b] + 1 stages of its arrays and nothing past them is written.
+static int quad_solve_host(int B, int N, const int* Nb, const double* Tsb, const double* x0, const double* xF, double Ts,
+                           double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
+                           const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
+                           int* exitflag, int* iters, double* kkt_err, double* solve_seconds) {
+  QuadProblem P;
+  if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  DevCtx* c;
+  int rc = get_ctx(opts ? opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  IpmOpts O = to_ipm(opts);
+  if (!opts) O.max_iter = 3000;                        // the reference sets no max_iter here (Ipopt default)
+  const size_t NS = N + 1;
+  const size_t n0 = 12 * (size_t)B, nx = 12 * NS * B, nu = 4 * (size_t)N * B, nt = NS * B, nl = 30 * NS * B, ns = 5 * NS * B;
+  const size_t dbytes = (2 * n0 + 2 * nx + nu + nt + nl + ns + B + (Nb ? B : 0)) * sizeof(double);
+  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + (Nb ? 3 : 2) * (size_t)B * sizeof(int));
+  if (rc) return rc;
+  double* d = (double*)c->stage;
+  double *d0 = d, *dF = d0 + n0, *dW = dF + n0, *dxp = dW + nx, *dup = dxp + nx, *dts = dup + nu, *dlp = dts + nt, *dsl = dlp + nl,
+         *derr = dsl + ns, *dTs = derr + B;
+  int* di = (int*)(c->stage + dbytes);
+  cudaStream_t st = c->st;
+  CK(cudaMemcpyAsync(d0, x0, n0 * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(dF, xF, n0 * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(dW, xWS, nx * 8, cudaMemcpyHostToDevice, st));
+  if (Nb) {
+    CK(cudaMemcpyAsync(di + 2 * (size_t)B, Nb, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dTs, Tsb, (size_t)B * 8, cudaMemcpyHostToDevice, st));
+  }
+  QBatchPtrs bp;
+  bp.x0 = d0; bp.xF = dF; bp.xWS = dW; bp.Nb = Nb ? di + 2 * (size_t)B : nullptr; bp.Tsb = Nb ? dTs : nullptr;
+  bp.timeWS = timeWS; bp.xp = dxp; bp.up = dup; bp.ts = dts; bp.lp = dlp; bp.slack = dsl;
+  bp.exitflag = di; bp.iters = di + B; bp.kkt_err = derr; bp.B = B; bp.prof = c->prof;
+  CK(cudaMemsetAsync(c->prof, 0, 8 * sizeof(unsigned long long), st));
+  CK(cudaEventRecord(c->ev0, st));
+  rc = signed_dist ? launch_quad<true>(*c, P, O, bp) : launch_quad<false>(*c, P, O, bp);
+  if (rc) return rc;
+  CK(cudaEventRecord(c->ev1, st));
+  if (!Nb) {
+    CK(cudaMemcpyAsync(xp, dxp, nx * 8, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(up, dup, nu * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(ts, dts, nt * 8, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(lp, dlp, nl * 8, cudaMemcpyDeviceToHost, st));
+    if (slack && signed_dist) CK(cudaMemcpyAsync(slack, dsl, ns * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(kkt_err, derr, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaMemcpyAsync(exitflag, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(iters, di + B, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(c->prof_host, c->prof, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  std::vector<double> h;
+  if (Nb) {     // the outputs come back through a host scratch; only each problem's own horizon goes to the caller's arrays
+    h.resize(nx + nu + nt + nl + ns + B);
+    CK(cudaMemcpyAsync(h.data(), dxp, h.size() * 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+  if (solve_seconds) *solve_seconds = ms * 1e-3;
+  if (Nb) {
+    const double *hx = h.data(), *hu = hx + nx, *ht = hu + nu, *hl = ht + nt, *hs = hl + nl, *he = hs + ns;
+    for (int q = 0; q < B; ++q) {
+      const size_t nsq = (size_t)Nb[q] + 1, nuq = (size_t)Nb[q];
+      memcpy(xp + 12 * NS * q, hx + 12 * NS * q, 12 * nsq * 8);
+      memcpy(up + 4 * (size_t)N * q, hu + 4 * (size_t)N * q, 4 * nuq * 8);
+      memcpy(ts + NS * q, ht + NS * q, nsq * 8);
+      memcpy(lp + 30 * NS * q, hl + 30 * NS * q, 30 * nsq * 8);
+      if (slack && signed_dist) memcpy(slack + 5 * NS * q, hs + 5 * NS * q, 5 * nsq * 8);
+    }
+    memcpy(kkt_err, he, (size_t)B * 8);
+  }
+  return 0;
+}
+
+// constrSatisfaction over a batch (host pointers).  Nb, Tsb (host pointers, optional, together): per-problem horizons <= N
+// and sampling times, with every per-problem array laid out for N.
+static int quad_check_host(int B, int N, const int* Nb, const double* Tsb, const double* x, const double* u,
+                           const double* timeScale, const double* x0, const double* xF, double Ts, const double* lambda,
+                           const double* ob, double R, const obca_opts* opts, int* feasible, double* worst) {
+  if (B <= 0 || !x || !u || !timeScale || !x0 || !xF || !lambda || !ob || !feasible) { set_err("null argument"); return OBCA_ERR_ARG; }
+  QuadProblem P;
+  if (fill_quad_problem(P, N, Ts, R, ob, 0)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  DevCtx* c;
+  int rc = get_ctx(opts ? opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  const size_t NS = N + 1;
+  const size_t n0 = 12 * (size_t)B, nx = 12 * NS * B, nu = 4 * (size_t)N * B, nt = NS * B, nl = 30 * NS * B;
+  const size_t dbytes = (2 * n0 + nx + nu + nt + nl + B + (Nb ? B : 0)) * sizeof(double);
+  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + (Nb ? 2 : 1) * (size_t)B * sizeof(int));
+  if (rc) return rc;
+  double* d = (double*)c->stage;
+  double *d0 = d, *dF = d0 + n0, *dx = dF + n0, *du = dx + nx, *dt = du + nu, *dl = dt + nt, *dw = dl + nl, *dTs = dw + B;
+  int* di = (int*)(c->stage + dbytes);
+  cudaStream_t st = c->st;
+  CK(cudaMemcpyAsync(d0, x0, n0 * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dF, xF, n0 * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(dx, x, nx * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(du, u, nu * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(dt, timeScale, nt * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dl, lambda, nl * 8, cudaMemcpyHostToDevice, st));
+  if (Nb) {
+    CK(cudaMemcpyAsync(di + B, Nb, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dTs, Tsb, (size_t)B * 8, cudaMemcpyHostToDevice, st));
+  }
+  const int grid = B < 4 * c->sms ? B : 4 * c->sms;
+  k_quad_check<<<grid, 128, 0, st>>>(P, B, Nb ? di + B : nullptr, Nb ? dTs : nullptr, d0, dF, dx, du, dt, dl, di, dw);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(feasible, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (worst) CK(cudaMemcpyAsync(worst, dw, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
 extern "C" {
 
 #ifdef OBCA_QPROF   // development builds only: cycles of the quadcopter sweep's phases, summed over CTAs; resets the counters
@@ -786,6 +909,17 @@ static int check_horizons(int B, const int* Nb, int Nmax) {
   for (int q = 0; q < B; ++q)
     if (Nb[q] < 2 || Nb[q] > Nmax) {
       set_err("Nb[" + std::to_string(q) + "] = " + std::to_string(Nb[q]) + " outside [2, Nmax = " + std::to_string(Nmax) + "]");
+      return OBCA_ERR_ARG;
+    }
+  return 0;
+}
+
+// per-problem sampling times: finite and > 0
+static int check_sampling_times(int B, const double* Tsb) {
+  if (!Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
+  for (int q = 0; q < B; ++q)
+    if (!(std::isfinite(Tsb[q]) && Tsb[q] > 0.0)) {
+      set_err("Tsb[" + std::to_string(q) + "] = " + std::to_string(Tsb[q]) + " is not a finite sampling time > 0");
       return OBCA_ERR_ARG;
     }
   return 0;
@@ -861,78 +995,40 @@ int obca_quadcopter_solve_batch(int B, int N, const double* x0, const double* xF
   if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
     set_err("null argument"); return OBCA_ERR_ARG;
   }
-  QuadProblem P;
-  if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
-  DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
+  return quad_solve_host(B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
+                         exitflag, iters, kkt_err, solve_seconds);
+}
+
+int obca_quadcopter_solve_mixed(int B, const int* Nb, int Nmax, const double* x0, const double* xF, const double* Tsb,
+                                double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
+                                const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
+                                int* exitflag, int* iters, double* kkt_err, double* solve_seconds) {
+  if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
+    set_err("null argument"); return OBCA_ERR_ARG;
+  }
+  int rc = check_horizons(B, Nb, Nmax);
   if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  IpmOpts O = to_ipm(opts);
-  if (!opts) O.max_iter = 3000;                        // the reference sets no max_iter here (Ipopt default)
-  const size_t NS = N + 1;
-  const size_t n0 = 12 * (size_t)B, nx = 12 * NS * B, nu = 4 * (size_t)N * B, nt = NS * B, nl = 30 * NS * B, ns = 5 * NS * B;
-  const size_t dbytes = (2 * n0 + 2 * nx + nu + nt + nl + ns + B) * sizeof(double);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + 2 * (size_t)B * sizeof(int));
+  rc = check_sampling_times(B, Tsb);
   if (rc) return rc;
-  double* d = (double*)c->stage;
-  double *d0 = d, *dF = d0 + n0, *dW = dF + n0, *dxp = dW + nx, *dup = dxp + nx, *dts = dup + nu, *dlp = dts + nt, *dsl = dlp + nl,
-         *derr = dsl + ns;
-  int* di = (int*)(c->stage + dbytes);
-  cudaStream_t st = c->st;
-  CK(cudaMemcpyAsync(d0, x0, n0 * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dF, xF, n0 * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dW, xWS, nx * 8, cudaMemcpyHostToDevice, st));
-  QBatchPtrs bp;
-  bp.x0 = d0; bp.xF = dF; bp.xWS = dW; bp.timeWS = timeWS; bp.xp = dxp; bp.up = dup; bp.ts = dts; bp.lp = dlp; bp.slack = dsl;
-  bp.exitflag = di; bp.iters = di + B; bp.kkt_err = derr; bp.B = B; bp.prof = c->prof;
-  CK(cudaMemsetAsync(c->prof, 0, 8 * sizeof(unsigned long long), st));
-  CK(cudaEventRecord(c->ev0, st));
-  rc = signed_dist ? launch_quad<true>(*c, P, O, bp) : launch_quad<false>(*c, P, O, bp);
-  if (rc) return rc;
-  CK(cudaEventRecord(c->ev1, st));
-  CK(cudaMemcpyAsync(xp, dxp, nx * 8, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(up, dup, nu * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(ts, dts, nt * 8, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(lp, dlp, nl * 8, cudaMemcpyDeviceToHost, st));
-  if (slack && signed_dist) CK(cudaMemcpyAsync(slack, dsl, ns * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(kkt_err, derr, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(exitflag, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(iters, di + B, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(c->prof_host, c->prof, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-  if (solve_seconds) *solve_seconds = ms * 1e-3;
-  return 0;
+  // the batch has no sampling time of its own: NaN, so that a read of it instead of Tsb[b] could not go unnoticed
+  return quad_solve_host(B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
+                         exitflag, iters, kkt_err, solve_seconds);
 }
 
 int obca_check_quadcopter(int B, int N, const double* x, const double* u, const double* timeScale, const double* x0,
                           const double* xF, double Ts, const double* lambda, const double* ob, double R,
                           const obca_opts* opts, int* feasible, double* worst) {
-  if (B <= 0 || !x || !u || !timeScale || !x0 || !xF || !lambda || !ob || !feasible) { set_err("null argument"); return OBCA_ERR_ARG; }
-  QuadProblem P;
-  if (fill_quad_problem(P, N, Ts, R, ob, 0)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
-  DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
+  return quad_check_host(B, N, nullptr, nullptr, x, u, timeScale, x0, xF, Ts, lambda, ob, R, opts, feasible, worst);
+}
+
+int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x, const double* u, const double* timeScale,
+                                const double* x0, const double* xF, const double* Tsb, const double* lambda,
+                                const double* ob, double R, const obca_opts* opts, int* feasible, double* worst) {
+  int rc = check_horizons(B, Nb, Nmax);
   if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  const size_t NS = N + 1;
-  const size_t n0 = 12 * (size_t)B, nx = 12 * NS * B, nu = 4 * (size_t)N * B, nt = NS * B, nl = 30 * NS * B;
-  const size_t dbytes = (2 * n0 + nx + nu + nt + nl + B) * sizeof(double);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + (size_t)B * sizeof(int));
+  rc = check_sampling_times(B, Tsb);
   if (rc) return rc;
-  double* d = (double*)c->stage;
-  double *d0 = d, *dF = d0 + n0, *dx = dF + n0, *du = dx + nx, *dt = du + nu, *dl = dt + nt, *dw = dl + nl;
-  int* di = (int*)(c->stage + dbytes);
-  cudaStream_t st = c->st;
-  CK(cudaMemcpyAsync(d0, x0, n0 * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dF, xF, n0 * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dx, x, nx * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(du, u, nu * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dt, timeScale, nt * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dl, lambda, nl * 8, cudaMemcpyHostToDevice, st));
-  const int grid = B < 4 * c->sms ? B : 4 * c->sms;
-  k_quad_check<<<grid, 128, 0, st>>>(P, B, d0, dF, dx, du, dt, dl, di, dw);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(feasible, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (worst) CK(cudaMemcpyAsync(worst, dw, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
+  return quad_check_host(B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst);
 }
 
 int obca_last_profile(int device, unsigned long long* out8) {

@@ -26,8 +26,8 @@ constexpr double QUAD_WH = 4.479906037125444;   // sqrt(mass*g/(4 k_F)) = sqrt(0
 constexpr int QNOB = 5;
 
 struct QuadProblem {
-  int N;
-  double Ts, R;
+  int N;          // the horizon the batch's arrays and the workspace are laid out for (the largest of a mixed batch)
+  double Ts, R;   // Ts: the batch's sampling time when it has one; each problem's own horizon and Ts are in QCtx
   double obs[QNOB][6];
   double xlo[QNX], xhi[QNX];   // :78-93 (x10 bounds differ between the variants, QuadcopterDist.jl:88)
   int signed_dist;
@@ -74,7 +74,9 @@ struct QOutputs {
 };
 
 struct QCtx {
-  const QuadProblem* P;
+  const QuadProblem* P;   // P->N, P->Ts: the horizon the batch's arrays are laid out for and the batch's sampling time
+  int N;                  // horizon of this problem (<= P->N): every stage loop, the KKT sweep and the reductions run to it
+  double Ts;              // sampling time of this problem
   const IpmOpts* O;
   QLay L;
   double* W;
@@ -82,6 +84,9 @@ struct QCtx {
   double* tile;
   ProbState* S;
   QInputs in;
+#if !defined(__CUDACC__)
+  QCtx() : N(0), Ts(0.0) {}   // host (development emulation): a context built without a horizon solves at P->N, P->Ts
+#endif
 };
 
 // Problem, options and layout: __constant__ memory on the device (as for the parking model, obca_solver.cuh), the context on the host.
@@ -101,6 +106,15 @@ __constant__ QLay c_qL;
 #define QCTX_L(C) ((C).L)
 #define QLOCALS(C) double* const W_ = (C).W; (void)W_
 #endif
+// horizon and sampling time of the problem of context C.  The device kernel always sets both; on the host C.N = 0 stands for
+// the layout's horizon and the batch's sampling time.
+#if defined(__CUDA_ARCH__)
+#define QCTX_N(C) ((C).N)
+#define QCTX_TS(C) ((C).Ts)
+#else
+#define QCTX_N(C) ((C).N > 0 ? (C).N : (C).P->N)
+#define QCTX_TS(C) ((C).N > 0 ? (C).Ts : (C).P->Ts)
+#endif
 #define QA(name, i, k) (W_[(size_t)(QCTX_L(C).name + (i)) * QCTX_L(C).NSP + (k)])
 
 OBCA_HD void quad_jac_tables(const int*& jr, const int*& jc, const int*& hi, const int*& hj) {
@@ -119,10 +133,16 @@ struct QuadSolver {
   typedef QCtx Ctx;
   typedef QLocalDims<SDV> LD;
 
-  OBCA_HD static int n_stages(const QCtx& C) { return QCTX_P(C).N + 1; }
+  OBCA_HD static int n_stages(const QCtx& C) { return QCTX_N(C) + 1; }
+#if defined(__CUDA_ARCH__)
+  // block reductions over the problem's own ceil((N+1)/32) warps, so that a problem gives the same bits in a CTA sized for a
+  // longer horizon of its batch as in one sized for its own
+  template <typename T>
+  __device__ static void reduce(T& v, const QCtx& C) { block_reduce_warps(v, C.red_scratch, (QCTX_N(C) + 32) >> 5); }
+#endif
   OBCA_HD static bool fixed_time(const QCtx&) { return false; }
   OBCA_HD static void mult_counts(const QCtx& C, double& n_mult, double& n_bmult) {
-    const double N = QCTX_P(C).N, NS = N + 1;
+    const double N = QCTX_N(C), NS = N + 1;
     double nb = 24.0 * (N - 1) + 8.0 * N + 30.0 * NS + 2.0 * NS + (SDV ? 5.0 * NS : 0.0);   // variable bounds
     nb += 5.0 * NS;                                                                          // dist slack bounds
     n_bmult = nb; n_mult = nb + 12.0 * N + 5.0 * NS + 5.0 * NS;
@@ -174,7 +194,7 @@ struct QuadSolver {
     QLOCALS(C);
     const QuadProblem& P = QCTX_P(C);
     const IpmOpts& O = QCTX_O(C);
-    const int N = P.N;
+    const int N = QCTX_N(C);
     const bool free_x = (k >= 1 && k <= N - 1);
     for (int i = 0; i < QNX; ++i) {
       double v = restart ? QA(X, i, k) : C.in.xWS[(size_t)QNX * k + i];
@@ -227,7 +247,7 @@ struct QuadSolver {
     QLOCALS(C);
     const QuadProblem& P = QCTX_P(C);
     const ProbState& S = *C.S;
-    const int N = P.N;
+    const int N = QCTX_N(C);
     const double mu_b = S.mu, dw = S.dw, t = S.t;
     const bool free_x = (k >= 1 && k <= N - 1);
     const bool has_u = k < N;
@@ -290,7 +310,7 @@ struct QuadSolver {
         }
       }
       double f[QNX], Jv[QD_NJ], Hv[QD_NH];
-      quad_dyn_full(x, u, t, P.Ts, c0, pi, f, Jv, Hv);
+      quad_dyn_full(x, u, t, QCTX_TS(C), c0, pi, f, Jv, Hv);
       const int *jr, *jc, *hi, *hj;
       quad_jac_tables(jr, jc, hi, hj);
       if (do_asm) {
@@ -386,9 +406,8 @@ struct QuadSolver {
   // ---- K3: dense Riccati sweep over [x | w | t] (17) with 4 controls, run by one thread ----
   OBCA_HD static int kkt_dense(const QCtx& C) {
     QLOCALS(C);
-    const QuadProblem& Pp = QCTX_P(C);
     ProbState& S = *C.S;
-    const int N = Pp.N;
+    const int N = QCTX_N(C);
     const int *jr, *jc, *hi, *hj;
     quad_jac_tables(jr, jc, hi, hj);
     double P[QNSV][QNSV], p[QNSV];
@@ -582,7 +601,7 @@ struct QuadSolver {
     long long qacc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, qt = clock64();
 #endif
     ProbState& S = *C.S;
-    const int N = QCTX_P(C).N;
+    const int N = QCTX_N(C);
     const int tid = threadIdx.x, nt = blockDim.x;
     const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
     const int gid = lane >> 2, tig = lane & 3;
@@ -845,7 +864,7 @@ struct QuadSolver {
     QLOCALS(C);
     const QuadProblem& P = QCTX_P(C);
     const ProbState& S = *C.S;
-    const int N = P.N;
+    const int N = QCTX_N(C);
     const double mu_b = S.mu, tau = S.tau;
     const bool free_x = (k >= 1 && k <= N - 1);
     double apr = 1.0, adu = 1.0, dphi = 0.0;
@@ -933,7 +952,7 @@ struct QuadSolver {
     QLOCALS(C);
     const QuadProblem& P = QCTX_P(C);
     const ProbState& S = *C.S;
-    const int N = P.N;
+    const int N = QCTX_N(C);
     const double mu_b = S.mu;
     const bool free_x = (k >= 1 && k <= N - 1);
     const double t = S.t + alpha * S.dt;
@@ -961,7 +980,7 @@ struct QuadSolver {
         lacc.add(al); lacc.add(au);
       }
       double f[QNX];
-      quad_dyn_f(x, u, t, P.Ts, c0, f);
+      quad_dyn_f(x, u, t, QCTX_TS(C), c0, f);
       for (int i = 0; i < QNX; ++i) {
         const double xn = (k + 1 == N) ? C.in.xF[i] : QA(X, i, k + 1) + alpha * QA(dX, i, k + 1);
         th += dabs(f[i] - xn);
@@ -998,7 +1017,7 @@ struct QuadSolver {
     QLOCALS(C);
     const QuadProblem& P = QCTX_P(C);
     const ProbState& S = *C.S;
-    const int N = P.N;
+    const int N = QCTX_N(C);
     const double mu_b = S.mu, ks = QCTX_O(C).kappa_sigma;
     const double alpha = S.alpha, adu = S.a_du, ay = dmin_(S.alpha, S.a_du);
     const bool free_x = (k >= 1 && k <= N - 1);
@@ -1043,25 +1062,25 @@ struct QuadSolver {
   // phase wrappers of the generic driver (the quadcopter model has no separate item pass: its 5 box blocks are evaluated
   // inside the stage functions)
   OBCA_HD static void eval_phase(const QCtx& C, bool do_err, EvalPart& ep) {
-    const int NS = QCTX_P(C).N + 1;
+    const int NS = QCTX_N(C) + 1;
     OBCA_FOR_STAGES(k, NS) { EvalPart e1; stage_eval(C, k, do_err, true, e1); part_merge(ep, e1); }
   }
   OBCA_HD static void recover_phase(const QCtx& C, StepPart& sp) {
-    const int NS = QCTX_P(C).N + 1;
+    const int NS = QCTX_N(C) + 1;
     OBCA_FOR_STAGES(k, NS) { StepPart s1; recover_stage(C, k, s1); part_merge(sp, s1); }
   }
   OBCA_HD static void merit_phase(const QCtx& C, double alpha, MeritPart& mp) {
-    const int NS = QCTX_P(C).N + 1;
+    const int NS = QCTX_N(C) + 1;
     OBCA_FOR_STAGES(k, NS) { MeritPart m1; merit_stage(C, k, alpha, m1); part_merge(mp, m1); }
   }
   OBCA_HD static void update_phase(const QCtx& C) {
-    const int NS = QCTX_P(C).N + 1;
+    const int NS = QCTX_N(C) + 1;
     OBCA_FOR_STAGES(k, NS) update_stage(C, k);
   }
 
   OBCA_HD static void store_stage(const QCtx& C, int k, const QOutputs& o) {
     QLOCALS(C);
-    const int N = QCTX_P(C).N;
+    const int N = QCTX_N(C);
     for (int i = 0; i < QNX; ++i) o.xp[(size_t)QNX * k + i] = QA(X, i, k);
     if (k < N) for (int j = 0; j < QNU; ++j) o.up[(size_t)QNU * k + j] = QA(U, j, k);
     o.ts[k] = C.S->t;
@@ -1076,11 +1095,11 @@ struct QuadSolver {
 // rows checked for i = 1..N only (:80), state box of the Dist variant ([-1.5, 3] on x10, :107,:119) for both
 // variants, norm row one-sided (<= 0, :166-176), quirk Q5 in the body-rate rows (:151-153).
 // x 12x(N+1), u 4xN, ts (N+1), lambda 30x(N+1) column-major.  Returns the worst violation per stage in `v`
-// (<= 1e-3 everywhere  <=>  the reference returns true).
+// (<= 1e-3 everywhere  <=>  the reference returns true).  N, Ts: the problem's own horizon and sampling time (P.N is the
+// layout's horizon of a batch, P.Ts its shared sampling time).
 // ------------------------------------------------------------------------------------------------------------
-OBCA_HD double quad_check_stage(const QuadProblem& P, int k, const double* x0, const double* xF, const double* x,
+OBCA_HD double quad_check_stage(const QuadProblem& P, int N, double Ts, int k, const double* x0, const double* xF, const double* x,
                                 const double* u, const double* ts, const double* lam) {
-  const int N = P.N;
   double worst = 0.0;
   if (k == 0)
     for (int i = 0; i < QNX; ++i) worst = dmax(worst, dabs(x[i] - x0[i]));                          // :56-61
@@ -1101,7 +1120,7 @@ OBCA_HD double quad_check_stage(const QuadProblem& P, int k, const double* x0, c
     if (lo[i] - xk[i] > 0.0 || xk[i] - hi[i] > 0.0) worst = dmax(worst, 1.0);
   double f[QNX];
   const double c0[3] = {x[9], x[10], x[11]};                                                         // linear indexing, :151-153
-  quad_dyn_f(xk, uk, ts[k], P.Ts, c0, f);
+  quad_dyn_f(xk, uk, ts[k], Ts, c0, f);
   for (int i = 0; i < QNX; ++i) worst = dmax(worst, dabs(x[(size_t)QNX * (k + 1) + i] - f[i]));      // :127-153
   worst = dmax(worst, dabs(ts[k] - ts[k + 1]));                                                      // :154
   for (int o = 0; o < QNOB; ++o) {

@@ -100,9 +100,23 @@ __device__ __forceinline__ void block_reduce(T& v, void* scratch) {
   if (threadIdx.x == 0)
     for (int w = 1; w < (int)((blockDim.x + 31) >> 5); ++w) part_merge(v, sc[w]);
 }
+// the same, merging only the first nw warps of the block: a problem that needs fewer warps than its CTA has merges only its
+// own (the surplus warps hold identities, but -0.0 + 0.0 = +0.0, so merging them could change the sign of a zero sum)
+template <typename T>
+__device__ __forceinline__ void block_reduce_warps(T& v, void* scratch, int nw) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) { T o = part_shfl(v, off); part_merge(v, o); }
+  T* sc = reinterpret_cast<T*>(scratch);
+  if ((threadIdx.x & 31) == 0) sc[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < nw; ++w) part_merge(v, sc[w]);
+}
 #define OBCA_REDUCE(v) block_reduce(v, C.red_scratch)
+#define OBCA_REDUCE_M(v) M::reduce(v, C)      // IpmDriver<M>: the model's own block reduction
 #else
 #define OBCA_REDUCE(v)
+#define OBCA_REDUCE_M(v)
 #endif
 
 // ---- what one (stage, obstacle) OBCA block contributes to its stage (K1).  The blocks are evaluated by the "item" pass of
@@ -1515,6 +1529,8 @@ struct ParkSolver {
   static constexpr bool KKT_BLOCK = false;   // the KKT sweep is run by warp 0 (kkt_solve_warp)
 #if defined(__CUDA_ARCH__)
   __device__ static int kkt_solve_block(const PkCtx&) { return 0; }
+  template <typename T>
+  __device__ static void reduce(T& v, const PkCtx& C) { block_reduce(v, C.red_scratch); }   // every warp of the CTA
 #endif
   OBCA_HD static int n_stages(const PkCtx& C) { return CTX_N(C) + 1; }
   OBCA_HD static bool fixed_time(const PkCtx& C) { return CTX_P(C).fix_time != 0; }
@@ -1597,7 +1613,7 @@ struct IpmDriver {
       EvalPart ep;
       part_init(ep);
       M::eval_phase(C, true, ep);
-      OBCA_REDUCE(ep);
+      OBCA_REDUCE_M(ep);
       OBCA_PROF(0); OBCA_PROF_COUNT(7);
       OBCA_SERIAL {
         apply_errors(C, ep);
@@ -1631,7 +1647,7 @@ struct IpmDriver {
       if (S.flag == 2) {   // mu changed: the barrier terms of the stage models (and phi) are stale
         part_init(ep);
         M::eval_phase(C, true, ep);
-        OBCA_REDUCE(ep);
+        OBCA_REDUCE_M(ep);
         OBCA_PROF(0); OBCA_PROF_COUNT(7);
         OBCA_SERIAL { apply_errors(C, ep); S.ok = ep.ok; }
         OBCA_SYNC();
@@ -1671,7 +1687,7 @@ struct IpmDriver {
         if (S.ok != 0) break;
         part_init(ep);
         M::eval_phase(C, false, ep);
-        OBCA_REDUCE(ep);
+        OBCA_REDUCE_M(ep);
         OBCA_SERIAL { S.ok = ep.ok; }
         OBCA_SYNC();
         OBCA_PROF(0); OBCA_PROF_COUNT(7);
@@ -1682,7 +1698,7 @@ struct IpmDriver {
       StepPart sp;
       part_init(sp);
       M::recover_phase(C, sp);
-      OBCA_REDUCE(sp);
+      OBCA_REDUCE_M(sp);
       OBCA_PROF(2);
       OBCA_SERIAL {
         const double apr = sp.apr, adu = sp.adu, dphi = sp.dphi;
@@ -1703,7 +1719,7 @@ struct IpmDriver {
         MeritPart mp;
         part_init(mp);
         M::merit_phase(C, alpha, mp);
-        OBCA_REDUCE(mp);
+        OBCA_REDUCE_M(mp);
         OBCA_PROF(3); OBCA_PROF_COUNT(6);
         OBCA_SERIAL {
           const double th = mp.th, ph = mp.phi;

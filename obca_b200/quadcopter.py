@@ -4,7 +4,8 @@
     QuadcopterDist        QuadcopterNavigation/QuadcopterDist.jl:25       -> same 7-tuple :280
     constrSatisfaction    QuadcopterNavigation/constrSatisfaction.jl:25   -> Bool
 
-All computation happens in libobca.so on the GPU (obca_quadcopter_solve_batch / obca_check_quadcopter)."""
+All computation happens in libobca.so on the GPU (obca_quadcopter_solve_batch / obca_check_quadcopter, and their _mixed
+twins for a batch whose problems have their own horizon and sampling time)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -13,6 +14,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import check, f64, lib, ptr
+from .parking import _pad_stages
 
 
 def quadcopter_solve_batch(x0, xF, N, Ts, R, obs, xWS, timeWS=1.0, signed_dist=1, opts=None):
@@ -31,6 +33,37 @@ def quadcopter_solve_batch(x0, xF, N, Ts, R, obs, xWS, timeWS=1.0, signed_dist=1
                                             ptr(lp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
     T = lambda a: np.transpose(a, (0, 2, 1))
     return dict(xp=T(xp), up=T(up), ts=ts, lp=T(lp), slack=T(sl), exitflag=ef, iters=it, kkt_err=err, time=float(sec[0]))
+
+
+def _per_problem(Ns, Ts):
+    Ns = np.ascontiguousarray(np.asarray(Ns).ravel(), dtype=np.int32)
+    Tsb = f64(np.broadcast_to(np.asarray(Ts, float).ravel() if np.ndim(Ts) else float(Ts), (len(Ns),)))
+    return Ns, Tsb, int(Ns.max())
+
+
+def quadcopter_solve_mixed(x0, xF, Ns, Ts, R, obs, xWS, timeWS=1.0, signed_dist=1, opts=None):
+    """One batched solve of problems with different horizons Ns[i] and sampling times (obca_quadcopter_solve_mixed).
+    x0, xF (B,12); Ts scalar or (B,); obs (5,6); xWS per-problem list, xWS[i] 12x(Ns[i]+1).  Problem i gives exactly what
+    quadcopter_solve_batch gives it at N = Ns[i], Ts = Ts[i].  Returns dict of per-problem lists in the Julia shapes
+    (xp[i] 12x(Ns[i]+1), up[i] 4xNs[i], ts[i] Ns[i]+1, lp[i] 30x(Ns[i]+1), slack[i] 5x(Ns[i]+1)), the arrays exitflag,
+    iters, kkt_err, N, Ts, and time."""
+    x0 = f64(np.atleast_2d(x0)); B = x0.shape[0]
+    Ns, Tsb, Nmax = _per_problem(Ns, Ts)
+    assert len(Ns) == B
+    NS = Nmax + 1
+    xF = f64(np.broadcast_to(np.asarray(xF, float).reshape(-1, 12), (B, 12)))
+    ob = f64(np.asarray(obs, float).reshape(5, 6))
+    xw = f64(_pad_stages([np.asarray(w, float).reshape(12, -1)[:, :n + 1].T for w, n in zip(xWS, Ns)], Nmax))
+    xp = np.zeros((B, NS, 12)); up = np.zeros((B, Nmax, 4)); ts = np.zeros((B, NS)); lp = np.zeros((B, NS, 30)); sl = np.zeros((B, NS, 5))
+    ef = np.zeros(B, np.int32); it = np.zeros(B, np.int32); err = np.zeros(B); sec = np.zeros(1)
+    if opts is None:
+        opts = _lib.default_opts(); opts.max_iter = 3000                 # as quadcopter_solve_batch
+    check(lib().obca_quadcopter_solve_mixed(C.c_int(B), ptr(Ns), C.c_int(Nmax), ptr(x0), ptr(xF), ptr(Tsb), C.c_double(R), ptr(ob), ptr(xw),
+                                            C.c_double(float(timeWS)), C.c_int(int(signed_dist)), C.byref(opts), ptr(xp), ptr(up), ptr(ts),
+                                            ptr(lp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
+    cut = lambda a, ext: [a[i, :n + ext].T.copy() for i, n in enumerate(Ns)]
+    return dict(xp=cut(xp, 1), up=cut(up, 0), ts=[ts[i, :n + 1].copy() for i, n in enumerate(Ns)], lp=cut(lp, 1), slack=cut(sl, 1),
+                exitflag=ef, iters=it, kkt_err=err, N=Ns.copy(), Ts=Tsb.copy(), time=float(sec[0]))
 
 
 def _single(sd, x0, xF, N, Ts, R, ob1, ob2, ob3, ob4, ob5, xWS, uWS, timeWS):
@@ -61,6 +94,25 @@ def check_quadcopter_batch(x, u, timeScale, x0, xF, Ts, lam, obs, R, opts=None):
     o = opts if opts is not None else _lib.default_opts()
     check(lib().obca_check_quadcopter(C.c_int(B), C.c_int(N), ptr(xx), ptr(uu), ptr(tt), ptr(x0), ptr(xF), C.c_double(Ts), ptr(ll), ptr(ob),
                                       C.c_double(R), C.byref(o), ptr(feas), ptr(worst)))
+    return feas, worst
+
+
+def check_quadcopter_mixed(x, u, timeScale, x0, xF, Ns, Ts, lam, obs, R, opts=None):
+    """check_quadcopter_batch over problems with different horizons Ns[i] and sampling times Ts (scalar or (B,))
+    (obca_check_quadcopter_mixed): per-problem lists x[i] 12x(Ns[i]+1), u[i] 4xNs[i], timeScale[i] Ns[i]+1,
+    lam[i] 30x(Ns[i]+1)."""
+    Ns, Tsb, Nmax = _per_problem(Ns, Ts)
+    B = len(Ns)
+    P = lambda arrs, ext: f64(_pad_stages([np.asarray(a, float).T[:k + ext] for a, k in zip(arrs, Ns)], Nmax))
+    xx, ll = P(x, 1), P(lam, 1)
+    uu = f64(P(u, 0)[:, :Nmax])
+    tt = f64(_pad_stages([np.ravel(t)[:k + 1] for t, k in zip(timeScale, Ns)], Nmax))
+    x0 = f64(np.broadcast_to(np.asarray(x0, float).reshape(-1, 12), (B, 12))); xF = f64(np.broadcast_to(np.asarray(xF, float).reshape(-1, 12), (B, 12)))
+    ob = f64(np.asarray(obs, float).reshape(5, 6))
+    feas = np.zeros(B, np.int32); worst = np.zeros(B)
+    o = opts if opts is not None else _lib.default_opts()
+    check(lib().obca_check_quadcopter_mixed(C.c_int(B), ptr(Ns), C.c_int(Nmax), ptr(xx), ptr(uu), ptr(tt), ptr(x0), ptr(xF), ptr(Tsb),
+                                            ptr(ll), ptr(ob), C.c_double(R), C.byref(o), ptr(feas), ptr(worst)))
     return feas, worst
 
 

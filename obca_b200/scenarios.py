@@ -8,6 +8,8 @@
   artefacts main.jl hands to ParkingSignedDist: rx, ry, ryaw (N+1), xWS (N+1)x4, uWS Nx2.
 * ``reverse_parking_batch`` -- BASELINE config 2: randomised start poses, numpy default_rng(seed).
 * ``reverse_parking_mixed_batch`` -- the same with a seeded horizon per problem (input of parking_solve_mixed).
+* ``quadcopter_mixed_batch`` -- BASELINE config 4 with a seeded horizon and its sampling time per problem (input of
+  quadcopter_solve_mixed).
 """
 from __future__ import annotations
 
@@ -231,6 +233,25 @@ def quadcopter_batch(B, N=100, seed=2):
     Ts = round((sc["Ts80"] * 80 / N) * 100) / 100
     xWS = np.stack([warmstart_quadcopter(x0[i], xF[i], N) for i in range(B)])
     sc.update(B=B, N=N, Ts=Ts, x0=x0, xF=xF, xWS=xWS, timeWS=1.0)
+    return sc
+
+
+def quadcopter_mixed_batch(B, N_range=(90, 127), seed=2, Ns=None):
+    """Config 4 with a horizon and a sampling time per problem (what a batch of 3-D A* warm starts looks like,
+    mainQuadcopter.jl:122-137): x0 / xF drawn exactly as in quadcopter_batch, then N_i ~ uniform over N_range (inclusive)
+    from the same generator unless Ns is given, Ts_i = round(Ts80 * 80 / N_i, 2) (:131) and the warm start at N_i.
+    The default range is the one the 3-D A* gives for config-4 start / goal pairs.  Ns, Ts are arrays; xWS[i] is
+    12 x (N_i+1)."""
+    sc = quadcopter_scenario()
+    rng = np.random.default_rng(seed)
+    x0 = np.zeros((B, 12)); xF = np.zeros((B, 12))
+    x0[:, 0] = 1; xF[:, 0] = 9
+    x0[:, 1] = rng.uniform(0.5, 9.5, B); x0[:, 2] = rng.uniform(0.5, 4.5, B)
+    xF[:, 1] = rng.uniform(0.5, 9.5, B); xF[:, 2] = rng.uniform(0.5, 4.5, B)
+    Ns = np.asarray(Ns if Ns is not None else rng.integers(N_range[0], N_range[1] + 1, B), dtype=np.int32)
+    Ts = np.array([round((sc["Ts80"] * 80 / int(n)) * 100) / 100 for n in Ns])      # as quadcopter_batch
+    xWS = [warmstart_quadcopter(x0[i], xF[i], int(Ns[i])) for i in range(B)]
+    sc.update(B=B, Ns=Ns, Ts=Ts, x0=x0, xF=xF, xWS=xWS, timeWS=1.0)
     return sc
 
 
