@@ -1,7 +1,10 @@
 """The flow of the reference's QuadcopterNavigation/mainQuadcopter.jl: environment and 3-D A* (mainQuadcopter.jl:36-128), warm
 start (:130-137), QuadcopterDist and QuadcopterSignedDist on the GPU (:145, :152), constrSatisfaction (:147, :154).
 
-usage: python examples/main_quadcopter.py                                          (needs a CUDA device for the two solves)
+usage: python examples/main_quadcopter.py [Y0 Z0 YF ZF]                            (needs a CUDA device for the two solves)
+
+Y0 Z0 YF ZF: the start (1, Y0, Z0) and the goal (9, YF, ZF) the reference asks its user to edit (mainQuadcopter.jl:48-51);
+by default the reference's (1, 1, 3) -> (9, 3, 2).  Corners of the box, e.g. 9.5 4.5 9.5 4.5, plan horizons up to N = 147.
 """
 import os
 import sys
@@ -17,9 +20,13 @@ from obca_b200 import scenarios                             # noqa: E402
 from obca_b200.planner import a_star_3d                     # noqa: E402
 
 
-def main():
+def main(argv):
     sc = scenarios.quadcopter_scenario()
-    x0, xF, R = sc["x0"], sc["xF"], sc["R"]
+    x0, xF, R = sc["x0"].copy(), sc["xF"].copy(), sc["R"]
+    if argv:
+        if len(argv) != 4:
+            print(__doc__); return 2
+        x0[1], x0[2], xF[1], xF[2] = (float(a) for a in argv)
     t0 = time.time()
     w = a_star_3d.plan_quadcopter_warm_start(x0, xF, sc["Ts80"])
     if w is None:
@@ -40,4 +47,4 @@ def main():
 
 
 if __name__ == "__main__":
-    sys.exit(main())
+    sys.exit(main(sys.argv[1:]))

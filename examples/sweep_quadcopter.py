@@ -2,7 +2,8 @@
 then solved) as a batch: plan K config-4 pairs on host processes (obca_b200.planner.a_star_3d, 8-11 s per pair), solve all planned
 pairs -- each with the horizon N = path length - 1 and the sampling time Ts = round(0.25 * 80 / N, 2) the planner gave it -- in ONE
 GPU call (obca_quadcopter_solve_mixed), run the reference's constrSatisfaction on every result in one more call.  Pairs whose
-horizon exceeds the solver's limit (N + 1 <= 128) are counted and listed as skipped.
+horizon exceeds the solver's limit (N + 1 <= 512; the planner gives N = 80..147 over the config-4 box) are counted and listed
+as skipped.
 
 usage: python examples/sweep_quadcopter.py [K] [seed] [workers]           (needs a CUDA device for the solves)
 """
@@ -20,7 +21,7 @@ import obca_b200                                                   # noqa: E402
 from obca_b200 import quadcopter, scenarios                        # noqa: E402
 from obca_b200.planner.a_star_3d import plan_quadcopter_warm_start  # noqa: E402
 
-N_LIMIT = 127      # the quadcopter solver's longest horizon (N + 1 <= 128 stages, one CTA of at most four warps)
+N_LIMIT = 511      # the quadcopter solver's longest horizon (N + 1 <= 512 stages, at most four per thread of a 128-thread CTA)
 
 
 def sweep(K=32, seed=2, signed_dist=1, workers=None):

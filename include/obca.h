@@ -147,7 +147,8 @@ int obca_check_parking_mixed(int B, const int* Nb, int Nmax, int nOb, const int*
  * outputs: xp 12x(N+1), up 4xN, ts (N+1), lp 30x(N+1) (= [l1;l2;l3;l4;l5], :296), slack 5x(N+1) (SD only, may be
  *          NULL), exitflag 1 / 0 / 2 (2 = converged but sum(slack) > 1e-3, :283-288), iters, kkt_err, solve_seconds.
  * A single solve attempt, like the reference (flag = 1, :227-235).  opts == NULL: defaults with max_iter = 3000
- * (the reference leaves Ipopt's default). */
+ * (the reference leaves Ipopt's default).  Horizons 2 <= N <= 511 (N + 1 <= 512 stages); N > 511: OBCA_ERR_UNSUPPORTED
+ * (the bound is in obca_last_error()), returned before any device work, no output touched. */
 int obca_quadcopter_solve_batch(int B, int N, const double* x0, const double* xF, double Ts, double R, const double* ob,
                                 const double* xWS, double timeWS, int signed_dist, const obca_opts* opts, double* xp,
                                 double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters,
@@ -169,7 +170,8 @@ int obca_check_quadcopter(int B, int N, const double* x, const double* u, const 
  * (outputs over its own horizon, exitflag including the slack gate value 2, iters, kkt_err) are bit-identical to solving
  * it with obca_quadcopter_solve_batch at N = Nb[b], Ts = Tsb[b] and the same options.  Nb or Tsb NULL, an Nb[b] outside
  * [2, Nmax] or a Tsb[b] that is not a finite number > 0: OBCA_ERR_ARG (the index is in obca_last_error()), no output
- * touched.  Nmax + 1 > 128 is answered like obca_quadcopter_solve_batch at N = Nmax. */
+ * touched.  Nmax <= 511 (N + 1 <= 512 stages), as for obca_quadcopter_solve_batch; Nmax > 511: OBCA_ERR_UNSUPPORTED
+ * (the bound is in obca_last_error()), whatever the problems' own horizons, no output touched. */
 int obca_quadcopter_solve_mixed(int B, const int* Nb, int Nmax, const double* x0, const double* xF, const double* Tsb,
                                 double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
                                 const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,

@@ -157,14 +157,14 @@ struct QBatchPtrs {
 #define OBCA_MINB_Q 2
 #endif
 template <bool SDV>
-__global__ void __launch_bounds__(128, OBCA_MINB_Q)
+__global__ void __launch_bounds__(QUAD_CTA, OBCA_MINB_Q)
 k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmOpts O, const QLay L, const QBatchPtrs bp,
              double* __restrict__ Wall, int* __restrict__ counter) {
   extern __shared__ double s_kkt[];      // QuadSolver::smem_doubles(N): block-cooperative KKT sweep
   __shared__ ProbState S;
-  __shared__ double s_red[4 * 12];
+  __shared__ double s_red[(QUAD_CTA / 32) * 12];      // one partial per warp (launched with at most QUAD_CTA threads)
   __shared__ int s_b;
-  __shared__ double s_sum[4];
+  __shared__ double s_sum[QUAD_CTA / 32];
   const int N = P.N, NS = N + 1;      // the layout: strides of the per-problem arrays
   double* W = Wall + (size_t)blockIdx.x * L.total * L.NSP;
   for (;;) {
@@ -193,7 +193,7 @@ k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmO
     __syncthreads();
     if (threadIdx.x == 0) {
       double tot = 0.0;
-      for (int w = 0; w < ((Np + 32) >> 5); ++w) tot += s_sum[w];      // the problem's own warps (see block_reduce)
+      for (int w = 0; w < QuadSolver<SDV>::own_warps(C); ++w) tot += s_sum[w];      // the problem's own warps (see reduce)
       int ef = S.status == 1 ? 1 : 0;
       if (SDV && ef == 1 && tot > 1e-3) ef = 2;      // sum-slack gate, QuadcopterSignedDist.jl:283-288
       bp.exitflag[b] = ef; bp.iters[b] = S.iters; bp.kkt_err[b] = S.e0;
@@ -557,12 +557,13 @@ static int launch_eval(DevCtx& c, const ParkProblem& P, int B, const EvalIn& in,
 template <bool SDV>
 static int launch_quad(DevCtx& c, const QuadProblem& P, const IpmOpts& O, const QBatchPtrs& bp) {
   QLay L = make_qlayout(P);
-  if (L.NSP > 128) { set_err("horizon too long for this build (N+1 <= 128)"); return OBCA_ERR_UNSUPPORTED; }
+  // the workspace rows keep the stride NSP = round32(N+1); past QUAD_CTA stages a thread handles several of them
+  const int threads = L.NSP < QUAD_CTA ? L.NSP : QUAD_CTA;
   const size_t smem = (size_t)QuadSolver<SDV>::smem_doubles(P.N) * sizeof(double);
   if (smem > 200 * 1024) { set_err("horizon too long for the quadcopter kernel's shared memory"); return OBCA_ERR_UNSUPPORTED; }
   CK(cudaFuncSetAttribute(k_quad_solve<SDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = 0;
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_quad_solve<SDV>, L.NSP, smem));
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_quad_solve<SDV>, threads, smem));
   if (occ < 1) occ = 1;
   int grid = c.sms * occ;
   if (grid > bp.B) grid = bp.B;
@@ -573,7 +574,7 @@ static int launch_quad(DevCtx& c, const QuadProblem& P, const IpmOpts& O, const 
   CK(cudaMemcpyToSymbolAsync(c_qP, &P, sizeof(P), 0, cudaMemcpyHostToDevice, c.st));
   CK(cudaMemcpyToSymbolAsync(c_qL, &L, sizeof(L), 0, cudaMemcpyHostToDevice, c.st));
   CK(cudaMemsetAsync(c.counter, 0, sizeof(int), c.st));
-  k_quad_solve<SDV><<<grid, L.NSP, smem, c.st>>>(P, O, L, bp, c.W, c.counter);
+  k_quad_solve<SDV><<<grid, threads, smem, c.st>>>(P, O, L, bp, c.W, c.counter);
   CK(cudaGetLastError());
   return 0;
 }
@@ -746,6 +747,11 @@ static int quad_solve_host(int B, int N, const int* Nb, const double* Tsb, const
                            int* exitflag, int* iters, double* kkt_err, double* solve_seconds) {
   QuadProblem P;
   if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  if (N > QUAD_NMAX) {      // before any device work: nothing is launched and no output is written
+    set_err("horizon too long for the quadcopter solver: N = " + std::to_string(N) + " > " + std::to_string(QUAD_NMAX) +
+            " (N + 1 <= " + std::to_string(QUAD_NMAX + 1) + " stages)");
+    return OBCA_ERR_UNSUPPORTED;
+  }
   DevCtx* c;
   int rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;

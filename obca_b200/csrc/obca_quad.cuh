@@ -24,6 +24,10 @@ constexpr int QNP = QNSV * (QNSV + 1) / 2;     // 153
 constexpr double QUAD_REG3 = 1e-4;              // :55
 constexpr double QUAD_WH = 4.479906037125444;   // sqrt(mass*g/(4 k_F)) = sqrt(0.5*9.81/(0.0611*4)), :62
 constexpr int QNOB = 5;
+// The solver kernel runs a problem in a CTA of min(round32(N+1), QUAD_CTA) threads; thread t handles the stages t, t + QUAD_CTA,
+// ...  The horizon is bounded so that a thread handles at most four stages (N + 1 <= 512).
+constexpr int QUAD_CTA = 128;
+constexpr int QUAD_NMAX = 4 * QUAD_CTA - 1;
 
 struct QuadProblem {
   int N;          // the horizon the batch's arrays and the workspace are laid out for (the largest of a mixed batch)
@@ -135,10 +139,12 @@ struct QuadSolver {
 
   OBCA_HD static int n_stages(const QCtx& C) { return QCTX_N(C) + 1; }
 #if defined(__CUDA_ARCH__)
-  // block reductions over the problem's own ceil((N+1)/32) warps, so that a problem gives the same bits in a CTA sized for a
-  // longer horizon of its batch as in one sized for its own
+  // warps that hold stages of the problem: ceil((N+1)/32), at most the CTA's (past QUAD_CTA stages every warp has some)
+  __device__ static int own_warps(const QCtx& C) { return min((QCTX_N(C) + 32) >> 5, (int)(blockDim.x >> 5)); }
+  // block reductions over the problem's own warps, so that a problem gives the same bits in a CTA sized for a longer horizon
+  // of its batch as in one sized for its own
   template <typename T>
-  __device__ static void reduce(T& v, const QCtx& C) { block_reduce_warps(v, C.red_scratch, (QCTX_N(C) + 32) >> 5); }
+  __device__ static void reduce(T& v, const QCtx& C) { block_reduce_warps(v, C.red_scratch, own_warps(C)); }
 #endif
   OBCA_HD static bool fixed_time(const QCtx&) { return false; }
   OBCA_HD static void mult_counts(const QCtx& C, double& n_mult, double& n_bmult) {

@@ -14,7 +14,8 @@ same bits for every problem.  --dump-outputs DIR: the outputs of the last single
 
 --workload quadcopter: the same comparison for config 4 (obca_quadcopter_solve_mixed against one obca_quadcopter_solve_batch call
 per horizon): B = 2048 (--batch) SignedDist problems of scenarios.quadcopter_mixed_batch(B, (90, 127), seed=0), a horizon and its
-sampling time Ts = round(0.25 * 80 / N, 2) per problem (defaults --nmin 90 --nmax 127).  `value` counts exitflag == 1."""
+sampling time Ts = round(0.25 * 80 / N, 2) per problem (defaults --nmin 90 --nmax 127; the solver takes horizons up to
+N = 511, e.g. --nmin 128 --nmax 160 for a batch of long horizons only).  `value` counts exitflag == 1."""
 from __future__ import annotations
 
 import argparse
@@ -37,7 +38,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--nmin", type=int, default=None, help="default 40 (parking) / 90 (quadcopter)")
-    ap.add_argument("--nmax", type=int, default=None, help="default 80 (parking) / 127 (quadcopter)")
+    ap.add_argument("--nmax", type=int, default=None, help="default 80 (parking) / 127 (quadcopter); at most 127 (parking) / 511 (quadcopter)")
     ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     if args.steps < 1:
