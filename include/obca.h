@@ -183,6 +183,35 @@ int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x,
                                 const double* x0, const double* xF, const double* Tsb, const double* lambda,
                                 const double* ob, double R, const obca_opts* opts, int* feasible, double* worst);
 
+/* Hybrid A* warm starts on the GPU: B start poses x0 (3 x B column-major: x, y, yaw) towards one goal xF (x, y, yaw) among the obstacle
+ * points (ox[i], oy[i]), i < n_ob, in ONE call -- main.jl:215-248 for each pose, as obca_plan_warmstart_batch of include/obca_planner.h
+ * does on host threads, with the same search decisions (the same heuristic map, priorities, insertion order and expansion budget) and
+ * the same outputs up to the last bits of sin / cos / atan2 / acos / tan / atan.  One CTA plans one pose at a time (k_plan).
+ *   Ts: the sampling time (> 0) of the warm start; L: wheelbase of the steering extraction; sampleN: down-sampling of the 0.1 m path.
+ *   max_expansions <= 0: 200000 (obca_plan_warmstart's budget).
+ *   max_nodes: node pool per resident CTA; <= 0 selects 32768 (the demo sweeps insert at most ~4500 nodes per plan).  Device scratch per
+ *     resident CTA (4 per SM): max_nodes x 176 bytes + a 4-byte cell table over the search grid (~1 MB for the demo clouds)
+ *     + ~0.2 MB of course buffers + 96 x cap x sampleN bytes; about 7.1 MB at the defaults, cap = 512, sampleN = 3.
+ *     Device memory of one call: min(B, 4 x SMs) x that scratch -- about 3.7 GB on a 132-SM H100 for B >= 528 at the defaults --
+ *     plus the batch's outputs, 72 x B x cap bytes (151 MB at B = 4096, cap = 512), which are copied to the device first (so that
+ *     the entries the planner does not write keep the caller's values) and back after the kernel.  All of it is freed before the
+ *     call returns.
+ * Outputs, with the stride cap, in the layout of obca_plan_warmstart_batch: rx / ry / ryaw [i*cap ..] (N[i]+1 values), xWS [i*4*cap ..]
+ * as (N[i]+1) x 4, uWS [i*2*cap ..] as N[i] x 2 column-major.  Nothing past a problem's own N[i]+1 stages is written.
+ * status[i]: OBCA_PLAN_OK (0), OBCA_PLAN_NO_PATH (1), OBCA_PLAN_CAPACITY (2; N[i] holds the horizon, nothing else written), or
+ * OBCA_PLAN_POOL_FULL (4): the search outgrew its device scratch and was stopped: it needed more than max_nodes nodes, or -- only for
+ * a start pose hundreds of metres from the goal -- an analytic expansion longer than the kernel's 4096-point course buffer (409.6 m).
+ * That pose is NOT planned (nothing else written, never a partial path); the host planner can plan it (obca_b200.planner.device.plan_batch
+ * does so).
+ * expansions[i] (may be NULL): nodes expanded.  plan_seconds (may be NULL): device time of the search kernel.
+ * Return: 0, OBCA_ERR_ARG (B < 0, a null array, n_ob <= 0, Ts <= 0, sampleN < 1, cap < 2; reason in obca_last_error()),
+ * OBCA_ERR_NO_DEVICE, OBCA_ERR_CUDA. */
+#define OBCA_PLAN_POOL_FULL 4
+int obca_plan_parking_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob,
+                                      double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap,
+                                      const obca_opts* opts, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
+                                      int* N, int* status, int* expansions, double* plan_seconds);
+
 /* Device times of the last obca_parking_solve_batch[_dev] / obca_parking_solve_mixed on `device`: DualMultWS (0 when the caller passed lWS / nWS) and the
  * solve alone (= what solve_seconds reports; the reference's `time`, ParkingSignedDist.jl:297). */
 int obca_last_times(int device, double* dualws_seconds, double* solve_seconds);

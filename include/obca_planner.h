@@ -6,6 +6,8 @@
  *   the warm-start extraction               main.jl:215-248
  * Same algorithms as the Python restatement obca_b200/planner/ (which documents the reference line by line); the two are tested to
  * produce the same paths (tests/test_planner_native.py).  The reference's planner is host code as well and runs once per problem.
+ * GPU twin: obca_plan_parking_warmstart_batch in include/obca.h (libobca.so) plans a batch of start poses in one call with the same search
+ * decisions; both libraries compile the algorithm from one source, obca_b200/planner/csrc/obca_plan_core.h.
  *
  * All arrays are Float64, owned by the caller, column-major where two-dimensional (Julia layout).
  */

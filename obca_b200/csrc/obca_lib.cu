@@ -236,7 +236,9 @@ __global__ void k_quad_check(const __grid_constant__ QuadProblem P, int B, const
 // ---------------------------------------------------------------------------------------------------------
 static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
-#define CK(call)                                                                                     \
+// the GPU planner's translation unit (obca_plan.cu, built without FMA contraction) reports through obca_last_error() as well
+void obca_set_last_error(const std::string& s) { g_err = s; }
+#define CK(call)                                                                                   \
   do {                                                                                               \
     cudaError_t e_ = (call);                                                                         \
     if (e_ != cudaSuccess) {                                                                         \

@@ -1,415 +1,75 @@
 // obca_planner.cpp -- host-side warm-start producer behind include/obca_planner.h (plain C++17, no CUDA): Hybrid A* with the
 // Reeds-Shepp analytic expansion, the vehicle / obstacle-point collision test, the grid heuristic, veloSmooth and the warm-start
-// extraction of main.jl:215-248.  Same algorithms, in the same order of floating-point operations, as the Python restatement
-// obca_b200/planner/*.py (which cites the reference line by line and documents its quirks); tests/test_planner_native.py compares
-// the two.  Build: g++ -O2 -std=c++17 -ffp-contract=off -shared -fPIC (see __graft_entry__.build()).
+// extraction of main.jl:215-248.  The algorithm's pieces live in obca_plan_core.h, which the GPU planner of libobca.so
+// (obca_b200/csrc/obca_plan.cu) compiles as well; this file holds the host search (hash maps and a priority queue) and the C entries.
+// Same algorithms, in the same order of floating-point operations, as the Python restatement obca_b200/planner/*.py (which cites the
+// reference line by line and documents its quirks); tests/test_planner_native.py compares the two.
+// Build: g++ -O2 -std=c++17 -ffp-contract=off -shared -fPIC (see __graft_entry__.build()).
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
-#include <functional>
 #include <limits>
 #include <queue>
-#include <atomic>
-#include <string>
 #include <thread>
 #include <tuple>
 #include <unordered_map>
-#include <unordered_set>
 #include <vector>
 
 #include "../../../include/obca_planner.h"
+#include "obca_plan_core.h"
 
 namespace {
 
 using std::vector;
-const double PI = 3.141592653589793;
+using namespace obca_plan;
 const double INF = std::numeric_limits<double>::infinity();
-
-// ---- constants of the reference (hybrid_a_star.jl:42-67, collision_check.jl:31-35, reeds_shepp.jl:35) ----
-const double VEHICLE_RADIUS = 1.0, YAW_GRID_RESOLUTION = 5.0 * PI / 180.0, N_STEER = 5.0, XY_GRID_RESOLUTION = 0.3, MOTION_RESOLUTION = 0.1;
-const double SB_COST = 10.0, BACK_COST = 0.0, STEER_CHANGE_COST = 10.0, STEER_COST = 0.0, H_COST = 1.0, WB = 2.7, MAX_STEER = 0.6;
-const double CAR_B = 1.0, CAR_C = 3.7, CAR_I = 2.0;
-const double WBUBBLE_DIST = (CAR_B + CAR_C) / 2.0 - CAR_B, WBUBBLE_R = (CAR_B + CAR_C) / 2.0;
-const double RS_STEP_SIZE = 0.1;
-
-long jround(double v) { return (long)std::floor(std::fabs(v) + 0.5) * (v >= 0 ? 1 : -1); }      // Julia round(Int64, x)
-double pi_2_pi(double a) {
-  while (a > PI) a -= 2.0 * PI;
-  while (a < -PI) a += 2.0 * PI;
-  return a;
-}
-double pymod(double x, double m) {      // Python float %: result has the sign of the divisor
-  double v = std::fmod(x, m);
-  if (v != 0.0 && ((v < 0.0) != (m < 0.0))) v += m;
-  return v;
-}
-double mod2pi(double x) {
-  double v = pymod(x, 2.0 * PI);
-  if (v < -PI) v += 2.0 * PI;
-  else if (v > PI) v -= 2.0 * PI;
-  return v;
-}
-void polar(double x, double y, double& r, double& th) { r = std::sqrt(x * x + y * y); th = std::atan2(y, x); }
 
 // =====================================================================================================================
 // Reeds-Shepp (obca_b200/planner/reeds_shepp.py)
 // =====================================================================================================================
-struct RsPath {
-  vector<double> lengths;
-  std::string ctypes;
-  double L = 0.0;
-  vector<double> x, y, yaw;
-  vector<int> directions;
-};
-struct Word { bool ok; double t, u, v; };
-const Word NONE{false, 0, 0, 0};
-
-Word LSL(double x, double y, double phi) {
-  double u, t; polar(x - std::sin(phi), y - 1.0 + std::cos(phi), u, t);
-  if (t >= 0.0) { double v = mod2pi(phi - t); if (v >= 0.0) return {true, t, u, v}; }
-  return NONE;
-}
-Word LSR(double x, double y, double phi) {
-  double u1, t1; polar(x + std::sin(phi), y - 1.0 - std::cos(phi), u1, t1);
-  u1 = u1 * u1;
-  if (u1 >= 4.0) {
-    double u = std::sqrt(u1 - 4.0), theta = std::atan2(2.0, u), t = mod2pi(t1 + theta), v = mod2pi(t - phi);
-    if (t >= 0.0 && v >= 0.0) return {true, t, u, v};
+RsSet generate_path(const double q0[3], const double q1[3], double maxc) {
+  double x, y, phi, xb, yb;
+  rs_frame(q0, q1, maxc, x, y, phi, xb, yb);
+  RsSet s;
+  s.n = 0;
+  for (int j = 0; j < RS_NCAND; ++j) {
+    RsCand c;
+    if (rs_candidate(j, x, y, phi, xb, yb, c)) set_path(s, c);
   }
-  return NONE;
+  return s;
 }
-Word LRL(double x, double y, double phi) {
-  double u1, t1; polar(x - std::sin(phi), y - 1.0 + std::cos(phi), u1, t1);
-  if (u1 <= 4.0) {
-    double u = -2.0 * std::asin(0.25 * u1), t = mod2pi(t1 + 0.5 * u + PI), v = mod2pi(phi - t + u);
-    if (t >= 0.0 && u <= 0.0) return {true, t, u, v};
-  }
-  return NONE;
-}
-Word SLS(double x, double y, double phi) {
-  phi = mod2pi(phi);
-  if (phi > 0.0 && phi < PI * 0.99 && y != 0.0) {
-    double xd = -y / std::tan(phi) + x, t = xd - std::tan(phi / 2.0), u = phi;
-    double r = std::sqrt((x - xd) * (x - xd) + y * y), v = (y > 0.0 ? r : -r) - std::tan(phi / 2.0);
-    return {true, t, u, v};
-  }
-  return NONE;
-}
-void tau_omega(double u, double v, double xi, double eta, double phi, double& tau, double& omega) {
-  double delta = mod2pi(u - v), A = std::sin(u) - std::sin(delta), B = std::cos(u) - std::cos(delta) - 1.0;
-  double t1 = std::atan2(eta * A - xi * B, xi * A + eta * B);
-  double t2 = 2.0 * (std::cos(delta) - std::cos(v) - std::cos(u)) + 3.0;
-  tau = t2 < 0 ? mod2pi(t1 + PI) : mod2pi(t1);
-  omega = mod2pi(tau - u + v - phi);
-}
-Word LRLRn(double x, double y, double phi) {
-  double xi = x + std::sin(phi), eta = y - 1.0 - std::cos(phi), rho = 0.25 * (2.0 + std::sqrt(xi * xi + eta * eta));
-  if (rho <= 1.0) {
-    double u = std::acos(rho), t, v; tau_omega(u, -u, xi, eta, phi, t, v);
-    if (t >= 0.0 && v <= 0.0) return {true, t, u, v};
-  }
-  return NONE;
-}
-Word LRLRp(double x, double y, double phi) {
-  double xi = x + std::sin(phi), eta = y - 1.0 - std::cos(phi), rho = (20.0 - xi * xi - eta * eta) / 16.0;
-  if (0.0 <= rho && rho <= 1.0) {
-    double u = -std::acos(rho);
-    if (u >= -0.5 * PI) { double t, v; tau_omega(u, u, xi, eta, phi, t, v); if (t >= 0.0 && v >= 0.0) return {true, t, u, v}; }
-  }
-  return NONE;
-}
-Word LRSR(double x, double y, double phi) {
-  double xi = x + std::sin(phi), eta = y - 1.0 - std::cos(phi), rho, theta; polar(-eta, xi, rho, theta);
-  if (rho >= 2.0) {
-    double t = theta, u = 2.0 - rho, v = mod2pi(t + 0.5 * PI - phi);
-    if (t >= 0.0 && u <= 0.0 && v <= 0.0) return {true, t, u, v};
-  }
-  return NONE;
-}
-Word LRSL(double x, double y, double phi) {
-  double xi = x - std::sin(phi), eta = y - 1.0 + std::cos(phi), rho, theta; polar(xi, eta, rho, theta);
-  if (rho >= 2.0) {
-    double r = std::sqrt(rho * rho - 4.0), u = 2.0 - r, t = mod2pi(theta + std::atan2(r, -2.0)), v = mod2pi(phi - 0.5 * PI - t);
-    if (t >= 0.0 && u <= 0.0 && v <= 0.0) return {true, t, u, v};
-  }
-  return NONE;
-}
-Word LRSLR(double x, double y, double phi) {
-  double xi = x + std::sin(phi), eta = y - 1.0 - std::cos(phi), rho, th; polar(xi, eta, rho, th);
-  if (rho >= 2.0) {
-    double u = 4.0 - std::sqrt(rho * rho - 4.0);
-    if (u <= 0.0) {
-      double t = mod2pi(std::atan2((4.0 - u) * xi - 2.0 * eta, -2.0 * xi + (u - 4.0) * eta)), v = mod2pi(t - phi);
-      if (t >= 0.0 && v >= 0.0) return {true, t, u, v};
-    }
-  }
-  return NONE;
-}
-const double HP = 0.5 * PI;
-
-// Python's built-in sum() of floats (CPython >= 3.12: Neumaier's compensated summation) -- the Python restatement uses it for the two
-// sums below, and the order of candidate words depends on their last bits
-struct PySum {
-  double f = 0.0, c = 0.0;
-  void add(double x) {
-    const double t = f + x;
-    if (std::fabs(f) >= std::fabs(x)) c += (f - t) + x;
-    else c += (x - t) + f;
-    f = t;
-  }
-  double value() const { return (c != 0.0 && std::isfinite(c)) ? f + c : f; }
-};
-void set_path(vector<RsPath>& paths, const vector<double>& lengths, const std::string& ctypes) {     // reeds_shepp.jl:207-230, quirk kept
-  for (const RsPath& tp : paths) {
-    if (tp.ctypes != ctypes) continue;
-    PySum s;
-    for (size_t i = 0; i < lengths.size(); ++i) s.add(tp.lengths[i] - lengths[i]);
-    if (s.value() <= 0.01) return;
-  }
-  PySum Ls;
-  for (double l : lengths) Ls.add(std::fabs(l));
-  const double L = Ls.value();
-  if (L < 0.01) return;
-  RsPath p; p.lengths = lengths; p.ctypes = ctypes; p.L = L;
-  paths.push_back(std::move(p));
-}
-typedef Word (*Solver)(double, double, double);
-typedef vector<double> (*Pattern)(double, double, double);
-vector<double> pat_tuv(double t, double u, double v) { return {t, u, v}; }
-vector<double> pat_ccsc(double t, double u, double v) { return {t, -HP, u, v}; }
-vector<double> pat_ccccn(double t, double u, double v) { return {t, u, -u, v}; }
-vector<double> pat_ccccp(double t, double u, double v) { return {t, u, u, v}; }
-vector<double> pat_ccscc(double t, double u, double v) { return {t, -HP, u, -HP, v}; }
-char swap_lr(char c) { return c == 'L' ? 'R' : (c == 'R' ? 'L' : 'S'); }
-
-void four_symmetries(vector<RsPath>& paths, Solver solver, const char* word, Pattern pattern, double x, double y, double phi, bool reverse) {
-  const double fx[4] = {x, -x, x, -x}, fy[4] = {y, y, -y, -y}, fp[4] = {phi, -phi, -phi, phi};
-  const bool flip[4] = {false, true, false, true}, reflect[4] = {false, false, true, true};
-  for (int k = 0; k < 4; ++k) {
-    Word w = solver(fx[k], fy[k], fp[k]);
-    if (!w.ok) continue;
-    vector<double> lengths = pattern(w.t, w.u, w.v);
-    std::string types(word);
-    if (reverse) { std::reverse(lengths.begin(), lengths.end()); std::reverse(types.begin(), types.end()); }
-    if (flip[k]) for (double& l : lengths) l = -l;
-    if (reflect[k]) for (char& c : types) c = swap_lr(c);
-    set_path(paths, lengths, types);
-  }
-}
-vector<RsPath> generate_path(const double q0[3], const double q1[3], double maxc) {
-  double dx = q1[0] - q0[0], dy = q1[1] - q0[1], dth = q1[2] - q0[2];
-  double c = std::cos(q0[2]), s = std::sin(q0[2]);
-  double x = (c * dx + s * dy) * maxc, y = (-s * dx + c * dy) * maxc, phi = dth;
-  vector<RsPath> paths;
-  Word w = SLS(x, y, phi);
-  if (w.ok) set_path(paths, {w.t, w.u, w.v}, "SLS");
-  w = SLS(x, -y, -phi);
-  if (w.ok) set_path(paths, {w.t, w.u, w.v}, "SRS");
-  double xb = x * std::cos(phi) + y * std::sin(phi), yb = x * std::sin(phi) - y * std::cos(phi);
-  four_symmetries(paths, LSL, "LSL", pat_tuv, x, y, phi, false);
-  four_symmetries(paths, LSR, "LSR", pat_tuv, x, y, phi, false);
-  four_symmetries(paths, LRL, "LRL", pat_tuv, x, y, phi, false);
-  four_symmetries(paths, LRL, "LRL", pat_tuv, xb, yb, phi, true);
-  four_symmetries(paths, LRLRn, "LRLR", pat_ccccn, x, y, phi, false);
-  four_symmetries(paths, LRLRp, "LRLR", pat_ccccp, x, y, phi, false);
-  four_symmetries(paths, LRSL, "LRSL", pat_ccsc, x, y, phi, false);
-  four_symmetries(paths, LRSR, "LRSR", pat_ccsc, x, y, phi, false);
-  four_symmetries(paths, LRSL, "LRSL", pat_ccsc, xb, yb, phi, true);
-  four_symmetries(paths, LRSR, "LRSR", pat_ccsc, xb, yb, phi, true);
-  four_symmetries(paths, LRSLR, "LRSLR", pat_ccscc, x, y, phi, false);
-  return paths;
-}
-void interpolate(int ind, double l, char m, double maxc, double ox, double oy, double oyaw, vector<double>& px, vector<double>& py,
-                 vector<double>& pyaw, vector<int>& directions) {
-  if (m == 'S') {
-    px[ind] = ox + l / maxc * std::cos(oyaw);
-    py[ind] = oy + l / maxc * std::sin(oyaw);
-    pyaw[ind] = oyaw;
-  } else {
-    double ldx = std::sin(l) / maxc, ldy = (1.0 - std::cos(l)) / (m == 'L' ? maxc : -maxc);
-    double gdx = std::cos(-oyaw) * ldx + std::sin(-oyaw) * ldy, gdy = -std::sin(-oyaw) * ldx + std::cos(-oyaw) * ldy;
-    px[ind] = ox + gdx;
-    py[ind] = oy + gdy;
-    pyaw[ind] = m == 'L' ? oyaw + l : oyaw - l;
-  }
-  directions[ind] = l > 0.0 ? 1 : -1;
-}
-void generate_local_course(double L, const vector<double>& lengths, const std::string& mode, double maxc, double step_size, vector<double>& px,
-                           vector<double>& py, vector<double>& pyaw, vector<int>& directions) {
-  const int npoint = (int)(L / step_size) + 2 * (int)lengths.size() + 8;
-  px.assign(npoint, 0.0); py.assign(npoint, 0.0); pyaw.assign(npoint, 0.0); directions.assign(npoint, 0);
-  int ind = 1;
-  directions[0] = lengths[0] > 0.0 ? 1 : -1;
-  double d = lengths[0] > 0.0 ? step_size : -step_size, pd = d, ll = 0.0;
-  for (size_t i = 0; i < lengths.size(); ++i) {
-    const char m = mode[i];
-    const double l = lengths[i];
-    d = l > 0.0 ? step_size : -step_size;
-    const double ox = px[ind], oy = py[ind], oyaw = pyaw[ind];
-    ind -= 1;
-    if (i >= 1 && lengths[i - 1] * lengths[i] > 0) pd = -d - ll;
-    else pd = d - ll;
-    while (std::fabs(pd) <= std::fabs(l)) {
-      ind += 1;
-      interpolate(ind, pd, m, maxc, ox, oy, oyaw, px, py, pyaw, directions);
-      pd += d;
-    }
-    ll = l - pd - d;
-    ind += 1;
-    interpolate(ind, l, m, maxc, ox, oy, oyaw, px, py, pyaw, directions);
-  }
-  while (!px.empty() && px.back() == 0.0) { px.pop_back(); py.pop_back(); pyaw.pop_back(); directions.pop_back(); }
-}
-vector<RsPath> calc_paths(double sx, double sy, double syaw, double gx, double gy, double gyaw, double maxc, double step_size) {
+// calc_shortest_path (reeds_shepp.jl:59-76): the shortest candidate's course in global coordinates, its lengths scaled by 1/maxc.
+// Only the shortest candidate is interpolated: the pick depends on the lengths alone.
+bool calc_shortest_path(double sx, double sy, double syaw, double gx, double gy, double gyaw, double maxc, double step_size, RsCand& best,
+                        vector<double>& px, vector<double>& py, vector<double>& pyaw) {
   const double q0[3] = {sx, sy, syaw}, q1[3] = {gx, gy, gyaw};
-  vector<RsPath> paths = generate_path(q0, q1, maxc);
-  const double c = std::cos(-q0[2]), s = std::sin(-q0[2]);
-  for (RsPath& p : paths) {
-    vector<double> x, y, yaw;
-    generate_local_course(p.L, p.lengths, p.ctypes, maxc, step_size * maxc, x, y, yaw, p.directions);
-    p.x.resize(x.size()); p.y.resize(x.size()); p.yaw.resize(x.size());
-    for (size_t i = 0; i < x.size(); ++i) {
-      p.x[i] = c * x[i] + s * y[i] + q0[0];
-      p.y[i] = -s * x[i] + c * y[i] + q0[1];
-      p.yaw[i] = pi_2_pi(yaw[i] + q0[2]);
-    }
-    for (double& l : p.lengths) l = l / maxc;
-    p.L = p.L / maxc;
-  }
-  return paths;
-}
-bool calc_shortest_path(double sx, double sy, double syaw, double gx, double gy, double gyaw, double maxc, double step_size, RsPath& best) {
-  vector<RsPath> paths = calc_paths(sx, sy, syaw, gx, gy, gyaw, maxc, step_size);
-  double minL = INF;
-  int bi = -1;
-  for (size_t i = 0; i < paths.size(); ++i)
-    if (paths[i].L <= minL) { minL = paths[i].L; bi = (int)i; }      // the last of equally short candidates wins (reeds_shepp.jl:67-72)
+  const RsSet s = generate_path(q0, q1, maxc);
+  const int bi = rs_shortest(s, maxc);
   if (bi < 0) return false;
-  best = std::move(paths[bi]);
+  best = s.p[bi];
+  const double step = step_size * maxc;
+  const int npoint = rs_npoint(s.L[bi], best.n, step);
+  vector<int> seg(npoint);
+  vector<double> par(npoint);
+  int n = rs_course_plan(best, step, npoint, seg.data(), par.data());
+  double org[RS_MAX_SEG][3];
+  rs_origins(best, maxc, org);
+  vector<double> lx(n), ly(n), lyaw(n);
+  for (int i = 0; i < n; ++i) rs_point(best, maxc, org, seg[i], par[i], lx[i], ly[i], lyaw[i]);
+  while (n > 0 && lx[n - 1] == 0.0) --n;
+  const double cq = std::cos(-q0[2]), sq = std::sin(-q0[2]);
+  px.resize(n); py.resize(n); pyaw.resize(n);
+  for (int i = 0; i < n; ++i) rs_to_global(q0, cq, sq, lx[i], ly[i], lyaw[i], px[i], py[i], pyaw[i]);
+  for (int i = 0; i < best.n; ++i) best.len[i] = best.len[i] / maxc;
   return true;
 }
 
-// =====================================================================================================================
-// collision test (obca_b200/planner/collision.py)
-// =====================================================================================================================
-const double VRX[5] = {CAR_C, CAR_C, -CAR_B, -CAR_B, CAR_C};
-const double VRY[5] = {-CAR_I / 2.0, CAR_I / 2.0, CAR_I / 2.0, -CAR_I / 2.0, -CAR_I / 2.0};
-
-struct Obstacles {
-  vector<double> ox, oy;
-  // uniform grid over the points (cell = bubble radius): the bubble query looks at 3 x 3 cells instead of all points
-  double x0 = 0, y0 = 0, cell = WBUBBLE_R;
-  int nx = 0, ny = 0;
-  vector<vector<int> > cells;
-  void build() {
-    if (ox.empty()) return;
-    x0 = *std::min_element(ox.begin(), ox.end()); y0 = *std::min_element(oy.begin(), oy.end());
-    const double x1 = *std::max_element(ox.begin(), ox.end()), y1 = *std::max_element(oy.begin(), oy.end());
-    nx = (int)std::floor((x1 - x0) / cell) + 1; ny = (int)std::floor((y1 - y0) / cell) + 1;
-    cells.assign((size_t)nx * ny, {});
-    for (size_t i = 0; i < ox.size(); ++i) cells[(size_t)cell_of(oy[i], y0, ny) * nx + cell_of(ox[i], x0, nx)].push_back((int)i);
-    for (auto& c : cells) std::sort(c.begin(), c.end());
-  }
-  int cell_of(double v, double v0, int n) const { int c = (int)std::floor((v - v0) / cell); return c < 0 ? 0 : (c >= n ? n - 1 : c); }
-};
-bool point_in_car(double ix, double iy, double iyaw, double px, double py) {      // collision_check.jl:58-98 for one point
-  const double c = std::cos(-iyaw), s = std::sin(-iyaw);
-  const double tx = px - ix, ty = py - iy;
-  const double lx = c * tx - s * ty, ly = s * tx + c * ty;
-  double sumangle = 0.0;
-  for (int e = 0; e < 4; ++e) {
-    const double x1 = VRX[e] - lx, y1 = VRY[e] - ly, x2 = VRX[e + 1] - lx, y2 = VRY[e + 1] - ly;
-    const double d1 = std::sqrt(x1 * x1 + y1 * y1), d2 = std::sqrt(x2 * x2 + y2 * y2);
-    const double th1 = std::atan2(y1, x1);
-    const double tty = -std::sin(th1) * x2 + std::cos(th1) * y2;
-    double tmp = (x1 * x2 + y1 * y2) / (d1 * d2);
-    if (!(tmp <= 1.0) && tmp == tmp) tmp = 1.0;      // min(tmp, 1) that keeps NaN
-    const double ang = std::acos(tmp);
-    sumangle += tty >= 0.0 ? ang : -ang;
-  }
-  return sumangle >= PI;
-}
-bool check_collision(const vector<double>& x, const vector<double>& y, const vector<double>& yaw, const Obstacles& ob) {      // true = free
-  for (size_t k = 0; k < x.size(); ++k) {
-    const double cx = x[k] + WBUBBLE_DIST * std::cos(yaw[k]), cy = y[k] + WBUBBLE_DIST * std::sin(yaw[k]);
-    if (ob.nx == 0) continue;
-    const int ci = (int)std::floor((cx - ob.x0) / ob.cell), cj = (int)std::floor((cy - ob.y0) / ob.cell);
-    for (int j = cj - 1; j <= cj + 1; ++j) {
-      if (j < 0 || j >= ob.ny) continue;
-      for (int i = ci - 1; i <= ci + 1; ++i) {
-        if (i < 0 || i >= ob.nx) continue;
-        for (int id : ob.cells[(size_t)j * ob.nx + i]) {
-          const double dx = ob.ox[id] - cx, dy = ob.oy[id] - cy;
-          if (std::sqrt(dx * dx + dy * dy) <= WBUBBLE_R && point_in_car(x[k], y[k], yaw[k], ob.ox[id], ob.oy[id])) return false;
-        }
-      }
-    }
-  }
+bool check_collision(const vector<double>& x, const vector<double>& y, const vector<double>& yaw, const ObGridView& g) {      // true = free
+  for (size_t k = 0; k < x.size(); ++k)
+    if (pose_collides(g, x[k], y[k], yaw[k])) return false;
   return true;
-}
-
-// =====================================================================================================================
-// grid heuristic (obca_b200/planner/grid_policy.py): exact 8-connected shortest distances from the goal
-// =====================================================================================================================
-struct DistPolicy {
-  vector<double> pmap;      // [xw][yw], INF where unreachable; entry (i-1, j-1) <-> cell (i + minx, j + miny)
-  long minx = 0, miny = 0;
-  int xw = 0, yw = 0;
-};
-DistPolicy calc_dist_policy(double gx, double gy, const vector<double>& ox, const vector<double>& oy, double reso, double vr) {
-  DistPolicy P;
-  vector<double> oxs(ox.size()), oys(oy.size());
-  for (size_t i = 0; i < ox.size(); ++i) { oxs[i] = ox[i] / reso; oys[i] = oy[i] / reso; }
-  const long minx = jround(*std::min_element(oxs.begin(), oxs.end())), miny = jround(*std::min_element(oys.begin(), oys.end()));
-  const long maxx = jround(*std::max_element(oxs.begin(), oxs.end())), maxy = jround(*std::max_element(oys.begin(), oys.end()));
-  const int xw = (int)(maxx - minx), yw = (int)(maxy - miny);
-  P.minx = minx; P.miny = miny; P.xw = xw; P.yw = yw;
-  vector<char> obmap((size_t)xw * yw, 0);
-  const double lim = vr / reso;
-  for (int ix = 1; ix <= xw; ++ix)
-    for (int iy = 1; iy <= yw; ++iy) {
-      const double cx = (double)(ix + minx), cy = (double)(iy + miny);
-      double best = INF;
-      for (size_t k = 0; k < oxs.size(); ++k) {
-        const double dx = oxs[k] - cx, dy = oys[k] - cy, d2 = dx * dx + dy * dy;
-        if (d2 < best) best = d2;
-      }
-      obmap[(size_t)(ix - 1) * yw + (iy - 1)] = std::sqrt(best) <= lim;
-    }
-  P.pmap.assign((size_t)xw * yw, INF);
-  const long g0 = jround(gx / reso), g1 = jround(gy / reso);
-  auto ok = [&](long x, long y) {
-    const long ix = x - minx, iy = y - miny;
-    return 0 < ix && ix < xw && 0 < iy && iy < yw && !obmap[(size_t)(ix - 1) * yw + (iy - 1)];
-  };
-  typedef std::tuple<double, long, long> Item;
-  std::priority_queue<Item, vector<Item>, std::greater<Item> > heap;
-  auto key = [](long x, long y) { return ((uint64_t)(uint32_t)(int32_t)x << 32) | (uint32_t)(int32_t)y; };
-  std::unordered_map<uint64_t, double> best;
-  std::unordered_set<uint64_t> done;
-  heap.push(Item(0.0, g0, g1));
-  best[key(g0, g1)] = 0.0;
-  const int MX[8] = {1, 0, -1, 0, -1, -1, 1, 1}, MY[8] = {0, 1, 0, -1, -1, 1, -1, 1};
-  const double s2 = std::sqrt(2.0);
-  const double MC[8] = {1.0, 1.0, 1.0, 1.0, s2, s2, s2, s2};
-  while (!heap.empty()) {
-    const Item it = heap.top(); heap.pop();
-    const double c = std::get<0>(it);
-    const long x = std::get<1>(it), y = std::get<2>(it);
-    if (done.count(key(x, y))) continue;
-    done.insert(key(x, y));
-    const long ix = x - minx, iy = y - miny;
-    if (1 <= ix && ix <= xw && 1 <= iy && iy <= yw) P.pmap[(size_t)(ix - 1) * yw + (iy - 1)] = c;
-    for (int m = 0; m < 8; ++m) {
-      const long nx = x + MX[m], ny = y + MY[m];
-      if (done.count(key(nx, ny)) || !ok(nx, ny)) continue;
-      const double nc = c + MC[m];
-      auto f = best.find(key(nx, ny));
-      if (f == best.end() || nc < f->second) { best[key(nx, ny)] = nc; heap.push(Item(nc, nx, ny)); }
-    }
-  }
-  return P;
 }
 
 // =====================================================================================================================
@@ -422,82 +82,27 @@ struct Node {
   double steer, cost;
   long pind;
 };
-struct Config { long minx, miny, minyaw, maxx, maxy, maxyaw, xw, yw, yaww; double xyreso, yawreso; };
-Config calc_config(const vector<double>& ox, const vector<double>& oy, double xyreso, double yawreso) {
-  Config c;
-  c.minx = jround(*std::min_element(ox.begin(), ox.end()) / xyreso); c.miny = jround(*std::min_element(oy.begin(), oy.end()) / xyreso);
-  c.maxx = jround(*std::max_element(ox.begin(), ox.end()) / xyreso); c.maxy = jround(*std::max_element(oy.begin(), oy.end()) / xyreso);
-  c.minyaw = jround(-PI / yawreso) - 1; c.maxyaw = jround(PI / yawreso);
-  c.xw = c.maxx - c.minx; c.yw = c.maxy - c.miny; c.yaww = c.maxyaw - c.minyaw; c.xyreso = xyreso; c.yawreso = yawreso;
-  return c;
-}
-long calc_index(const Node& n, const Config& c) { return (n.yawind - c.minyaw) * c.xw * c.yw + (n.yind - c.miny) * c.xw + (n.xind - c.minx); }
-Node calc_next_node(const Node& cur, long c_id, double u, double d, const Config& c) {
-  const double arc_l = XY_GRID_RESOLUTION;
-  const int nlist = (int)jround(arc_l / MOTION_RESOLUTION) + 1;
-  Node n;
-  n.x.assign(nlist, 0.0); n.y.assign(nlist, 0.0); n.yaw.assign(nlist, 0.0);
-  n.x[0] = cur.x.back() + d * MOTION_RESOLUTION * std::cos(cur.yaw.back());
-  n.y[0] = cur.y.back() + d * MOTION_RESOLUTION * std::sin(cur.yaw.back());
-  n.yaw[0] = pi_2_pi(cur.yaw.back() + d * MOTION_RESOLUTION / WB * std::tan(u));
-  for (int i = 0; i < nlist - 1; ++i) {
-    n.x[i + 1] = n.x[i] + d * MOTION_RESOLUTION * std::cos(n.yaw[i]);
-    n.y[i + 1] = n.y[i] + d * MOTION_RESOLUTION * std::sin(n.yaw[i]);
-    n.yaw[i + 1] = pi_2_pi(n.yaw[i] + d * MOTION_RESOLUTION / WB * std::tan(u));
-  }
-  const bool direction = d > 0;
-  double added = direction ? std::fabs(arc_l) : std::fabs(arc_l) * BACK_COST;
-  if (direction != cur.direction) added += SB_COST;
-  added += STEER_COST * std::fabs(u);
-  added += STEER_CHANGE_COST * std::fabs(cur.steer - u);
-  n.xind = jround(n.x.back() / c.xyreso); n.yind = jround(n.y.back() / c.xyreso); n.yawind = jround(n.yaw.back() / c.yawreso);
-  n.direction = direction; n.steer = u; n.cost = cur.cost + added; n.pind = c_id;
-  return n;
-}
-double calc_rs_path_cost(const RsPath& p) {
-  double cost = 0.0;
-  for (double l : p.lengths) cost += l >= 0 ? l : std::fabs(l) * BACK_COST;
-  for (size_t i = 0; i + 1 < p.lengths.size(); ++i)
-    if (p.lengths[i] * p.lengths[i + 1] < 0.0) cost += SB_COST;
-  for (char ct : p.ctypes)
-    if (ct != 'S') cost += STEER_COST * std::fabs(MAX_STEER);
-  vector<double> ul;
-  for (char ct : p.ctypes) ul.push_back(ct == 'R' ? -MAX_STEER : (ct == 'L' ? MAX_STEER : 0.0));
-  for (size_t i = 0; i + 1 < ul.size(); ++i) cost += STEER_CHANGE_COST * std::fabs(ul[i + 1] - ul[i]);
-  return cost;
-}
 int hybrid_astar(double sx, double sy, double syaw, double gx, double gy, double gyaw, const vector<double>& ox, const vector<double>& oy,
                  double xyreso, double yawreso, long max_expansions, vector<double>& rx, vector<double>& ry, vector<double>& ryaw) {
   syaw = pi_2_pi(syaw); gyaw = pi_2_pi(gyaw);
   const Config c = calc_config(ox, oy, xyreso, yawreso);
   Obstacles ob; ob.ox = ox; ob.oy = oy; ob.build();
+  const ObGridView grid = ob.view();
   Node nstart{jround(sx / xyreso), jround(sy / xyreso), jround(syaw / yawreso), true, {sx}, {sy}, {syaw}, 0.0, 0.0, -1};
   Node ngoal{jround(gx / xyreso), jround(gy / xyreso), jround(gyaw / yawreso), true, {gx}, {gy}, {gyaw}, 0.0, 0.0, -1};
   const DistPolicy H = calc_dist_policy(gx, gy, ox, oy, xyreso, VEHICLE_RADIUS);
-  auto cost_of = [&](const Node& n) {
-    const long i = n.xind - H.minx, j = n.yind - H.miny;
-    const double h = (1 <= i && i <= H.xw && 1 <= j && j <= H.yw) ? H.pmap[(size_t)(i - 1) * H.yw + (j - 1)] : INF;
-    return n.cost + H_COST * h;
-  };
+  auto cost_of = [&](const Node& n) { return n.cost + H_COST * heuristic(H.pmap.data(), H.minx, H.miny, H.xw, H.yw, n.xind, n.yind); };
   std::unordered_map<long, Node> open_, closed;
-  const long sid = calc_index(nstart, c);
+  const long sid = calc_index(nstart.xind, nstart.yind, nstart.yawind, c);
   open_[sid] = nstart;
   typedef std::tuple<double, long, long> Item;      // (priority, insertion tick, node id): heapq order of the Python restatement
   std::priority_queue<Item, vector<Item>, std::greater<Item> > pq;
   long tick = 0;
   pq.push(Item(cost_of(nstart), tick, sid));
-  vector<double> us, ds;
-  {
-    const double step = MAX_STEER / N_STEER;
-    vector<double> up;
-    for (int i = 0; i < (int)jround(N_STEER); ++i) up.push_back(step * (i + 1));
-    vector<double> u{0.0};
-    for (double v : up) u.push_back(v);
-    for (double v : up) u.push_back(-v);
-    us = u; us.insert(us.end(), u.begin(), u.end());
-    ds.assign(u.size(), 1.0); ds.insert(ds.end(), u.size(), -1.0);
-  }
-  const double maxc = std::tan(MAX_STEER) / WB;
+  vector<double> us, ds, tanu;
+  motion_inputs(us, ds, tanu);
+  const int nlist = motion_nlist();
+  const double maxc = max_curvature();
   Node final_node;
   long expansions = 0;
   for (;;) {
@@ -508,26 +113,31 @@ int hybrid_astar(double sx, double sy, double syaw, double gx, double gy, double
     if (it == open_.end()) continue;
     Node cur = it->second;
     ++expansions;
-    RsPath ap;
+    RsCand ap;
+    vector<double> apx, apy, apyaw;
     const bool have = calc_shortest_path(cur.x.back(), cur.y.back(), cur.yaw.back(), ngoal.x.back(), ngoal.y.back(), ngoal.yaw.back(), maxc,
-                                         MOTION_RESOLUTION, ap);
-    if (have && check_collision(ap.x, ap.y, ap.yaw, ob)) {
-      if (ap.x.size() >= 2) {
-        cur.x.insert(cur.x.end(), ap.x.begin() + 1, ap.x.end() - 1);
-        cur.y.insert(cur.y.end(), ap.y.begin() + 1, ap.y.end() - 1);
-        cur.yaw.insert(cur.yaw.end(), ap.yaw.begin() + 1, ap.yaw.end() - 1);
+                                         MOTION_RESOLUTION, ap, apx, apy, apyaw);
+    if (have && check_collision(apx, apy, apyaw, grid)) {
+      if (apx.size() >= 2) {
+        cur.x.insert(cur.x.end(), apx.begin() + 1, apx.end() - 1);
+        cur.y.insert(cur.y.end(), apy.begin() + 1, apy.end() - 1);
+        cur.yaw.insert(cur.yaw.end(), apyaw.begin() + 1, apyaw.end() - 1);
       }
-      cur.cost += calc_rs_path_cost(ap);
+      cur.cost += calc_rs_path_cost(ap.len, ap.ty, ap.n);
       final_node = cur;
       break;
     }
     open_.erase(it);
     closed[c_id] = cur;
     for (size_t m = 0; m < us.size(); ++m) {
-      Node node = calc_next_node(cur, c_id, us[m], ds[m], c);
+      Node node;
+      node.x.assign(nlist, 0.0); node.y.assign(nlist, 0.0); node.yaw.assign(nlist, 0.0);
+      next_poses(cur.x.back(), cur.y.back(), cur.yaw.back(), ds[m], tanu[m], nlist, node.x.data(), node.y.data(), node.yaw.data());
+      node.xind = jround(node.x.back() / c.xyreso); node.yind = jround(node.y.back() / c.xyreso); node.yawind = jround(node.yaw.back() / c.yawreso);
+      node.direction = ds[m] > 0; node.steer = us[m]; node.cost = cur.cost + step_cost(cur.direction, cur.steer, us[m], ds[m]); node.pind = c_id;
       if (!(0 < node.xind - c.minx && node.xind - c.minx < c.xw) || !(0 < node.yind - c.miny && node.yind - c.miny < c.yw)) continue;
-      if (!check_collision(node.x, node.y, node.yaw, ob)) continue;
-      const long nid = calc_index(node, c);
+      if (!check_collision(node.x, node.y, node.yaw, grid)) continue;
+      const long nid = calc_index(node.xind, node.yind, node.yawind, c);
       if (closed.count(nid) || open_.count(nid)) continue;
       const double pr = cost_of(node);
       open_[nid] = std::move(node);
@@ -551,66 +161,6 @@ int hybrid_astar(double sx, double sy, double syaw, double gx, double gy, double
   return OBCA_PLAN_OK;
 }
 
-// =====================================================================================================================
-// veloSmooth (obca_b200/planner/velo_smooth.py) and the warm-start extraction (warmstart.py)
-// =====================================================================================================================
-vector<double> linspace(double a, double b, int num) {
-  vector<double> y(num);
-  if (num == 1) { y[0] = a; return y; }
-  const double step = (b - a) / (num - 1);
-  for (int i = 0; i < num; ++i) y[i] = step != 0.0 ? (double)i * step + a : a;
-  y[num - 1] = b;
-  return y;
-}
-double sgn(double v) { return v > 0 ? 1.0 : (v < 0 ? -1.0 : 0.0); }
-void velo_smooth(const vector<double>& v, double amax, double Ts, vector<double>& v_mm, vector<double>& a) {
-  const int PAD = 19, n = (int)v.size(), M = n + 40;
-  vector<double> v_ex(M, 0.0);
-  vector<vector<double> > v_bar(4, vector<double>(M, 0.0));
-  for (int i = 0; i < n; ++i) { v_ex[PAD + i] = v[i]; for (int r = 0; r < 4; ++r) v_bar[r][PAD + i] = v[i]; }
-  const double v0 = std::fabs(v[0]), cut1 = 0.25 * v0, cut2 = 1.25 * v0;
-  const int acc = (int)jround(v0 / amax / Ts);
-  vector<int> idx1, idx2, idx3, idx4;      // 1-based indices into diff(v_ex), as in the reference
-  for (int i = 0; i + 1 < M; ++i) {
-    const double dv = v_ex[i + 1] - v_ex[i];
-    if (dv > cut1 && dv < cut2) idx1.push_back(i + 1);
-    if (dv > cut2) idx2.push_back(i + 1);
-    if (dv < -cut1 && dv > -cut2) idx3.push_back(i + 1);
-    if (dv < -cut2) idx4.push_back(i + 1);
-  }
-  if (!idx1.empty() && idx1[0] == 19) idx1[0] += 1;
-  if (!idx3.empty() && idx3[0] == 19) idx3[0] += 1;
-  auto ex = [&](int i) { return v_ex[i - 1]; };
-  auto put = [&](int row, int lo, int hi, double A, double B) {      // v_bar[row, lo:hi] = linspace(A, B, hi - lo + 1), 1-based inclusive
-    if (hi < lo) return;
-    const vector<double> y = linspace(A, B, hi - lo + 1);
-    for (int k = lo; k <= hi; ++k)
-      if (k >= 1 && k <= M) v_bar[row][k - 1] = y[k - lo];
-  };
-  for (int i : idx1) {
-    if (ex(i) > cut1 || ex(i + 1) > cut1) put(0, i, i + acc, 0.0, v0);
-    else if (ex(i) < -cut1 || ex(i + 1) < -cut1) put(0, i - acc + 1, i + 1, -v0, 0.0);
-  }
-  for (int i : idx3) {
-    if (ex(i) > cut1 || ex(i + 1) > cut1) put(1, i - acc + 1, i + 1, v0, 0.0);
-    else if (ex(i) < -cut1 || ex(i + 1) < -cut1) put(1, i, i + acc, 0.0, -v0);
-  }
-  for (int i : idx2) put(2, i - acc, i + acc, -v0, v0);
-  for (int i : idx4) put(3, i - acc, i + acc, v0, -v0);
-  v_mm.assign(n, 0.0);
-  for (int j = 0; j < n; ++j) {
-    const double ve = v_ex[PAD + j];
-    double mn = INF, mx = -INF;
-    for (int r = 0; r < 4; ++r) {
-      const double vb = v_bar[r][PAD + j];
-      const double w = vb == 0.0 ? vb : (sgn(ve) != sgn(vb) ? ve : vb);
-      mn = std::min(mn, w); mx = std::max(mx, w);
-    }
-    v_mm[j] = ve > 0 ? mn : mx;
-  }
-  a.assign(n > 0 ? n - 1 : 0, 0.0);
-  for (int j = 0; j + 1 < n; ++j) a[j] = (v_mm[j + 1] - v_mm[j]) / Ts;
-}
 vector<double> frange(double a, double b, double step) {
   const int n = (int)std::floor((b - a) / step + 1e-9);
   vector<double> r;
@@ -680,25 +230,16 @@ int obca_plan_warmstart(const double* x0, const double* xF, int scenario, double
   if (rc) return rc;
   // main.jl:222-248
   const int n = (int)px.size();
-  const double dt = Ts / sampleN, motionStep = MOTION_RESOLUTION, amax = 0.3;
-  vector<double> rv(n, 0.0), v, a;
-  for (int i = 0; i + 1 < n; ++i) rv[i] = (px[i + 1] - px[i]) / dt * std::cos(pyaw[i]) + (py[i + 1] - py[i]) / dt * std::sin(pyaw[i]);
-  velo_smooth(rv, amax, dt, v, a);
+  const double dt = Ts / sampleN;
+  vector<double> rv(n, 0.0), v(n), a(n > 0 ? n - 1 : 0), work(5 * (size_t)(n + 40));
+  for (int i = 0; i + 1 < n; ++i) rv[i] = ws_speed(px.data(), py.data(), pyaw.data(), i, dt);
+  velo_smooth(rv.data(), n, WS_AMAX, dt, work.data(), v.data(), a.data());
   vector<double> delta(n > 0 ? n - 1 : 0);
-  for (int i = 0; i + 1 < n; ++i) delta[i] = std::atan((pyaw[i + 1] - pyaw[i]) * L / motionStep * sgn(v[i]));
+  for (int i = 0; i + 1 < n; ++i) delta[i] = ws_steer(pyaw.data(), v.data(), i, L);
   const int ns = (n + sampleN - 1) / sampleN;      // len(rx[::sampleN])
-  const int N = ns - 1;
-  *N_out = N;
+  *N_out = ns - 1;
   if (ns > cap || !rx || !ry || !ryaw || !xWS || !uWS) return OBCA_PLAN_CAPACITY;
-  for (int k = 0; k < ns; ++k) {
-    const int i = k * sampleN;
-    rx[k] = px[i]; ry[k] = py[i]; ryaw[k] = pyaw[i];
-    xWS[k] = px[i]; xWS[ns + k] = py[i]; xWS[2 * ns + k] = pyaw[i]; xWS[3 * ns + k] = v[i];
-  }
-  for (int k = 0; k < N; ++k) {
-    const int i = k * sampleN;
-    uWS[k] = delta[i]; uWS[N + k] = a[i];
-  }
+  ws_store(px.data(), py.data(), pyaw.data(), v.data(), a.data(), delta.data(), n, sampleN, rx, ry, ryaw, xWS, uWS);
   return OBCA_PLAN_OK;
 }
 
@@ -726,9 +267,9 @@ int obca_plan_warmstart_batch(int B, const double* x0, const double* xF, int sce
 
 double obca_reeds_shepp_length(double sx, double sy, double syaw, double gx, double gy, double gyaw, double maxc) {
   const double q0[3] = {sx, sy, syaw}, q1[3] = {gx, gy, gyaw};
-  const vector<RsPath> paths = generate_path(q0, q1, maxc);
+  const RsSet s = generate_path(q0, q1, maxc);
   double best = INF;
-  for (const RsPath& p : paths) best = std::min(best, p.L / maxc);
+  for (int i = 0; i < s.n; ++i) best = std::min(best, s.L[i] / maxc);
   return best;
 }
 
