@@ -262,7 +262,8 @@ struct DevCtx {
   double* slots = nullptr; size_t slots_bytes = 0;  // stage slots of every problem, B x (N+1) x RSTRIDE
   char* pstate = nullptr; size_t pstate_bytes = 0;  // ProbState per problem
   int* act = nullptr; size_t act_bytes = 0;         // two active lists
-  int* ncnt = nullptr;                              // device: three rotating active counts, [3] tail work counter
+  int* ncnt = nullptr;                              // device: three rotating active counts, [3] tail work counter,
+                                                    // [4] / [5] work queues of k_pk_eval / k_pk_step
   int* h_n = nullptr;                               // pinned ring of active counts read back per round
   cudaEvent_t evr[16] = {nullptr};
   std::vector<cudaEvent_t> tev;                     // OBCA_PHASE_TIMING=1: pool of timing events
@@ -289,7 +290,7 @@ static int get_ctx(int dev, DevCtx** out) {
     c.sms = pr.multiProcessorCount;
     CK(cudaMalloc(&c.counter, sizeof(int)));
     CK(cudaMalloc(&c.prof, 8 * sizeof(unsigned long long)));
-    CK(cudaMalloc(&c.ncnt, 4 * sizeof(int)));
+    CK(cudaMalloc(&c.ncnt, 6 * sizeof(int)));
     CK(cudaMallocHost(&c.h_n, 16 * sizeof(int)));
     for (int i = 0; i < 16; ++i) CK(cudaEventCreateWithFlags(&c.evr[i], cudaEventDisableTiming));
     c.init = true;
@@ -384,8 +385,8 @@ static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, cons
   const int thresh = env_int("OBCA_TAIL_THRESH", mode == 2 ? 0 : (B / 2 > tail_cap ? B / 2 : tail_cap));
   const bool rounds = mode == 2 || (mode == 0 && B > 2 * tail_cap);
   c.last_rounds = 0; c.last_tail = B;
-  int h_init[4] = {B, 0, 0, 0};
-  CK(cudaMemcpyAsync(c.ncnt, h_init, 4 * sizeof(int), cudaMemcpyHostToDevice, st));
+  int h_init[6] = {B, 0, 0, 0, 0, 0};
+  CK(cudaMemcpyAsync(c.ncnt, h_init, 6 * sizeof(int), cudaMemcpyHostToDevice, st));
   if (!rounds) {
     const int grid = B < tail_cap ? B : tail_cap;
     k_pk_tail<VM, SDV><<<grid, PK_THREADS, smem_slots, st>>>(P, O, L, bp, c.W, Sg, nullptr, c.ncnt, c.ncnt + 3, 1);
@@ -407,16 +408,21 @@ static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, cons
     cudaEventRecord(c.tev[n_ev++], st);
   };
   auto cap = [](int n, int m) { return n < m ? (n > 0 ? n : 1) : m; };
-  // one round = three launches + the read-back of the active count; grids from an upper bound nb of the active count
+  // one round = three launches + the read-back of the active count; grids from an upper bound nb of the active count.  Work
+  // queues: k_pk_eval takes from ncnt[4] and zeroes ncnt[5] for the k_pk_step of its round, which zeroes ncnt[4] in turn.
+  // The two launches must stay paired and alternate: a schedule that launches one without the other (a k_pk_step alone before
+  // the hand-over, say) has to zero the counter it takes from itself, or the launch finds it spent and skips every problem.
   auto launch_round = [&](int rr, int nb, bool readback) -> int {
     const int* a_in = act[rr & 1]; int* a_out = act[(rr + 1) & 1];
     int* n_in = c.ncnt + (rr % 3); int* n_out = c.ncnt + ((rr + 1) % 3); int* n_zero = c.ncnt + ((rr + 2) % 3);
+    int* q_eval = c.ncnt + 4; int* q_step = c.ncnt + 5;
     mark();
-    k_pk_eval<VM, SDV><<<cap(nb, eval_cap), PK_THREADS, smem_slots, st>>>(P, O, L, bp, c.W, c.slots, Sg, a_in, n_in, a_out, n_out, rr == 0 ? 1 : 0);
+    k_pk_eval<VM, SDV><<<cap(nb, eval_cap), PK_THREADS, smem_slots, st>>>(P, O, L, bp, c.W, c.slots, Sg, a_in, n_in, a_out, n_out, rr == 0 ? 1 : 0,
+                                                                          q_eval, q_step);
     mark();
     k_pk_sweep<VM, SDV><<<(nb + SWEEP_WARPS - 1) / SWEEP_WARPS, 32 * SWEEP_WARPS, smem_sweep, st>>>(P, O, L, c.W, c.slots, Sg, a_out, n_out, n_zero);
     mark();
-    k_pk_step<VM, SDV><<<cap(nb, step_cap), PK_THREADS, smem_step, st>>>(P, O, L, bp, c.W, c.slots, Sg, a_out, n_out);
+    k_pk_step<VM, SDV><<<cap(nb, step_cap), PK_THREADS, smem_step, st>>>(P, O, L, bp, c.W, c.slots, Sg, a_out, n_out, q_step, q_eval);
     mark();
     CK(cudaGetLastError());
     if (readback) CK(cudaMemcpyAsync(c.h_n + (rr & 15), n_out, sizeof(int), cudaMemcpyDeviceToHost, st));

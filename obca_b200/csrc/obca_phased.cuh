@@ -16,6 +16,7 @@
 //     k_pk_step    persistent CTAs, one problem at a time: K4 -- item pass (steps of the block unknowns from the stored
 //                  local maps) + stage pass (costates, bounds), fraction-to-the-boundary, filter line search (merit
 //                  function: item + stage pass), iterate update.  The step of the block unknowns lives in shared memory.
+// The persistent CTAs of k_pk_eval and k_pk_step take their problems from an atomic work queue (pk_queue_next).
 // The iterate, the local maps and the stage slots of every problem live in HBM (layout: problem-major, then [array][stage],
 // so each warp streams contiguous slices); between kernels a problem is described by its ProbState record (phase,
 // iteration, barrier parameter, filter, ...).  When the active set has shrunk far enough the remaining problems are handed to
@@ -414,6 +415,18 @@ __device__ __forceinline__ void state_fresh(ProbState& S, int N) {
 // per-thread partial sums of a reduction depend on it, and the schedules must round identically.
 constexpr int PK_THREADS = OBCA_PK_THREADS;
 
+// Work queues of K_eval and K_step: a CTA takes the next problem of the active list from an atomic counter when it has
+// finished the last one, instead of every gridDim.x-th problem.  The cost of a problem varies several-fold (re-evaluation
+// after a barrier update, end of an attempt, backtracking in the line search), and with a fixed stride a launch lasted as
+// long as the CTA whose share held the most of it.  Each of the two kernels has its own counter and zeroes the other's
+// (the two alternate on the stream, with the sweep between them), so no host memset is needed between the launches of a
+// CUDA graph.
+__device__ __forceinline__ int pk_queue_next(int* queue, int* s_i) {
+  if (threadIdx.x == 0) *s_i = atomicAdd(queue, 1);
+  __syncthreads();
+  return *s_i;
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // K_eval: persistent CTAs, one problem at a time (see the file header).  fresh: first launch of a solve -- every problem
 // of the batch starts from its warm start (no active list yet).
@@ -426,17 +439,21 @@ __global__ void __launch_bounds__(PK_THREADS, OBCA_MINB_A)
 k_pk_eval(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpts O, const PkLay L, const BatchPtrs bp,
           double* __restrict__ Wall, double* __restrict__ slots, ProbState* __restrict__ Sg,
           const int* __restrict__ act_in, const int* __restrict__ n_in, int* __restrict__ act_out, int* __restrict__ n_out,
-          int fresh) {
+          int fresh, int* __restrict__ queue, int* __restrict__ queue_next) {
   extern __shared__ __align__(16) double s_ric[];     // (N+1) x RSTRIDE stage slots: hand-over area of the item pass, then
                                                      // the assembled stage models, bulk-copied out for the sweep kernel
   __shared__ ProbState S;
   __shared__ double s_red[4 * 12];
   __shared__ PkFinalScratch s_fin;
+  __shared__ int s_i;
   __shared__ PkCtx C; __shared__ PkOutputs out;
   const int NSL = P.N + 1;      // stage slots per problem in `slots`
   const int n = fresh ? bp.B : *n_in;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *queue_next = 0;
   unsigned long long n_eval = 0, n_eval2 = 0;
-  for (int a = blockIdx.x; a < n; a += gridDim.x) {
+  for (;;) {
+    const int a = pk_queue_next(queue, &s_i);
+    if (a >= n) break;
     const int b = fresh ? a : act_in[a];
     if (fresh) state_fresh(S, pk_horizon(bp, P, b)); else state_load(S, Sg + b);
     if (threadIdx.x == 0) {
@@ -577,17 +594,24 @@ template <int VM, bool SDV>
 __global__ void __launch_bounds__(PK_THREADS, OBCA_MINB_C)
 k_pk_step(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpts O, const PkLay L, const BatchPtrs bp,
           double* __restrict__ Wall, double* __restrict__ slots, ProbState* __restrict__ Sg,
-          const int* __restrict__ act, const int* __restrict__ n_act) {
+          const int* __restrict__ act, const int* __restrict__ n_act, int* __restrict__ queue, int* __restrict__ queue_next) {
   extern __shared__ __align__(16) double s_step[];      // (dRS + 1 - dLAM) x NSP
   __shared__ ProbState S;
   __shared__ double s_red[4 * 12];
+  __shared__ int s_i;
   __shared__ PkCtx C; __shared__ PkOutputs out;
   const int NSL = P.N + 1;      // stage slots per problem in `slots`
   const int n = *n_act;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *queue_next = 0;
   unsigned long long n_merit = 0;
-  for (int a = blockIdx.x; a < n; a += gridDim.x) {
+  for (;;) {
+    const int a = pk_queue_next(queue, &s_i);
+    if (a >= n) break;
     const int b = act[a];
-    if (Sg[b].phase != PH_RECOVER) continue;      // (uniform: every thread reads the same word)
+    if (Sg[b].phase != PH_RECOVER) {      // (uniform: every thread reads the same word)
+      __syncthreads();                    // every thread has read s_i before thread 0 takes the next problem
+      continue;
+    }
     state_load(S, Sg + b);
     if (threadIdx.x == 0) {
       pk_make_ctx<VM, SDV>(C, out, P, O, L, bp, b, Wall + (size_t)b * L.total * L.NSP);
