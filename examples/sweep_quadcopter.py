@@ -1,11 +1,13 @@
 """The quadcopter flow of the reference's QuadcopterNavigation/mainQuadcopter.jl:122-154 (each start / goal pair planned by the 3-D A*,
-then solved) as a batch: plan K config-4 pairs on host processes (obca_b200.planner.a_star_3d, 8-11 s per pair), solve all planned
+then solved) as a batch: plan K config-4 pairs -- planner "python": the Python restatement obca_b200.planner.a_star_3d on host
+processes (8-11 s per pair); "host": the same search in C++ on host threads (native.plan_quadcopter_batch); "gpu": on the GPU in one
+call (device.plan_quadcopter_batch); all three give the same plans --, solve all planned
 pairs -- each with the horizon N = path length - 1 and the sampling time Ts = round(0.25 * 80 / N, 2) the planner gave it -- in ONE
 GPU call (obca_quadcopter_solve_mixed), run the reference's constrSatisfaction on every result in one more call.  Pairs whose
 horizon exceeds the solver's limit (N + 1 <= 512; the planner gives N = 80..147 over the config-4 box) are counted and listed
 as skipped.
 
-usage: python examples/sweep_quadcopter.py [K] [seed] [workers]           (needs a CUDA device for the solves)
+usage: python examples/sweep_quadcopter.py [K] [seed] [workers] [python|host|gpu]      (needs a CUDA device for the solves)
 """
 import os
 import sys
@@ -19,20 +21,28 @@ sys.path.insert(0, ROOT)
 
 import obca_b200                                                   # noqa: E402
 from obca_b200 import quadcopter, scenarios                        # noqa: E402
+from obca_b200.planner import device, native                        # noqa: E402
 from obca_b200.planner.a_star_3d import plan_quadcopter_warm_start  # noqa: E402
 
 N_LIMIT = 511      # the quadcopter solver's longest horizon (N + 1 <= 512 stages, at most four per thread of a 128-thread CTA)
 
 
-def sweep(K=32, seed=2, signed_dist=1, workers=None):
+def sweep(K=32, seed=2, signed_dist=1, workers=None, planner="python"):
     sc = scenarios.quadcopter_batch(K, seed=seed)          # config-4 start / goal pairs (mainQuadcopter.jl:48-51)
     t0 = time.time()
-    with ProcessPoolExecutor(workers) as ex:
-        plans = list(ex.map(plan_quadcopter_warm_start, sc["x0"], sc["xF"], [sc["Ts80"]] * K))
+    if planner == "python":
+        with ProcessPoolExecutor(workers) as ex:
+            plans = list(ex.map(plan_quadcopter_warm_start, sc["x0"], sc["xF"], [sc["Ts80"]] * K))
+    elif planner == "host":
+        plans = native.plan_quadcopter_batch(sc["x0"], sc["xF"], sc["Ts80"], nthreads=workers or 0)
+    elif planner == "gpu":
+        plans = device.plan_quadcopter_batch(sc["x0"], sc["xF"], sc["Ts80"])
+    else:
+        raise ValueError(f"planner must be python, host or gpu, not {planner!r}")
     t_plan = time.time() - t0
     N = np.array([p["N"] if p else -1 for p in plans])
     idx = [i for i in range(K) if 2 <= N[i] <= N_LIMIT]
-    out = dict(K=K, planned=int((N >= 0).sum()), skipped=[(i, int(N[i])) for i in range(K) if N[i] > N_LIMIT], t_plan=t_plan,
+    out = dict(K=K, planner=planner, planned=int((N >= 0).sum()), skipped=[(i, int(N[i])) for i in range(K) if N[i] > N_LIMIT], t_plan=t_plan,
                t_solve=0.0, converged=0, feasible=0, N=N, Ts=np.array([p["Ts"] if p else np.nan for p in plans]))
     if not idx:
         return out
@@ -48,11 +58,12 @@ def sweep(K=32, seed=2, signed_dist=1, workers=None):
 if __name__ == "__main__":
     a = sys.argv
     try:
-        o = sweep(int(a[1]) if len(a) > 1 else 32, int(a[2]) if len(a) > 2 else 2, 1, int(a[3]) if len(a) > 3 else None)
+        o = sweep(int(a[1]) if len(a) > 1 else 32, int(a[2]) if len(a) > 2 else 2, 1, int(a[3]) if len(a) > 3 and int(a[3]) > 0 else None,
+                  a[4] if len(a) > 4 else "python")
     except obca_b200.ObcaError as e:
         print("solve not run:", e); sys.exit(2)
     ok = o["N"][o["N"] >= 0]
-    print(f"{o['K']} start / goal pairs: {o['planned']} planned in {o['t_plan']:.1f} s (host processes), N = {ok.min()}..{ok.max()} "
+    print(f"{o['K']} start / goal pairs: {o['planned']} planned in {o['t_plan']:.1f} s ({o['planner']} planner), N = {ok.min()}..{ok.max()} "
           f"({len(set(ok.tolist()))} distinct), Ts = {np.nanmin(o['Ts']):.2f}..{np.nanmax(o['Ts']):.2f}")
     if o["skipped"]:
         print(f"skipped {len(o['skipped'])} pair(s) with N > {N_LIMIT} (pair, N): {o['skipped']}")

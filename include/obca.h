@@ -212,6 +212,31 @@ int obca_plan_parking_warmstart_batch(int B, const double* x0, const double* xF,
                                       const obca_opts* opts, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
                                       int* N, int* status, int* expansions, double* plan_seconds);
 
+/* 3-D A* warm starts of the quadcopter flow on the GPU: B start / goal pairs (x0, xF: 3 x B column-major positions, each pair its own)
+ * among one obstacle point cloud (ox, oy, oz, n_ob >= 0 points; lo, hi: the bound corners in raw units; reso > 0: the cell size) in ONE
+ * call -- the inputs and outputs of obca_astar3d_batch of include/obca_planner.h, with the same search decisions bit for bit (the search
+ * compiles from the same source, obca_b200/planner/csrc/obca_astar3d_core.h): the same status, N, path and expansion count.  One warp
+ * plans one pair at a time (k_plan3d); the obstacle bitmap is built on the host, once per call.
+ *   max_nodes: node pool per warp; <= 0 selects 262144 (2^18; the largest config-4 search of 2048 pairs uses 229043 nodes); at most 2^28.
+ *     The queue holds max_nodes / 4 entries (at least 64).  Device scratch per warp: a 4-byte cell table over the map (2.4 MB for the
+ *     105 x 105 x 55 demo grid) + max_nodes x 16 bytes + the queue's 4 x max_nodes bytes; about 7.7 MB at the defaults.
+ *     Device memory of one call: min(B rounded up to 4, 4 x SMs) warps x that scratch -- about 4.0 GB on a 132-SM H100 for B >= 528 at
+ *     the defaults --, plus the bitmap (w0 x w1 x w2 / 8 bytes, 76 KB for the demo grid), 48 x B bytes of cells and the outputs,
+ *     24 x B x cap + 12 x B bytes, which are copied to the device first (so that the entries the planner does not write keep the
+ *     caller's values) and back after the kernel.  All of it is freed before the call returns.
+ * Outputs, with the stride cap: rx / ry / rz [i*cap ..]: the path, start first, as cell * reso (N[i]+1 points).
+ * status[i]: OBCA_PLAN_OK (0), OBCA_PLAN_NO_PATH (1), OBCA_PLAN_CAPACITY (2: more than cap points; N[i] holds the horizon, nothing else
+ * written), or OBCA_PLAN_POOL_FULL (4): the search needed more than max_nodes nodes or max_nodes / 4 queue entries and was stopped; that
+ * pair is NOT planned (nothing else written); the host library can plan it (obca_b200.planner.device.plan_quadcopter_batch does so).
+ * expansions[i] (may be NULL): cells closed, the goal included.  plan_seconds (may be NULL): device time of the search kernel.
+ * Return: 0, OBCA_ERR_ARG (B < 0, a null array, n_ob < 0, reso <= 0, cap < 1, max_nodes > 2^28, a non-finite coordinate, a map of
+ * more than 2^27 cells or a start / goal more than 2^30 cells from it; reason in obca_last_error(), nothing written), OBCA_ERR_NO_DEVICE,
+ * OBCA_ERR_CUDA. */
+int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz,
+                                         int n_ob, const double* lo, const double* hi, double reso, int max_nodes, int cap,
+                                         const obca_opts* opts, double* rx, double* ry, double* rz, int* N, int* status, int* expansions,
+                                         double* plan_seconds);
+
 /* Device times of the last obca_parking_solve_batch[_dev] / obca_parking_solve_mixed on `device`: DualMultWS (0 when the caller passed lWS / nWS) and the
  * solve alone (= what solve_seconds reports; the reference's `time`, ParkingSignedDist.jl:297). */
 int obca_last_times(int device, double* dualws_seconds, double* solve_seconds);

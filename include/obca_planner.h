@@ -48,6 +48,26 @@ int obca_plan_warmstart(const double* x0, const double* xF, int scenario, double
 int obca_plan_warmstart_batch(int B, const double* x0, const double* xF, int scenario, double Ts, double L, int sampleN, int cap, int nthreads,
                               double* rx, double* ry, double* ryaw, double* xWS, double* uWS, int* N, int* status);
 
+/* 3-D grid A* of the quadcopter flow (a_star_3D.jl:49-154, mainQuadcopter.jl:122-135) for B start / goal pairs among one obstacle point
+ * cloud, on nthreads host threads (<= 0: hardware concurrency).  The decisions are those of the Python restatement
+ * obca_b200/planner/a_star_3d.py (calc_astar_path), bit for bit.
+ *   x0, xF: 3 x B column-major start / goal positions (each pair its own); ox, oy, oz: n_ob >= 0 obstacle points; lo, hi: the two bound
+ *   corners (x, y, z) of the map, in raw units -- not divided by reso, as in calc_obstacle_map; reso > 0: the cell size.
+ * Pair i writes status[i] (OBCA_PLAN_OK / NO_PATH / CAPACITY), expansions[i] (may be NULL: cells closed, the goal included) and, on OK,
+ * N[i] = points - 1 and the path, start first, as cell * reso into rx / ry / rz [i*cap ..]; on CAPACITY (more than cap points) only N[i].
+ * Return OBCA_PLAN_BAD_ARG (no output written) for B < 0, a null array, n_ob < 0, reso <= 0, cap < 1, a non-finite coordinate, a map of
+ * more than 2^27 cells or a start / goal more than 2^30 cells away from it; else OBCA_PLAN_OK.
+ * GPU twin: obca_plan_quadcopter_warmstart_batch in include/obca.h; both compile the search from obca_b200/planner/csrc/obca_astar3d_core.h. */
+int obca_astar3d_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz, int n_ob,
+                       const double* lo, const double* hi, double reso, int cap, int nthreads, double* rx, double* ry, double* rz, int* N,
+                       int* status, int* expansions);
+
+/* The obstacle map both 3-D A* entries build (calc_obstacle_map of a_star_3d.py for the points divided by reso): mn[3] (the cell of map
+ * index 0), w[3] (the map's extent), and, when w0 * w1 * w2 <= cap, blocked[(ix * w1 + iy) * w2 + iz] = 1 for a blocked cell, else 0
+ * (OBCA_PLAN_CAPACITY otherwise).  Used by tests. */
+int obca_astar3d_obstacle_map(const double* ox, const double* oy, const double* oz, int n_ob, const double* lo, const double* hi, double reso,
+                              long long* mn, int* w, unsigned char* blocked, long long cap);
+
 /* Reeds-Shepp shortest path length between two poses for maximum curvature maxc (reeds_shepp.jl:79-96); used by tests. */
 double obca_reeds_shepp_length(double sx, double sy, double syaw, double gx, double gy, double gyaw, double maxc);
 

@@ -1,0 +1,174 @@
+// obca_plan3d.cu -- the GPU 3-D A* warm-start producer of the quadcopter flow (obca_plan_quadcopter_warmstart_batch of include/obca.h):
+// k_plan3d and its entry.  Built as its own translation unit WITHOUT FMA contraction (-fmad=false), because the host planner it reproduces
+// is built with -ffp-contract=off; linked into libobca.so next to obca_lib.cu (see __graft_entry__.build()).
+//
+// k_plan3d: persistent CTAs of P3_WARPS warps; every warp takes pairs from an atomic counter (the longest config-4 search expands 10x
+// the cells of the shortest) and runs astar3d_one (obca_astar3d_core.h) with its 32 lanes: lanes 0..25 test one neighbour each, a ballot
+// and a prefix count give the new nodes and the insertion ticks in motion order, and the lanes compare the 32 children of a queue entry in
+// one reduction.  Each warp owns its scratch in global memory (cell -> node table, node pool, queue), reused pair after pair.
+#include <cuda_runtime.h>
+
+#include <string>
+#include <vector>
+
+#include "../../include/obca.h"
+#include "../../include/obca_planner.h"
+#include "../planner/csrc/obca_astar3d_core.h"
+
+void obca_set_last_error(const std::string& s);      // obca_lib.cu
+static_assert(obca_astar3d::A3_POOL_FULL == OBCA_PLAN_POOL_FULL, "status code of a full node pool or queue");
+static_assert(obca_astar3d::A3_CAPACITY == OBCA_PLAN_CAPACITY && obca_astar3d::A3_NO_PATH == OBCA_PLAN_NO_PATH, "status codes");
+
+using namespace obca_astar3d;
+
+namespace {
+
+constexpr int P3_WARPS = 4;                    // warps per CTA, one CTA per SM: 528 searches in flight on a 132-SM H100
+constexpr int P3_DEFAULT_NODES = 1 << 18;      // the most nodes a config-4 search of quadcopter_batch(2048, seed=2) uses is 229043
+constexpr unsigned FULL = 0xffffffffu;
+
+// The 32 lanes of a warp: lane m < 26 holds the values of move m.
+struct WarpLanes {
+  template <class T> using PerMove = T;
+  __device__ int lane() const { return threadIdx.x & 31; }
+  __device__ int width() const { return 32; }
+  __device__ void sync() const { __syncwarp(); }
+  template <class T> __device__ T& at(T& v, int) const { return v; }
+  template <class T> __device__ T take(const T& v, int m) const { return __shfl_sync(FULL, v, m); }
+  __device__ unsigned mask(bool v) const { return __ballot_sync(FULL, lane() < N_MOVES && v); }
+  // the smallest (f, tick) over the lanes; bj < 0: this lane holds no child
+  __device__ void qmin(A3Item& best, int& bj) const {
+    for (int o = 16; o > 0; o >>= 1) {
+      const double f = __shfl_xor_sync(FULL, best.f, o);
+      const unsigned t = __shfl_xor_sync(FULL, best.tick, o);
+      const int nd = __shfl_xor_sync(FULL, best.node, o), j = __shfl_xor_sync(FULL, bj, o);
+      const A3Item x{f, t, nd};
+      if (j >= 0 && (bj < 0 || a3_less(x, best))) { best = x; bj = j; }
+    }
+  }
+};
+
+__global__ void __launch_bounds__(P3_WARPS * 32) k_plan3d(int B, A3Const C, A3IO io, A3Scratch W0, size_t table_stride, int* counter) {
+  const size_t w = (size_t)blockIdx.x * P3_WARPS + threadIdx.x / 32;
+  const A3Scratch W{W0.table + w * table_stride, W0.pool + w * C.max_nodes, W0.queue + w * C.max_queue};
+  const WarpLanes ln{};
+  for (;;) {
+    int p = 0;
+    if (ln.lane() == 0) p = atomicAdd(counter, 1);
+    p = __shfl_sync(FULL, p, 0);
+    if (p >= B) break;
+    astar3d_one(ln, C, W, io, p);
+  }
+}
+
+#define PCK(call)                                                                    \
+  do {                                                                               \
+    cudaError_t e_ = (call);                                                         \
+    if (e_ != cudaSuccess) {                                                         \
+      obca_set_last_error(std::string(#call) + ": " + cudaGetErrorString(e_));       \
+      rc = OBCA_ERR_CUDA;                                                            \
+      goto done;                                                                     \
+    }                                                                                \
+  } while (0)
+
+template <class T>
+T* carve(char*& p, size_t n) {
+  T* r = (T*)p;
+  p += (n * sizeof(T) + 255) / 256 * 256;
+  return r;
+}
+size_t padded(size_t bytes) { return (bytes + 255) / 256 * 256; }
+
+}  // namespace
+
+extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy,
+                                                    const double* oz, int n_ob, const double* lo, const double* hi, double reso,
+                                                    int max_nodes, int cap, const obca_opts* opts, double* rx, double* ry, double* rz,
+                                                    int* N, int* status, int* expansions, double* plan_seconds) {
+  if (!rx || !ry || !rz || !N || !status) { obca_set_last_error("null argument"); return OBCA_ERR_ARG; }
+  if (max_nodes > A3_MAX_NODES) { obca_set_last_error("max_nodes > 2^28"); return OBCA_ERR_ARG; }
+  A3Setup S;
+  {
+    std::string why;
+    if (astar3d_setup(S, why, B, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, cap)) { obca_set_last_error(why); return OBCA_ERR_ARG; }
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { obca_set_last_error("no CUDA device visible"); return OBCA_ERR_NO_DEVICE; }
+  const int dev = opts ? opts->device : 0;
+  if (dev < 0 || dev >= ndev) { obca_set_last_error("bad device ordinal"); return OBCA_ERR_ARG; }
+  if (plan_seconds) *plan_seconds = 0.0;
+  if (B == 0) return 0;
+  if (max_nodes <= 0) max_nodes = P3_DEFAULT_NODES;
+  A3Const C = S.C;
+  C.max_nodes = max_nodes;
+  C.max_queue = max_nodes / 4 > 64 ? max_nodes / 4 : 64;
+
+  int rc = 0, sms = 0;
+  cudaStream_t st = nullptr;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  char *dconst = nullptr, *dscr = nullptr, *dio = nullptr;
+  {
+    PCK(cudaSetDevice(dev));
+    PCK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PCK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    PCK(cudaEventCreate(&e0)); PCK(cudaEventCreate(&e1));
+    const int grid = (B + P3_WARPS - 1) / P3_WARPS < sms ? (B + P3_WARPS - 1) / P3_WARPS : sms;
+    const size_t nw = (size_t)grid * P3_WARPS, nmap = S.map.size(), Bs = (size_t)B;
+    // batch constants: the obstacle bitmap, the pairs' cells, the counter
+    PCK(cudaMalloc(&dconst, padded(nmap * 4) + 2 * padded(3 * Bs * 8) + 256));
+    char* q = dconst;
+    uint32_t* dmap = carve<uint32_t>(q, nmap);
+    long long* ds = carve<long long>(q, 3 * Bs);
+    long long* dg = carve<long long>(q, 3 * Bs);
+    int* dcounter = carve<int>(q, 1);
+    PCK(cudaMemcpyAsync(dmap, S.map.data(), nmap * 4, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(ds, S.s.data(), 3 * Bs * 8, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(dg, S.g.data(), 3 * Bs * 8, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemsetAsync(dcounter, 0, sizeof(int), st));
+    C.map = dmap;
+    // per warp: cell table, node pool, queue
+    const size_t table_stride = padded((size_t)(S.cells > 0 ? S.cells : 1) * 4) / 4;
+    PCK(cudaMalloc(&dscr, padded(table_stride * 4 * nw) + padded(sizeof(A3Node) * C.max_nodes * nw) +
+                              padded(sizeof(A3Item) * C.max_queue * nw)));
+    q = dscr;
+    A3Scratch W0;
+    W0.table = carve<int>(q, table_stride * nw);
+    W0.pool = carve<A3Node>(q, (size_t)C.max_nodes * nw);
+    W0.queue = carve<A3Item>(q, (size_t)C.max_queue * nw);
+    PCK(cudaMemsetAsync(W0.table, 0xff, table_stride * 4 * nw, st));      // -1: no node
+    // outputs: copied in first, so that the kernel leaves every entry it does not write as the caller had it
+    const size_t cb = Bs * cap;
+    PCK(cudaMalloc(&dio, 3 * padded(cb * 8) + 3 * padded(Bs * 4)));
+    q = dio;
+    double* drx = carve<double>(q, cb); double* dry = carve<double>(q, cb); double* drz = carve<double>(q, cb);
+    int* dN = carve<int>(q, Bs); int* dst = carve<int>(q, Bs); int* dex = carve<int>(q, Bs);
+    PCK(cudaMemcpyAsync(drx, rx, cb * 8, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(dry, ry, cb * 8, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(drz, rz, cb * 8, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(dN, N, Bs * 4, cudaMemcpyHostToDevice, st));
+    if (expansions) PCK(cudaMemcpyAsync(dex, expansions, Bs * 4, cudaMemcpyHostToDevice, st));
+    const A3IO io{ds, dg, drx, dry, drz, dN, dst, expansions ? dex : nullptr, nullptr, nullptr};
+    PCK(cudaEventRecord(e0, st));
+    k_plan3d<<<grid, P3_WARPS * 32, 0, st>>>(B, C, io, W0, table_stride, dcounter);
+    PCK(cudaGetLastError());
+    PCK(cudaEventRecord(e1, st));
+    PCK(cudaMemcpyAsync(rx, drx, cb * 8, cudaMemcpyDeviceToHost, st));
+    PCK(cudaMemcpyAsync(ry, dry, cb * 8, cudaMemcpyDeviceToHost, st));
+    PCK(cudaMemcpyAsync(rz, drz, cb * 8, cudaMemcpyDeviceToHost, st));
+    PCK(cudaMemcpyAsync(N, dN, Bs * 4, cudaMemcpyDeviceToHost, st));
+    PCK(cudaMemcpyAsync(status, dst, Bs * 4, cudaMemcpyDeviceToHost, st));
+    if (expansions) PCK(cudaMemcpyAsync(expansions, dex, Bs * 4, cudaMemcpyDeviceToHost, st));
+    PCK(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    PCK(cudaEventElapsedTime(&ms, e0, e1));
+    if (plan_seconds) *plan_seconds = ms * 1e-3;
+  }
+done:
+  if (dio) cudaFree(dio);
+  if (dscr) cudaFree(dscr);
+  if (dconst) cudaFree(dconst);
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  if (st) cudaStreamDestroy(st);
+  return rc;
+}

@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../../include/obca_planner.h"
+#include "obca_astar3d_core.h"
 #include "obca_plan_core.h"
 
 namespace {
@@ -262,6 +263,62 @@ int obca_plan_warmstart_batch(int B, const double* x0, const double* xF, int sce
   for (int t = 1; t < nthreads; ++t) pool.emplace_back(work);
   work();
   for (auto& t : pool) t.join();
+  return OBCA_PLAN_OK;
+}
+
+int obca_astar3d_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz, int n_ob,
+                       const double* lo, const double* hi, double reso, int cap, int nthreads, double* rx, double* ry, double* rz, int* N,
+                       int* status, int* expansions) {
+  namespace a3 = obca_astar3d;
+  if (!rx || !ry || !rz || !N || !status) return OBCA_PLAN_BAD_ARG;
+  a3::A3Setup S;
+  std::string why;
+  if (a3::astar3d_setup(S, why, B, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, cap)) return OBCA_PLAN_BAD_ARG;
+  if (nthreads <= 0) nthreads = (int)std::thread::hardware_concurrency();
+  if (nthreads < 1) nthreads = 1;
+  if (nthreads > B) nthreads = B > 0 ? B : 1;
+  const a3::A3IO io{S.s.data(), S.g.data(), rx, ry, rz, N, status, expansions, nullptr, nullptr};
+  const long long most_nodes = S.cells + 1;      // every map cell and a start outside the map
+  std::atomic<int> next(0);
+  auto work = [&]() {
+    // one scratch per thread, reused pair after pair; a search that outgrows it is repeated with twice the room (same decisions)
+    a3::A3Const C = S.C;
+    C.max_nodes = (int)std::min<long long>(most_nodes, 1 << 16);
+    C.max_queue = 1 << 14;
+    vector<int> table(S.cells > 0 ? S.cells : 1, -1);
+    vector<a3::A3Node> pool(C.max_nodes);
+    vector<a3::A3Item> queue(C.max_queue);
+    for (;;) {
+      const int i = next.fetch_add(1);
+      if (i >= B) break;
+      for (;;) {
+        a3::astar3d_one(a3::SeqLanes(), C, a3::A3Scratch{table.data(), pool.data(), queue.data()}, io, i);
+        if (status[i] != a3::A3_POOL_FULL) break;
+        C.max_nodes = (int)std::min<long long>(most_nodes, 2LL * C.max_nodes);
+        C.max_queue *= 2;
+        pool.resize(C.max_nodes);
+        queue.resize(C.max_queue);
+      }
+    }
+  };
+  vector<std::thread> threads;
+  for (int t = 1; t < nthreads; ++t) threads.emplace_back(work);
+  work();
+  for (auto& t : threads) t.join();
+  return OBCA_PLAN_OK;
+}
+
+int obca_astar3d_obstacle_map(const double* ox, const double* oy, const double* oz, int n_ob, const double* lo, const double* hi, double reso,
+                              long long* mn, int* w, unsigned char* blocked, long long cap) {
+  namespace a3 = obca_astar3d;
+  if (!mn || !w) return OBCA_PLAN_BAD_ARG;
+  a3::A3Setup S;
+  std::string why;
+  const double zero[3] = {0.0, 0.0, 0.0};
+  if (a3::astar3d_setup(S, why, 0, zero, zero, ox, oy, oz, n_ob, lo, hi, reso, 1)) return OBCA_PLAN_BAD_ARG;
+  for (int a = 0; a < 3; ++a) { mn[a] = S.C.mn[a]; w[a] = S.C.w[a]; }
+  if (S.cells > cap || !blocked) return OBCA_PLAN_CAPACITY;
+  for (long long c = 0; c < S.cells; ++c) blocked[c] = (S.map[c >> 5] >> (c & 31)) & 1u;
   return OBCA_PLAN_OK;
 }
 

@@ -1,7 +1,9 @@
-"""The GPU Hybrid A* warm-start producer (obca_plan_parking_warmstart_batch in libobca.so, include/obca.h): B start poses towards one
-goal in one call, with the search decisions of the host planner (obca_b200.planner.native).  Without a CUDA device the call raises.
-A pose whose search outgrows the device's scratch comes back as POOL_FULL in `status` (plan_raw); plan_batch plans those poses with
-the host planner, which makes the same decisions."""
+"""The GPU warm-start producers of libobca.so (include/obca.h), with the search decisions of the host planners (obca_b200.planner.native):
+  - obca_plan_parking_warmstart_batch, Hybrid A*: B start poses towards one goal in one call (plan_raw, plan_batch);
+  - obca_plan_quadcopter_warmstart_batch, the 3-D A* of the quadcopter flow: B start / goal pairs in one call (plan_quadcopter_raw,
+    plan_quadcopter_batch).
+Without a CUDA device the calls raise.  A search that outgrows the device's scratch comes back as POOL_FULL in `status` (the *_raw
+functions); the *_batch functions plan those problems with the host planner, which makes the same decisions."""
 from __future__ import annotations
 
 import ctypes as C
@@ -34,6 +36,52 @@ def plan_raw(x0s, xF, ox, oy, Ts, L=2.7, sampleN=3, cap=512, max_nodes=0, max_ex
     _lib.check(rc)
     o["seconds"] = secs.value
     return o
+
+
+def plan_quadcopter_raw(starts, goals, ox, oy, oz, lo, hi, reso, cap=1024, max_nodes=0, opts=None):
+    """obca_plan_quadcopter_warmstart_batch's outputs as arrays (rx, ry, rz (B, cap), N, status, expansions, seconds): the outputs of
+    native.astar3d_raw, planned on the GPU.  The output buffers start as NaN (N and expansions as -1): entries the planner does not write
+    stay so."""
+    f = lambda a: np.ascontiguousarray(np.asarray(a, float))
+    s = f(np.asarray(starts, float).reshape(-1, 3)); g = f(np.asarray(goals, float).reshape(-1, 3)); B = s.shape[0]
+    ox, oy, oz, lo, hi = f(ox), f(oy), f(oz), f(lo), f(hi)
+    o = dict(rx=np.full((B, cap), np.nan), ry=np.full((B, cap), np.nan), rz=np.full((B, cap), np.nan), N=np.full(B, -1, np.int32),
+             status=np.full(B, -1, np.int32), expansions=np.full(B, -1, np.int32))
+    secs = C.c_double(0.0)
+    opts = opts if opts is not None else _lib.default_opts()
+    p = _lib.ptr
+    fn = _lib.lib().obca_plan_quadcopter_warmstart_batch
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_int] + [C.c_void_p] * 8
+    rc = fn(B, p(s), p(g), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), int(cap), C.cast(C.byref(opts), C.c_void_p),
+            *[p(o[k]) for k in ("rx", "ry", "rz", "N", "status", "expansions")], C.cast(C.byref(secs), C.c_void_p))
+    _lib.check(rc)
+    o["seconds"] = secs.value
+    return o
+
+
+def plan_quadcopter_batch(x0s, xFs, Ts=0.25, cap=1024, max_nodes=0, opts=None):
+    """native.plan_quadcopter_batch on the GPU: for every pair the dictionary of a_star_3d.plan_quadcopter_warm_start (None where no path
+    was found).  Pairs whose search outgrew the device's scratch (POOL_FULL, see include/obca.h) are planned by the host library, which
+    makes the same decisions; raises if a path did not fit `cap`, as native.plan_quadcopter_batch does."""
+    s, g, ox, oy, oz, lo, hi, reso = native.quadcopter_problem(x0s, xFs)
+    o = plan_quadcopter_raw(s, g, ox, oy, oz, lo, hi, reso, cap, max_nodes, opts)
+    st = o["status"].copy()
+    full = np.nonzero(st == POOL_FULL)[0]
+    if full.size:
+        h = native.astar3d_raw(s[full], g[full], ox, oy, oz, lo, hi, reso, cap)
+        for k in ("rx", "ry", "rz", "N", "status"):
+            o[k][full] = h[k]
+        st[full] = h["status"]
+    if (st > 1).any():
+        raise native.PlannerError(f"obca_plan_quadcopter_warmstart_batch: status {st[st > 1][:5]} at pairs {np.nonzero(st > 1)[0][:5]}")
+    out = []
+    for i in range(len(st)):
+        if st[i]:
+            out.append(None); continue
+        n = int(o["N"][i]) + 1
+        out.append(native.quadcopter_warm_start(o["rx"][i, :n].copy(), o["ry"][i, :n].copy(), o["rz"][i, :n].copy(), Ts))
+    return out
 
 
 def plan_batch(x0s, xF, scenario="backwards", Ts=None, L=2.7, sampleN=3, cap=512, max_nodes=0, opts=None):

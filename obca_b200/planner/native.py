@@ -35,6 +35,10 @@ def lib():
         L.obca_plan_warmstart_batch.argtypes = [i, p, p, i, d, d, i, i, i] + [p] * 7
         L.obca_reeds_shepp_length.restype = d
         L.obca_reeds_shepp_length.argtypes = [d] * 7
+        L.obca_astar3d_batch.restype = i
+        L.obca_astar3d_batch.argtypes = [i] + [p] * 5 + [i, p, p, d, i, i] + [p] * 6
+        L.obca_astar3d_obstacle_map.restype = i
+        L.obca_astar3d_obstacle_map.argtypes = [p] * 3 + [i, p, p, d, p, p, p, C.c_longlong]
         _lib = L
     return _lib
 
@@ -108,3 +112,84 @@ def plan_batch(x0s, xF, scenario="backwards", workers=0, Ts=None, L=2.7, sampleN
 
 def reeds_shepp_length(sx, sy, syaw, gx, gy, gyaw, maxc):
     return lib().obca_reeds_shepp_length(float(sx), float(sy), float(syaw), float(gx), float(gy), float(gyaw), float(maxc))
+
+
+# ---- the 3-D A* of the quadcopter flow (obca_astar3d_batch; same decisions as obca_b200.planner.a_star_3d.calc_astar_path) ----
+
+def _f64(a):
+    return np.ascontiguousarray(np.asarray(a, float))
+
+
+def astar3d_obstacle_map(ox, oy, oz, lo, hi, reso):
+    """(blocked (w0, w1, w2) bool, mn, w): the map the 3-D A* entries build; equals a_star_3d.calc_obstacle_map(ox / reso, ..., lo, hi, reso)."""
+    ox, oy, oz, lo, hi = _f64(ox), _f64(oy), _f64(oz), _f64(lo), _f64(hi)
+    mn = np.zeros(3, np.int64); w = np.zeros(3, np.int32)
+    rc = lib().obca_astar3d_obstacle_map(_p(ox), _p(oy), _p(oz), int(ox.size), _p(lo), _p(hi), float(reso), _p(mn), _p(w), None, 0)
+    if rc not in (0, 2):
+        raise PlannerError(f"obca_astar3d_obstacle_map: {rc}")
+    blocked = np.zeros(int(np.prod(w.astype(np.int64))), np.uint8)
+    rc = lib().obca_astar3d_obstacle_map(_p(ox), _p(oy), _p(oz), int(ox.size), _p(lo), _p(hi), float(reso), _p(mn), _p(w), _p(blocked), blocked.size)
+    if rc:
+        raise PlannerError(f"obca_astar3d_obstacle_map: {rc}")
+    return blocked.reshape(tuple(w.tolist())).astype(bool), mn.tolist(), w.tolist()
+
+
+def astar3d_raw(starts, goals, ox, oy, oz, lo, hi, reso, cap=1024, nthreads=0):
+    """obca_astar3d_batch's outputs as arrays: rx, ry, rz (B, cap), N, status, expansions.  The output buffers start as NaN (N as -1)."""
+    s = _f64(np.asarray(starts, float).reshape(-1, 3)); g = _f64(np.asarray(goals, float).reshape(-1, 3)); B = s.shape[0]
+    ox, oy, oz, lo, hi = _f64(ox), _f64(oy), _f64(oz), _f64(lo), _f64(hi)
+    o = dict(rx=np.full((B, cap), np.nan), ry=np.full((B, cap), np.nan), rz=np.full((B, cap), np.nan), N=np.full(B, -1, np.int32),
+             status=np.full(B, -1, np.int32), expansions=np.full(B, -1, np.int32))
+    rc = lib().obca_astar3d_batch(B, _p(s), _p(g), _p(ox), _p(oy), _p(oz), int(ox.size), _p(lo), _p(hi), float(reso), int(cap), int(nthreads),
+                                  *[_p(o[k]) for k in ("rx", "ry", "rz", "N", "status", "expansions")])
+    if rc:
+        raise PlannerError(f"obca_astar3d_batch: {rc}")
+    return o
+
+
+def calc_astar_path(sx, sy, sz, gx, gy, gz, ox, oy, oz, xmin, ymin, zmin, xmax, ymax, zmax, reso, cap=4096):
+    """a_star_3d.calc_astar_path in one native call: (rx, ry, rz), or (None, None, None) when there is no path."""
+    o = astar3d_raw([(sx, sy, sz)], [(gx, gy, gz)], ox, oy, oz, (xmin, ymin, zmin), (xmax, ymax, zmax), reso, cap, 1)
+    st = int(o["status"][0])
+    if st == 1:
+        return None, None, None
+    if st:
+        raise PlannerError(f"obca_astar3d_batch: status {st}")
+    n = int(o["N"][0]) + 1
+    return o["rx"][0, :n].copy(), o["ry"][0, :n].copy(), o["rz"][0, :n].copy()
+
+
+def quadcopter_warm_start(rx, ry, rz, Ts):
+    """The dictionary of a_star_3d.plan_quadcopter_warm_start for the path (rx, ry, rz) on the 10x grid (mainQuadcopter.jl:130-137)."""
+    from .grid_policy import jround
+    N = rx.size - 1
+    Ts_as = jround(Ts * 80 / N * 100) / 100
+    xWS = np.zeros((12, N + 1))
+    xWS[0], xWS[1], xWS[2] = rx / 10.0, ry / 10.0, rz / 10.0
+    return dict(N=N, Ts=Ts_as, xWS=xWS, uWS=0.5 * np.ones((4, N)), timeWS=1.0, path=(rx, ry, rz))
+
+
+def quadcopter_problem(x0s, xFs):
+    """The inputs of plan_quadcopter_warm_start for a batch: starts and goals on the 10x grid (B, 3), the environment's points and
+    bounds, reso = 1."""
+    from .a_star_3d import quadcopter_environment
+    x0s = np.asarray(x0s, float).reshape(len(x0s), -1)[:, :3]; xFs = np.asarray(xFs, float).reshape(len(xFs), -1)[:, :3]
+    ox, oy, oz, lo, hi = quadcopter_environment()
+    return x0s * 10.0, xFs * 10.0, ox, oy, oz, lo, hi, 1.0
+
+
+def plan_quadcopter_batch(x0s, xFs, Ts=0.25, nthreads=0, cap=1024):
+    """a_star_3d.plan_quadcopter_warm_start for every pair (x0s[i], xFs[i]) on a pool of host threads: the same list of dictionaries
+    (None where no path was found)."""
+    s, g, ox, oy, oz, lo, hi, reso = quadcopter_problem(x0s, xFs)
+    o = astar3d_raw(s, g, ox, oy, oz, lo, hi, reso, cap, nthreads)
+    st = o["status"]
+    if (st > 1).any():
+        raise PlannerError(f"obca_astar3d_batch: status {st[st > 1][:5]} at pairs {np.nonzero(st > 1)[0][:5]}")
+    out = []
+    for i in range(len(st)):
+        if st[i]:
+            out.append(None); continue
+        n = int(o["N"][i]) + 1
+        out.append(quadcopter_warm_start(o["rx"][i, :n].copy(), o["ry"][i, :n].copy(), o["rz"][i, :n].copy(), Ts))
+    return out
