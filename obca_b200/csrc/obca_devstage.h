@@ -1,0 +1,134 @@
+// obca_devstage.h -- host glue of the C-ABI's CUDA translation units (obca_lib.cu, obca_plan.cu, obca_plan3d.cu): error reporting,
+// the device check, the layout of the typed arrays carved from one device buffer, typed copies, a per-horizon scatter and owners of
+// per-call device resources.  Host code only, and not included by obca_host.h: the development emulation builds without CUDA headers.
+#pragma once
+#include <cuda_runtime.h>
+#include <string.h>
+
+#include <string>
+#include <vector>
+
+#include "../../include/obca.h"
+
+void obca_set_last_error(const std::string& s);      // obca_lib.cu: the text of obca_last_error()
+
+// A failed CUDA call records "<call>: <CUDA error>" for obca_last_error() and returns OBCA_ERR_CUDA from the enclosing function.
+#define CK(call)                                                                                   \
+  do {                                                                                               \
+    cudaError_t e_ = (call);                                                                         \
+    if (e_ != cudaSuccess) {                                                                         \
+      obca_set_last_error(std::string(#call) + ": " + cudaGetErrorString(e_));                       \
+      return OBCA_ERR_CUDA;                                                                          \
+    }                                                                                                \
+  } while (0)
+
+namespace obca {
+
+// A CUDA device must be visible and dev one of them; argument errors are reported before this check.
+inline int check_device(int dev) {
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) { obca_set_last_error("no CUDA device visible"); return OBCA_ERR_NO_DEVICE; }
+  if (dev < 0 || dev >= n) { obca_set_last_error("bad device ordinal"); return OBCA_ERR_ARG; }
+  return 0;
+}
+
+// Typed arrays in one device buffer, each at a 256-byte boundary, and their host counterparts.  Recording an array grows `bytes`, so the
+// size of a buffer is the sum of what is carved from it; place(base) then points every recorded pointer into a buffer of that size.
+//   add(d, n)       device only
+//   in(d, h, n)     copied from h to the device by copy_in()
+//   out(d, h, n)    copied from the device to h by copy_out()
+//   inout(d, h, n)  both
+// copy_in() and copy_out() issue their copies in the order the arrays were recorded, with n * sizeof(T) bytes each; a null host pointer
+// (an optional input or output the caller did not pass) skips that copy.
+class DevLayout {
+ public:
+  size_t bytes = 0;
+  template <class T>
+  void add(T*& d, size_t n) { record(d, n, nullptr, nullptr); }
+  template <class T>
+  void in(T*& d, const T* h, size_t n) { record(d, n, h, nullptr); }
+  template <class T>
+  void out(T*& d, T* h, size_t n) { record(d, n, nullptr, h); }
+  template <class T>
+  void inout(T*& d, T* h, size_t n) { record(d, n, h, h); }
+  static size_t padded(size_t b) { return (b + 255) / 256 * 256; }
+  void place(void* base) {
+    base_ = (char*)base;
+    for (const Part& q : parts_) q.set(q.slot, base_ + q.off);
+  }
+  cudaError_t copy_in(cudaStream_t st) const {
+    for (const Part& q : parts_)
+      if (q.src && q.n) {
+        const cudaError_t e = cudaMemcpyAsync(base_ + q.off, q.src, q.n, cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) return e;
+      }
+    return cudaSuccess;
+  }
+  cudaError_t copy_out(cudaStream_t st) const {
+    for (const Part& q : parts_)
+      if (q.dst && q.n) {
+        const cudaError_t e = cudaMemcpyAsync(q.dst, base_ + q.off, q.n, cudaMemcpyDeviceToHost, st);
+        if (e != cudaSuccess) return e;
+      }
+    return cudaSuccess;
+  }
+  // the address of the recorded array d in a host copy of the placed buffer
+  template <class T>
+  const T* in_copy(const T* d, const void* copy) const { return (const T*)((const char*)copy + ((const char*)d - base_)); }
+
+ private:
+  struct Part {
+    void* slot;
+    void (*set)(void*, char*);
+    size_t off, n;      // bytes
+    const void* src;
+    void* dst;
+  };
+  template <class T>
+  static void set(void* slot, char* at) { *(T**)slot = (T*)at; }
+  template <class T>
+  void record(T*& d, size_t n, const void* src, void* dst) {
+    parts_.push_back({&d, &set<T>, bytes, n * sizeof(T), src, dst});
+    bytes += padded(n * sizeof(T));
+  }
+  std::vector<Part> parts_;
+  char* base_ = nullptr;
+};
+
+// n elements from the device to h on the stream st
+template <class T>
+cudaError_t to_host(T* h, const T* d, size_t n, cudaStream_t st) {
+  return cudaMemcpyAsync(h, d, n * sizeof(T), cudaMemcpyDeviceToHost, st);
+}
+
+// Problem q of a per-problem array with the stride `per` (laid out for the batch's longest horizon) keeps rows * (Nb[q] + ext)
+// entries: only those go from the host scratch src to dst, so the padding past each problem's horizon is never written.  dst null:
+// an optional output the caller did not pass.
+inline void scatter_horizons(double* dst, const double* src, int B, const int* Nb, size_t per, size_t rows, int ext) {
+  if (!dst) return;
+  for (int q = 0; q < B; ++q) memcpy(dst + per * q, src + per * q, rows * (size_t)(Nb[q] + ext) * sizeof(double));
+}
+
+// Owner of a per-call CUDA handle, released on every return path.
+template <class H, cudaError_t (*Release)(H)>
+struct Owned {
+  H h = nullptr;
+  Owned() = default;
+  Owned(const Owned&) = delete;
+  Owned& operator=(const Owned&) = delete;
+  ~Owned() {
+    if (h) Release(h);
+  }
+};
+using DevBuf = Owned<void*, cudaFree>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+
+// a device buffer of the layout's size, with the layout's pointers placed in it
+inline cudaError_t alloc_layout(DevBuf& buf, DevLayout& lay) {
+  const cudaError_t e = cudaMalloc(&buf.h, lay.bytes);
+  if (e == cudaSuccess) lay.place(buf.h);
+  return e;
+}
+
+}  // namespace obca

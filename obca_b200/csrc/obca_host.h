@@ -1,8 +1,9 @@
-// obca_host.h -- host-side helpers shared by the C-ABI (obca_capi.cu) and the development emulation
-// (tests/emul/emul.cpp): building the POD problem description from the reference's argument list and copying a
-// finished solve out of the per-CTA workspace in the reference's (Julia, column-major) output shapes.
+// obca_host.h -- host-side helpers shared by the C-ABI (obca_lib.cu) and the development emulation (tests/emul/): building the
+// POD problem description from the reference's argument list and choosing a parking problem's template variant.
 #pragma once
 #include <string.h>
+
+#include <type_traits>
 
 #include "obca_solver.cuh"
 #include "obca_quad.cuh"
@@ -57,13 +58,18 @@ inline int max_vob(const ParkProblem& P) {
   return m;
 }
 
-template <int VM, bool SDV>
-inline int nfac_of() { return LocalDims<VM, SDV>::NFAC; }
+// The template variant of a parking problem: f(vm, sdv) with vm = std::integral_constant<int, VM> (VM = 2 when no obstacle has more
+// than two half-spaces, else 4) and sdv = std::integral_constant<bool, SDV> (the signed-distance formulation).
+template <class F>
+inline auto with_variant(const ParkProblem& P, F&& f) {
+  using V2 = std::integral_constant<int, 2>;
+  using V4 = std::integral_constant<int, 4>;
+  if (P.signed_dist) return max_vob(P) <= 2 ? f(V2(), std::true_type()) : f(V4(), std::true_type());
+  return max_vob(P) <= 2 ? f(V2(), std::false_type()) : f(V4(), std::false_type());
+}
 
 inline int nfac_for(const ParkProblem& P) {
-  const int vm = max_vob(P) <= 2 ? 2 : 4;
-  if (P.signed_dist) return vm == 2 ? nfac_of<2, true>() : nfac_of<4, true>();
-  return vm == 2 ? nfac_of<2, false>() : nfac_of<4, false>();
+  return with_variant(P, [](auto vm, auto sdv) { return LocalDims<decltype(vm)::value, decltype(sdv)::value>::NFAC; });
 }
 
 }  // namespace obca

@@ -7,6 +7,8 @@
 //   k_dualws<VM>             K2: one thread per (problem, stage, obstacle) micro interior-point solve.
 //   k_check                  K5: ParkingConstraints twin + strict audit, one CTA per problem.
 // There is NO CPU fallback: every compute entry point returns OBCA_ERR_NO_DEVICE without a CUDA device.
+// Host-pointer entries stage their arrays through one device buffer per device (DevCtx::stage), laid out, copied and scattered back
+// with the helpers of obca_devstage.h, which the GPU planners (obca_plan.cu, obca_plan3d.cu) use for their per-call buffers too.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -19,6 +21,7 @@
 
 #include "../../include/obca.h"
 #include "obca_check.cuh"
+#include "obca_devstage.h"
 #include "obca_dualws.cuh"
 #include "obca_eval.cuh"
 #include "obca_host.h"
@@ -238,15 +241,6 @@ static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
 // the GPU planner's translation unit (obca_plan.cu, built without FMA contraction) reports through obca_last_error() as well
 void obca_set_last_error(const std::string& s) { g_err = s; }
-#define CK(call)                                                                                   \
-  do {                                                                                               \
-    cudaError_t e_ = (call);                                                                         \
-    if (e_ != cudaSuccess) {                                                                         \
-      set_err(std::string(#call) + ": " + cudaGetErrorString(e_));                                   \
-      return OBCA_ERR_CUDA;                                                                          \
-    }                                                                                                \
-  } while (0)
-
 struct DevCtx {
   bool init = false;
   cudaStream_t st = nullptr;
@@ -272,13 +266,14 @@ struct DevCtx {
   double last_dualws_s = 0.0, last_solve_s = 0.0;
   std::recursive_mutex mu;
 };
-static DevCtx g_dev[64];
+constexpr int MAX_DEVICES = 64;
+static DevCtx g_dev[MAX_DEVICES];
 static std::mutex g_init_mu;
 
 static int get_ctx(int dev, DevCtx** out) {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) { set_err("no CUDA device visible"); return OBCA_ERR_NO_DEVICE; }
-  if (dev < 0 || dev >= n || dev >= 64) { set_err("bad device ordinal"); return OBCA_ERR_ARG; }
+  const int rc = check_device(dev);
+  if (rc) return rc;
+  if (dev >= MAX_DEVICES) { set_err("bad device ordinal"); return OBCA_ERR_ARG; }
   DevCtx& c = g_dev[dev];
   CK(cudaSetDevice(dev));
   std::lock_guard<std::mutex> lk(g_init_mu);
@@ -298,6 +293,8 @@ static int get_ctx(int dev, DevCtx** out) {
   *out = &c;
   return 0;
 }
+// the context of a device that has run a call (obca_last_*), or null
+static const DevCtx* used_ctx(int dev) { return dev >= 0 && dev < MAX_DEVICES && g_dev[dev].init ? &g_dev[dev] : nullptr; }
 static int ensure(void** p, size_t* have, size_t need) {
   if (*have >= need) return 0;
   if (*p) cudaFree(*p);
@@ -322,20 +319,17 @@ static IpmOpts to_ipm(const obca_opts* o) {
   return r;
 }
 
-template <int VM>
-static int launch_dualws(DevCtx& c, const ParkProblem& P, int B, const int* Nb, const double* rx, const double* ry,
-                         const double* ryaw, double* lp, double* np, double* dd) {
+static int run_dualws(DevCtx& c, const ParkProblem& P, int B, const int* Nb, const double* rx, const double* ry,
+                      const double* ryaw, double* lp, double* np, double* dd) {
   const size_t total = (size_t)B * P.nOb * (P.N + 1);
   const int threads = 128;
   const int blocks = (int)((total + threads - 1) / threads);
-  k_dualws<VM><<<blocks, threads, 0, c.st>>>(P, B, Nb, rx, ry, ryaw, 1e-5, 100, lp, np, dd);
+  with_variant(P, [&](auto vm, auto) {      // the multipliers do not depend on the formulation
+    k_dualws<decltype(vm)::value><<<blocks, threads, 0, c.st>>>(P, B, Nb, rx, ry, ryaw, 1e-5, 100, lp, np, dd);
+    return 0;
+  });
   CK(cudaGetLastError());
   return 0;
-}
-static int run_dualws(DevCtx& c, const ParkProblem& P, int B, const int* Nb, const double* rx, const double* ry,
-                      const double* ryaw, double* lp, double* np, double* dd) {
-  return max_vob(P) <= 2 ? launch_dualws<2>(c, P, B, Nb, rx, ry, ryaw, lp, np, dd)
-                         : launch_dualws<4>(c, P, B, Nb, rx, ry, ryaw, lp, np, dd);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -501,7 +495,6 @@ static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, cons
 }
 
 static int solve_dev_impl(DevCtx& c, const ParkProblem& P, const IpmOpts& O, BatchPtrs bp, double* seconds) {
-  const int vm = max_vob(P) <= 2 ? 2 : 4;
   {  // problem, options and workspace layout -> __constant__ memory (stream-ordered with the kernels below)
     const PkLay Lc = make_layout(P, nfac_for(P));
     CK(cudaMemcpyToSymbolAsync(c_pkP, &P, sizeof(P), 0, cudaMemcpyHostToDevice, c.st));
@@ -529,13 +522,12 @@ static int solve_dev_impl(DevCtx& c, const ParkProblem& P, const IpmOpts& O, Bat
     if (q.Nb) q.Nb += o;
     q.exitflag += o; q.iters += o; q.kkt_err += o;
 #ifdef OBCA_FAST_BUILD   // development builds: only the config-2 instantiation
-    if (!(P.signed_dist && vm == 2)) { set_err("fast build: only <2,true>"); return OBCA_ERR_UNSUPPORTED; }
+    if (!(P.signed_dist && max_vob(P) <= 2)) { set_err("fast build: only <2,true>"); return OBCA_ERR_UNSUPPORTED; }
     rc = launch_phased<2, true>(c, P, O, q, mode);
 #else
     // OBCA_MODE: 0 auto (phase-split rounds for large batches + tail kernel for the stragglers, tail kernel alone for small
     // batches), 1 tail kernel only, 2 rounds only
-    if (P.signed_dist) rc = vm == 2 ? launch_phased<2, true>(c, P, O, q, mode) : launch_phased<4, true>(c, P, O, q, mode);
-    else rc = vm == 2 ? launch_phased<2, false>(c, P, O, q, mode) : launch_phased<4, false>(c, P, O, q, mode);
+    rc = with_variant(P, [&](auto vm, auto sdv) { return launch_phased<decltype(vm)::value, decltype(sdv)::value>(c, P, O, q, mode); });
 #endif
   }
   if (rc) return rc;
@@ -549,16 +541,6 @@ static int solve_dev_impl(DevCtx& c, const ParkProblem& P, const IpmOpts& O, Bat
   CK(cudaEventElapsedTime(&ms_ws, c.ev0, c.evm));
   c.last_solve_s = ms * 1e-3; c.last_dualws_s = ms_ws * 1e-3; c.phase_ms[4] = ms_ws;
   if (seconds) *seconds = ms * 1e-3;
-  return 0;
-}
-
-template <int VM, bool SDV>
-static int launch_eval(DevCtx& c, const ParkProblem& P, int B, const EvalIn& in, const EvalOut& out, int reps) {
-  const size_t total = (size_t)B * (P.N + 1);
-  const int threads = 128;
-  int blocks = (int)((total + threads - 1) / threads);
-  for (int r = 0; r < reps; ++r) k_parking_eval<VM, SDV><<<blocks, threads, 0, c.st>>>(P, B, in, out);
-  CK(cudaGetLastError());
   return 0;
 }
 
@@ -628,78 +610,108 @@ static int parking_solve_dev(int B, int N, const int* Nb, int nOb, const int* vO
   return solve_dev_impl(*c, P, O, bp, solve_seconds);
 }
 
-// Host-pointer parking solve (staged through one device buffer).  Nb (host pointer, optional): per-problem horizons
-// <= N, with every per-problem array laid out for N.
-static int parking_solve_host(int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b,
+// per-problem horizons: Nb[b] in [2, Nmax]
+static int check_horizons(int B, const int* Nb, int Nmax) {
+  if (!Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
+  for (int q = 0; q < B; ++q)
+    if (Nb[q] < 2 || Nb[q] > Nmax) {
+      set_err("Nb[" + std::to_string(q) + "] = " + std::to_string(Nb[q]) + " outside [2, Nmax = " + std::to_string(Nmax) + "]");
+      return OBCA_ERR_ARG;
+    }
+  return 0;
+}
+
+// per-problem sampling times: finite and > 0
+static int check_sampling_times(int B, const double* Tsb) {
+  if (!Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
+  for (int q = 0; q < B; ++q)
+    if (!(std::isfinite(Tsb[q]) && Tsb[q] > 0.0)) {
+      set_err("Tsb[" + std::to_string(q) + "] = " + std::to_string(Tsb[q]) + " is not a finite sampling time > 0");
+      return OBCA_ERR_ARG;
+    }
+  return 0;
+}
+
+// Host-pointer parking solve (staged through one device buffer), behind the uniform and the mixed entries.  Every per-problem array
+// is laid out for the horizon N.  mixed: Nb (host pointer) holds per-problem horizons in [2, N]; otherwise Nb is null.
+static int parking_solve_host(bool mixed, int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b,
                               const double* x0, const double* xF, double Ts, double L, const double* ego,
                               const double* XYbounds, const double* rx, const double* ry, const double* ryaw,
                               const double* xWS, const double* uWS, const double* lWS, const double* nWS,
                               int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
                               double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                               double* solve_seconds) {
+  if (B <= 0 || !vOb || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up || !ts || !lp || !np ||
+      !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
+  int rc = mixed ? check_horizons(B, Nb, N) : 0;
+  if (rc) return rc;
   if (N < 2 || nOb < 1 || nOb > OBCA_MAX_OB) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
   int V = 0;
   for (int j = 0; j < nOb; ++j) V += vOb[j];
   DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
+  rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
-  const size_t NS = N + 1;
-  const size_t n_x0 = 4, n_r = NS, n_xw = 4 * NS, n_uw = 2 * (size_t)N, n_l = V * NS, n_n = 4 * (size_t)nOb * NS, n_s = nOb * NS;
+  // elements per problem
+  const size_t Bs = B, NS = N + 1, n_x = 4 * NS, n_u = 2 * (size_t)N, n_l = V * NS, n_n = 4 * (size_t)nOb * NS, n_s = nOb * NS;
   const bool have_ws = lWS && nWS;
-  // staging layout (doubles): inputs then outputs
-  size_t off = 0;
-  auto take = [&](size_t n) { size_t o = off; off += n * (size_t)B; return o; };
-  const size_t o_x0 = take(n_x0), o_xF = take(n_x0), o_rx = take(n_r), o_ry = take(n_r), o_ryaw = take(n_r);
-  const size_t o_xw = take(n_xw), o_uw = take(n_uw), o_lw = take(n_l), o_nw = take(n_n);
-  const size_t o_xp = take(n_xw), o_up = take(n_uw), o_ts = take(n_r), o_lp = take(n_l), o_np = take(n_n), o_sl = take(n_s);
-  const size_t o_err = take(1);
-  const size_t dbytes = off * sizeof(double);
-  const size_t ibytes = (Nb ? 3 : 2) * (size_t)B * sizeof(int);
+  double *d0, *dF, *drx, *dry, *dryaw, *dxw, *duw, *dlw, *dnw;
+  double *dxp, *dup, *dts, *dlp, *dnp, *dsl, *derr;
+  int *dflag, *diters, *dNb;
+  char* dout;
+  DevLayout outs;      // the per-problem outputs, copied back in one piece when the horizons differ
+  outs.out(dxp, xp, n_x * Bs);
+  outs.out(dup, up, n_u * Bs);
+  outs.out(dts, ts, NS * Bs);
+  outs.out(dlp, lp, n_l * Bs);
+  outs.out(dnp, np, n_n * Bs);
+  outs.out(dsl, sl, n_s * Bs);
+  outs.out(derr, kkt_err, Bs);
+  DevLayout lay;
+  lay.in(d0, x0, 4 * Bs);
+  lay.in(dF, xF, 4 * Bs);
+  lay.in(drx, rx, NS * Bs);
+  lay.in(dry, ry, NS * Bs);
+  lay.in(dryaw, ryaw, NS * Bs);
+  lay.in(dxw, xWS, n_x * Bs);
+  lay.in(duw, uWS, n_u * Bs);
+  lay.in(dlw, have_ws ? lWS : nullptr, n_l * Bs);
+  lay.in(dnw, have_ws ? nWS : nullptr, n_n * Bs);
+  lay.in(dNb, Nb, Bs);
+  lay.add(dout, outs.bytes);
+  lay.out(dflag, exitflag, Bs);
+  lay.out(diters, iters, Bs);
   // one staging buffer per device: the whole call (copies in, solve, copies out) runs under the device lock
   std::lock_guard<std::recursive_mutex> lk(c->mu);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + ibytes);
+  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
   if (rc) return rc;
-  double* d = (double*)c->stage;
-  int* di = (int*)(c->stage + dbytes);
+  lay.place(c->stage);
+  outs.place(dout);
   cudaStream_t st = c->st;
-#define H2D(dst, src, n) CK(cudaMemcpyAsync(d + (dst), (src), (n) * (size_t)B * sizeof(double), cudaMemcpyHostToDevice, st))
-  H2D(o_x0, x0, n_x0); H2D(o_xF, xF, n_x0); H2D(o_rx, rx, n_r); H2D(o_ry, ry, n_r); H2D(o_ryaw, ryaw, n_r);
-  H2D(o_xw, xWS, n_xw); H2D(o_uw, uWS, n_uw);
-  if (have_ws) { H2D(o_lw, lWS, n_l); H2D(o_nw, nWS, n_n); }
-#undef H2D
-  if (Nb) CK(cudaMemcpyAsync(di + 2 * B, Nb, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(lay.copy_in(st));
   obca_opts o2;
   if (opts) o2 = *opts; else obca_default_opts(&o2);
-  rc = parking_solve_dev(B, N, Nb ? di + 2 * B : nullptr, nOb, vOb, A, b, d + o_x0, d + o_xF, Ts, L, ego, XYbounds, d + o_rx,
-                         d + o_ry, d + o_ryaw, d + o_xw, d + o_uw, have_ws ? d + o_lw : nullptr, have_ws ? d + o_nw : nullptr,
-                         fixTime, signed_dist, &o2, d + o_xp, d + o_up, d + o_ts, d + o_lp, d + o_np, d + o_sl, di, di + B,
-                         d + o_err, solve_seconds);
+  rc = parking_solve_dev(B, N, Nb ? dNb : nullptr, nOb, vOb, A, b, d0, dF, Ts, L, ego, XYbounds, drx, dry, dryaw, dxw, duw,
+                         have_ws ? dlw : nullptr, have_ws ? dnw : nullptr, fixTime, signed_dist, &o2, dxp, dup, dts, dlp, dnp, dsl,
+                         dflag, diters, derr, solve_seconds);
   if (rc) return rc;
-  CK(cudaMemcpyAsync(exitflag, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(iters, di + B, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(lay.copy_out(st));
   if (!Nb) {
-#define D2H(dst, src, n) CK(cudaMemcpyAsync((dst), d + (src), (n) * (size_t)B * sizeof(double), cudaMemcpyDeviceToHost, st))
-    D2H(xp, o_xp, n_xw); D2H(up, o_up, n_uw); D2H(ts, o_ts, n_r); D2H(lp, o_lp, n_l); D2H(np, o_np, n_n);
-    if (sl) D2H(sl, o_sl, n_s);
-    D2H(kkt_err, o_err, 1);
-#undef D2H
+    CK(outs.copy_out(st));
     CK(cudaStreamSynchronize(st));
     return 0;
   }
   // per-problem horizons: the outputs come back through a host scratch, and only the entries of each problem's own
   // horizon are copied into the caller's arrays (the padding past it is never written)
-  std::vector<double> h(off - o_xp);
-  CK(cudaMemcpyAsync(h.data(), d + o_xp, h.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  std::vector<double> h(outs.bytes / sizeof(double));
+  CK(to_host((char*)h.data(), dout, outs.bytes, st));
   CK(cudaStreamSynchronize(st));
-  for (int q = 0; q < B; ++q) {
-    const size_t ns = (size_t)Nb[q] + 1, nu = (size_t)Nb[q];
-#define PUT(dst, o_src, per, len) memcpy((dst) + (per) * q, h.data() + ((o_src) - o_xp) + (per) * q, (len) * sizeof(double))
-    PUT(xp, o_xp, n_xw, 4 * ns); PUT(up, o_up, n_uw, 2 * nu); PUT(ts, o_ts, n_r, ns);
-    PUT(lp, o_lp, n_l, (size_t)V * ns); PUT(np, o_np, n_n, 4 * (size_t)nOb * ns);
-    if (sl) PUT(sl, o_sl, n_s, (size_t)nOb * ns);
-#undef PUT
-  }
-  memcpy(kkt_err, h.data() + (o_err - o_xp), (size_t)B * sizeof(double));
+  scatter_horizons(xp, outs.in_copy(dxp, h.data()), B, Nb, n_x, 4, 1);
+  scatter_horizons(up, outs.in_copy(dup, h.data()), B, Nb, n_u, 2, 0);
+  scatter_horizons(ts, outs.in_copy(dts, h.data()), B, Nb, NS, 1, 1);
+  scatter_horizons(lp, outs.in_copy(dlp, h.data()), B, Nb, n_l, V, 1);
+  scatter_horizons(np, outs.in_copy(dnp, h.data()), B, Nb, n_n, 4 * (size_t)nOb, 1);
+  scatter_horizons(sl, outs.in_copy(dsl, h.data()), B, Nb, n_s, nOb, 1);
+  memcpy(kkt_err, outs.in_copy(derr, h.data()), Bs * sizeof(double));
   return 0;
 }
 
@@ -719,40 +731,54 @@ static int check_parking(int B, int N, const int* Nb, int nOb, const int* vOb, c
   int rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
-  const size_t NS = N + 1;
-  const size_t nx = 4 * NS * B, nu = 2 * (size_t)N * B, nl = (size_t)P.V * NS * B, nn = 4 * (size_t)nOb * NS * B, nt = NS * B,
-               ns = (size_t)nOb * NS * B, n0 = 4 * (size_t)B;
-  const size_t dbytes = (2 * n0 + nx + nu + nl + nn + nt + ns) * sizeof(double);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + (Nb ? 10 : 9) * (size_t)B * sizeof(int));
+  const size_t Bs = B, NS = N + 1;
+  const size_t n0 = 4 * Bs, nx = 4 * NS * Bs, nu = 2 * (size_t)N * Bs, nl = (size_t)P.V * NS * Bs, nn = 4 * (size_t)nOb * NS * Bs,
+               nt = NS * Bs, ns = (size_t)nOb * NS * Bs;
+  double *d0, *dF, *dx, *du, *dl, *dn, *dt, *ds;
+  int *dfeas, *de, *dstrict, *dNb;
+  DevLayout lay;
+  lay.in(d0, x0, n0);
+  lay.in(dF, xF, n0);
+  lay.in(dx, x, nx);
+  lay.in(du, u, nu);
+  lay.in(dl, l, nl);
+  lay.in(dn, n, nn);
+  lay.in(dt, timeScale, nt);
+  lay.in(ds, sl, ns);
+  lay.in(dNb, Nb, Bs);
+  lay.out(dfeas, feasible, Bs);
+  lay.out(de, e, 7 * Bs);
+  lay.out(dstrict, strict, Bs);
+  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
   if (rc) return rc;
-  double* d = (double*)c->stage;
-  double *d0 = d, *dF = d0 + n0, *dx = dF + n0, *du = dx + nx, *dl = du + nu, *dn = dl + nl, *dt = dn + nn, *ds = dt + nt;
-  int* di = (int*)(c->stage + dbytes);
+  lay.place(c->stage);
   cudaStream_t st = c->st;
-  CK(cudaMemcpyAsync(d0, x0, n0 * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dF, xF, n0 * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dx, x, nx * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(du, u, nu * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dl, l, nl * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dn, n, nn * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dt, timeScale, nt * 8, cudaMemcpyHostToDevice, st));
-  if (sl) CK(cudaMemcpyAsync(ds, sl, ns * 8, cudaMemcpyHostToDevice, st));
-  if (Nb) CK(cudaMemcpyAsync(di + 9 * (size_t)B, Nb, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(lay.copy_in(st));
   const int grid = B < 4 * c->sms ? B : 4 * c->sms;
-  k_check<<<grid, 128, 0, st>>>(P, B, Nb ? di + 9 * (size_t)B : nullptr, d0, dF, dx, du, dl, dn, dt, sl ? ds : nullptr, sd, di, di + B, di + 8 * (size_t)B);
+  k_check<<<grid, 128, 0, st>>>(P, B, Nb ? dNb : nullptr, d0, dF, dx, du, dl, dn, dt, sl ? ds : nullptr, sd, dfeas, de, dstrict);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(feasible, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (e) CK(cudaMemcpyAsync(e, di + B, 7 * (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (strict) CK(cudaMemcpyAsync(strict, di + 8 * (size_t)B, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(lay.copy_out(st));
   CK(cudaStreamSynchronize(st));
   return 0;
 }
 
 
 // The quadcopter solve behind the uniform and the mixed entries (host pointers, staged through one device buffer).  Every
-// per-problem array is laid out for the horizon N.  Nb, Tsb (host pointers, optional, together): per-problem horizons <= N
-// and sampling times; problem b uses the first Nb[b] + 1 stages of its arrays and nothing past them is written.
-static int quad_solve_host(int B, int N, const int* Nb, const double* Tsb, const double* x0, const double* xF, double Ts,
+// per-problem array is laid out for the horizon N.  mixed: Nb, Tsb (host pointers) hold per-problem horizons in [2, N] and sampling
+// times; problem b uses the first Nb[b] + 1 stages of its arrays and nothing past them is written.  Otherwise Nb and Tsb are null.
+static int quad_solve_host(bool mixed, int B, int N, const int* Nb, const double* Tsb, const double* x0, const double* xF, double Ts,
                            double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
                            const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
                            int* exitflag, int* iters, double* kkt_err, double* solve_seconds) {
+  if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
+    set_err("null argument"); return OBCA_ERR_ARG;
+  }
+  if (mixed) {
+    int rc = check_horizons(B, Nb, N);
+    if (rc) return rc;
+    rc = check_sampling_times(B, Tsb);
+    if (rc) return rc;
+  }
   QuadProblem P;
   if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
   if (N > QUAD_NMAX) {      // before any device work: nothing is launched and no output is written
@@ -766,61 +792,63 @@ static int quad_solve_host(int B, int N, const int* Nb, const double* Tsb, const
   std::lock_guard<std::recursive_mutex> lk(c->mu);
   IpmOpts O = to_ipm(opts);
   if (!opts) O.max_iter = 3000;                        // the reference sets no max_iter here (Ipopt default)
-  const size_t NS = N + 1;
-  const size_t n0 = 12 * (size_t)B, nx = 12 * NS * B, nu = 4 * (size_t)N * B, nt = NS * B, nl = 30 * NS * B, ns = 5 * NS * B;
-  const size_t dbytes = (2 * n0 + 2 * nx + nu + nt + nl + ns + B + (Nb ? B : 0)) * sizeof(double);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + (Nb ? 3 : 2) * (size_t)B * sizeof(int));
+  // elements per problem
+  const size_t Bs = B, NS = N + 1, n_x = 12 * NS, n_u = 4 * (size_t)N, n_l = 30 * NS, n_s = 5 * NS;
+  double *d0, *dF, *dW, *dTs;
+  double *dxp, *dup, *dts, *dlp, *dsl, *derr;
+  int *dflag, *diters, *dNb;
+  char* dout;
+  double* slack_out = signed_dist ? slack : nullptr;      // the Dist formulation has no slacks
+  DevLayout outs;      // the per-problem outputs, copied back in one piece when the horizons differ
+  outs.out(dxp, xp, n_x * Bs);
+  outs.out(dup, up, n_u * Bs);
+  outs.out(dts, ts, NS * Bs);
+  outs.out(dlp, lp, n_l * Bs);
+  outs.out(dsl, slack_out, n_s * Bs);
+  outs.out(derr, kkt_err, Bs);
+  DevLayout lay;
+  lay.in(d0, x0, 12 * Bs);
+  lay.in(dF, xF, 12 * Bs);
+  lay.in(dW, xWS, n_x * Bs);
+  lay.in(dNb, Nb, Bs);
+  lay.in(dTs, Tsb, Bs);
+  lay.add(dout, outs.bytes);
+  lay.out(dflag, exitflag, Bs);
+  lay.out(diters, iters, Bs);
+  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
   if (rc) return rc;
-  double* d = (double*)c->stage;
-  double *d0 = d, *dF = d0 + n0, *dW = dF + n0, *dxp = dW + nx, *dup = dxp + nx, *dts = dup + nu, *dlp = dts + nt, *dsl = dlp + nl,
-         *derr = dsl + ns, *dTs = derr + B;
-  int* di = (int*)(c->stage + dbytes);
+  lay.place(c->stage);
+  outs.place(dout);
   cudaStream_t st = c->st;
-  CK(cudaMemcpyAsync(d0, x0, n0 * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dF, xF, n0 * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dW, xWS, nx * 8, cudaMemcpyHostToDevice, st));
-  if (Nb) {
-    CK(cudaMemcpyAsync(di + 2 * (size_t)B, Nb, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dTs, Tsb, (size_t)B * 8, cudaMemcpyHostToDevice, st));
-  }
+  CK(lay.copy_in(st));
   QBatchPtrs bp;
-  bp.x0 = d0; bp.xF = dF; bp.xWS = dW; bp.Nb = Nb ? di + 2 * (size_t)B : nullptr; bp.Tsb = Nb ? dTs : nullptr;
+  bp.x0 = d0; bp.xF = dF; bp.xWS = dW; bp.Nb = Nb ? dNb : nullptr; bp.Tsb = Nb ? dTs : nullptr;
   bp.timeWS = timeWS; bp.xp = dxp; bp.up = dup; bp.ts = dts; bp.lp = dlp; bp.slack = dsl;
-  bp.exitflag = di; bp.iters = di + B; bp.kkt_err = derr; bp.B = B; bp.prof = c->prof;
+  bp.exitflag = dflag; bp.iters = diters; bp.kkt_err = derr; bp.B = B; bp.prof = c->prof;
   CK(cudaMemsetAsync(c->prof, 0, 8 * sizeof(unsigned long long), st));
   CK(cudaEventRecord(c->ev0, st));
   rc = signed_dist ? launch_quad<true>(*c, P, O, bp) : launch_quad<false>(*c, P, O, bp);
   if (rc) return rc;
   CK(cudaEventRecord(c->ev1, st));
-  if (!Nb) {
-    CK(cudaMemcpyAsync(xp, dxp, nx * 8, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(up, dup, nu * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ts, dts, nt * 8, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(lp, dlp, nl * 8, cudaMemcpyDeviceToHost, st));
-    if (slack && signed_dist) CK(cudaMemcpyAsync(slack, dsl, ns * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(kkt_err, derr, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaMemcpyAsync(exitflag, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(iters, di + B, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(c->prof_host, c->prof, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  if (!Nb) CK(outs.copy_out(st));
+  CK(lay.copy_out(st));
+  CK(to_host(c->prof_host, c->prof, 8, st));
   std::vector<double> h;
   if (Nb) {     // the outputs come back through a host scratch; only each problem's own horizon goes to the caller's arrays
-    h.resize(nx + nu + nt + nl + ns + B);
-    CK(cudaMemcpyAsync(h.data(), dxp, h.size() * 8, cudaMemcpyDeviceToHost, st));
+    h.resize(outs.bytes / sizeof(double));
+    CK(to_host((char*)h.data(), dout, outs.bytes, st));
   }
   CK(cudaStreamSynchronize(st));
   float ms = 0.f;
   CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
   if (solve_seconds) *solve_seconds = ms * 1e-3;
   if (Nb) {
-    const double *hx = h.data(), *hu = hx + nx, *ht = hu + nu, *hl = ht + nt, *hs = hl + nl, *he = hs + ns;
-    for (int q = 0; q < B; ++q) {
-      const size_t nsq = (size_t)Nb[q] + 1, nuq = (size_t)Nb[q];
-      memcpy(xp + 12 * NS * q, hx + 12 * NS * q, 12 * nsq * 8);
-      memcpy(up + 4 * (size_t)N * q, hu + 4 * (size_t)N * q, 4 * nuq * 8);
-      memcpy(ts + NS * q, ht + NS * q, nsq * 8);
-      memcpy(lp + 30 * NS * q, hl + 30 * NS * q, 30 * nsq * 8);
-      if (slack && signed_dist) memcpy(slack + 5 * NS * q, hs + 5 * NS * q, 5 * nsq * 8);
-    }
-    memcpy(kkt_err, he, (size_t)B * 8);
+    scatter_horizons(xp, outs.in_copy(dxp, h.data()), B, Nb, n_x, 12, 1);
+    scatter_horizons(up, outs.in_copy(dup, h.data()), B, Nb, n_u, 4, 0);
+    scatter_horizons(ts, outs.in_copy(dts, h.data()), B, Nb, NS, 1, 1);
+    scatter_horizons(lp, outs.in_copy(dlp, h.data()), B, Nb, n_l, 30, 1);
+    scatter_horizons(slack_out, outs.in_copy(dsl, h.data()), B, Nb, n_s, 5, 1);
+    memcpy(kkt_err, outs.in_copy(derr, h.data()), Bs * sizeof(double));
   }
   return 0;
 }
@@ -837,27 +865,30 @@ static int quad_check_host(int B, int N, const int* Nb, const double* Tsb, const
   int rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
-  const size_t NS = N + 1;
-  const size_t n0 = 12 * (size_t)B, nx = 12 * NS * B, nu = 4 * (size_t)N * B, nt = NS * B, nl = 30 * NS * B;
-  const size_t dbytes = (2 * n0 + nx + nu + nt + nl + B + (Nb ? B : 0)) * sizeof(double);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, dbytes + (Nb ? 2 : 1) * (size_t)B * sizeof(int));
+  const size_t Bs = B, NS = N + 1;
+  const size_t n0 = 12 * Bs, nx = 12 * NS * Bs, nu = 4 * (size_t)N * Bs, nt = NS * Bs, nl = 30 * NS * Bs;
+  double *d0, *dF, *dx, *du, *dt, *dl, *dw, *dTs;
+  int *dfeas, *dNb;
+  DevLayout lay;
+  lay.in(d0, x0, n0);
+  lay.in(dF, xF, n0);
+  lay.in(dx, x, nx);
+  lay.in(du, u, nu);
+  lay.in(dt, timeScale, nt);
+  lay.in(dl, lambda, nl);
+  lay.in(dNb, Nb, Bs);
+  lay.in(dTs, Tsb, Bs);
+  lay.out(dfeas, feasible, Bs);
+  lay.out(dw, worst, Bs);
+  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
   if (rc) return rc;
-  double* d = (double*)c->stage;
-  double *d0 = d, *dF = d0 + n0, *dx = dF + n0, *du = dx + nx, *dt = du + nu, *dl = dt + nt, *dw = dl + nl, *dTs = dw + B;
-  int* di = (int*)(c->stage + dbytes);
+  lay.place(c->stage);
   cudaStream_t st = c->st;
-  CK(cudaMemcpyAsync(d0, x0, n0 * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dF, xF, n0 * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dx, x, nx * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(du, u, nu * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dt, timeScale, nt * 8, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(dl, lambda, nl * 8, cudaMemcpyHostToDevice, st));
-  if (Nb) {
-    CK(cudaMemcpyAsync(di + B, Nb, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dTs, Tsb, (size_t)B * 8, cudaMemcpyHostToDevice, st));
-  }
+  CK(lay.copy_in(st));
   const int grid = B < 4 * c->sms ? B : 4 * c->sms;
-  k_quad_check<<<grid, 128, 0, st>>>(P, B, Nb ? di + B : nullptr, Nb ? dTs : nullptr, d0, dF, dx, du, dt, dl, di, dw);
+  k_quad_check<<<grid, 128, 0, st>>>(P, B, Nb ? dNb : nullptr, Nb ? dTs : nullptr, d0, dF, dx, du, dt, dl, dfeas, dw);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(feasible, di, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (worst) CK(cudaMemcpyAsync(worst, dw, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
+  CK(lay.copy_out(st));
   CK(cudaStreamSynchronize(st));
   return 0;
 }
@@ -911,32 +942,8 @@ int obca_parking_solve_batch(int B, int N, int nOb, const int* vOb, const double
                              int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
                              double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                              double* solve_seconds) {
-  if (B <= 0 || !vOb || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up || !ts || !lp || !np ||
-      !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
-  return parking_solve_host(B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS,
+  return parking_solve_host(false, B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS,
                             fixTime, signed_dist, opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds);
-}
-
-// per-problem horizons: Nb[b] in [2, Nmax]
-static int check_horizons(int B, const int* Nb, int Nmax) {
-  if (!Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
-  for (int q = 0; q < B; ++q)
-    if (Nb[q] < 2 || Nb[q] > Nmax) {
-      set_err("Nb[" + std::to_string(q) + "] = " + std::to_string(Nb[q]) + " outside [2, Nmax = " + std::to_string(Nmax) + "]");
-      return OBCA_ERR_ARG;
-    }
-  return 0;
-}
-
-// per-problem sampling times: finite and > 0
-static int check_sampling_times(int B, const double* Tsb) {
-  if (!Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
-  for (int q = 0; q < B; ++q)
-    if (!(std::isfinite(Tsb[q]) && Tsb[q] > 0.0)) {
-      set_err("Tsb[" + std::to_string(q) + "] = " + std::to_string(Tsb[q]) + " is not a finite sampling time > 0");
-      return OBCA_ERR_ARG;
-    }
-  return 0;
 }
 
 int obca_parking_solve_mixed(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
@@ -946,11 +953,7 @@ int obca_parking_solve_mixed(int B, const int* Nb, int Nmax, int nOb, const int*
                              int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
                              double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                              double* solve_seconds) {
-  if (B <= 0 || !vOb || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up || !ts || !lp || !np ||
-      !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
-  const int rc = check_horizons(B, Nb, Nmax);
-  if (rc) return rc;
-  return parking_solve_host(B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS,
+  return parking_solve_host(true, B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS,
                             fixTime, signed_dist, opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds);
 }
 
@@ -966,18 +969,21 @@ int obca_dualmultws_batch(int B, int N, int nOb, const int* vOb, const double* A
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
   const size_t NS = N + 1, nr = NS * B, nl = (size_t)P.V * NS * B, nn = 4 * (size_t)nOb * NS * B, ndd = (size_t)nOb * NS * B;
-  rc = ensure((void**)&c->stage, &c->stage_bytes, (3 * nr + nl + nn + ndd) * sizeof(double));
+  double *drx, *dry, *dryaw, *dl, *dn, *ddv;
+  DevLayout lay;
+  lay.in(drx, rx, nr);
+  lay.in(dry, ry, nr);
+  lay.in(dryaw, ryaw, nr);
+  lay.out(dl, lp, nl);
+  lay.out(dn, np, nn);
+  lay.out(ddv, dd, ndd);
+  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
   if (rc) return rc;
-  double* d = (double*)c->stage;
-  CK(cudaMemcpyAsync(d, rx, nr * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  CK(cudaMemcpyAsync(d + nr, ry, nr * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  CK(cudaMemcpyAsync(d + 2 * nr, ryaw, nr * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  double* dl = d + 3 * nr; double* dn = dl + nl; double* ddv = dn + nn;
-  rc = run_dualws(*c, P, B, nullptr, d, d + nr, d + 2 * nr, dl, dn, ddv);
+  lay.place(c->stage);
+  CK(lay.copy_in(c->st));
+  rc = run_dualws(*c, P, B, nullptr, drx, dry, dryaw, dl, dn, ddv);
   if (rc) return rc;
-  CK(cudaMemcpyAsync(lp, dl, nl * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  CK(cudaMemcpyAsync(np, dn, nn * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  if (dd) CK(cudaMemcpyAsync(dd, ddv, ndd * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  CK(lay.copy_out(c->st));
   CK(cudaStreamSynchronize(c->st));
   return 0;
 }
@@ -1006,10 +1012,7 @@ int obca_quadcopter_solve_batch(int B, int N, const double* x0, const double* xF
                                 const double* xWS, double timeWS, int signed_dist, const obca_opts* opts, double* xp,
                                 double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters,
                                 double* kkt_err, double* solve_seconds) {
-  if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
-    set_err("null argument"); return OBCA_ERR_ARG;
-  }
-  return quad_solve_host(B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
+  return quad_solve_host(false, B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
                          exitflag, iters, kkt_err, solve_seconds);
 }
 
@@ -1017,15 +1020,8 @@ int obca_quadcopter_solve_mixed(int B, const int* Nb, int Nmax, const double* x0
                                 double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
                                 const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
                                 int* exitflag, int* iters, double* kkt_err, double* solve_seconds) {
-  if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
-    set_err("null argument"); return OBCA_ERR_ARG;
-  }
-  int rc = check_horizons(B, Nb, Nmax);
-  if (rc) return rc;
-  rc = check_sampling_times(B, Tsb);
-  if (rc) return rc;
   // the batch has no sampling time of its own: NaN, so that a read of it instead of Tsb[b] could not go unnoticed
-  return quad_solve_host(B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
+  return quad_solve_host(true, B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
                          exitflag, iters, kkt_err, solve_seconds);
 }
 
@@ -1046,23 +1042,26 @@ int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x,
 }
 
 int obca_last_profile(int device, unsigned long long* out8) {
-  if (device < 0 || device >= 64 || !out8 || !g_dev[device].init) { set_err("no profile"); return OBCA_ERR_ARG; }
-  for (int i = 0; i < 8; ++i) out8[i] = g_dev[device].prof_host[i];
+  const DevCtx* c = used_ctx(device);
+  if (!c || !out8) { set_err("no profile"); return OBCA_ERR_ARG; }
+  for (int i = 0; i < 8; ++i) out8[i] = c->prof_host[i];
   return 0;
 }
 
 int obca_last_schedule(int device, int* rounds, int* handed_over, double* kernel_ms5) {
-  if (device < 0 || device >= 64 || !g_dev[device].init) { set_err("no schedule"); return OBCA_ERR_ARG; }
-  if (rounds) *rounds = g_dev[device].last_rounds;
-  if (handed_over) *handed_over = g_dev[device].last_tail;
-  if (kernel_ms5) for (int i = 0; i < 5; ++i) kernel_ms5[i] = g_dev[device].phase_ms[i];
+  const DevCtx* c = used_ctx(device);
+  if (!c) { set_err("no schedule"); return OBCA_ERR_ARG; }
+  if (rounds) *rounds = c->last_rounds;
+  if (handed_over) *handed_over = c->last_tail;
+  if (kernel_ms5) for (int i = 0; i < 5; ++i) kernel_ms5[i] = c->phase_ms[i];
   return 0;
 }
 
 int obca_last_times(int device, double* dualws_seconds, double* solve_seconds) {
-  if (device < 0 || device >= 64 || !g_dev[device].init) { set_err("no solve yet"); return OBCA_ERR_ARG; }
-  if (dualws_seconds) *dualws_seconds = g_dev[device].last_dualws_s;
-  if (solve_seconds) *solve_seconds = g_dev[device].last_solve_s;
+  const DevCtx* c = used_ctx(device);
+  if (!c) { set_err("no solve yet"); return OBCA_ERR_ARG; }
+  if (dualws_seconds) *dualws_seconds = c->last_dualws_s;
+  if (solve_seconds) *solve_seconds = c->last_solve_s;
   return 0;
 }
 
@@ -1094,11 +1093,15 @@ int obca_parking_eval_batch_dev(int B, int N, int nOb, const int* vOb, const dou
   in.np = np; in.sl = sl; in.y = y;
   EvalOut out; out.c = c_out; out.gradL = gradL_out; out.fk = fk_out;
   if (reps < 1) reps = 1;
-  const int vm = max_vob(P) <= 2 ? 2 : 4;
+  const size_t total = (size_t)B * (P.N + 1);
+  const int threads = 128;
+  const int blocks = (int)((total + threads - 1) / threads);
   CK(cudaEventRecord(c->ev0, c->st));
-  if (P.signed_dist) rc = vm == 2 ? launch_eval<2, true>(*c, P, B, in, out, reps) : launch_eval<4, true>(*c, P, B, in, out, reps);
-  else rc = vm == 2 ? launch_eval<2, false>(*c, P, B, in, out, reps) : launch_eval<4, false>(*c, P, B, in, out, reps);
-  if (rc) return rc;
+  with_variant(P, [&](auto vm, auto sdv) {
+    for (int r = 0; r < reps; ++r) k_parking_eval<decltype(vm)::value, decltype(sdv)::value><<<blocks, threads, 0, c->st>>>(P, B, in, out);
+    return 0;
+  });
+  CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
   CK(cudaStreamSynchronize(c->st));
   float ms = 0.f;

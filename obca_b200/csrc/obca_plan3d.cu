@@ -14,11 +14,12 @@
 #include "../../include/obca.h"
 #include "../../include/obca_planner.h"
 #include "../planner/csrc/obca_astar3d_core.h"
+#include "obca_devstage.h"
 
-void obca_set_last_error(const std::string& s);      // obca_lib.cu
 static_assert(obca_astar3d::A3_POOL_FULL == OBCA_PLAN_POOL_FULL, "status code of a full node pool or queue");
 static_assert(obca_astar3d::A3_CAPACITY == OBCA_PLAN_CAPACITY && obca_astar3d::A3_NO_PATH == OBCA_PLAN_NO_PATH, "status codes");
 
+using namespace obca;
 using namespace obca_astar3d;
 
 namespace {
@@ -61,24 +62,6 @@ __global__ void __launch_bounds__(P3_WARPS * 32) k_plan3d(int B, A3Const C, A3IO
   }
 }
 
-#define PCK(call)                                                                    \
-  do {                                                                               \
-    cudaError_t e_ = (call);                                                         \
-    if (e_ != cudaSuccess) {                                                         \
-      obca_set_last_error(std::string(#call) + ": " + cudaGetErrorString(e_));       \
-      rc = OBCA_ERR_CUDA;                                                            \
-      goto done;                                                                     \
-    }                                                                                \
-  } while (0)
-
-template <class T>
-T* carve(char*& p, size_t n) {
-  T* r = (T*)p;
-  p += (n * sizeof(T) + 255) / 256 * 256;
-  return r;
-}
-size_t padded(size_t bytes) { return (bytes + 255) / 256 * 256; }
-
 }  // namespace
 
 extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy,
@@ -92,10 +75,9 @@ extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, con
     std::string why;
     if (astar3d_setup(S, why, B, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, cap)) { obca_set_last_error(why); return OBCA_ERR_ARG; }
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { obca_set_last_error("no CUDA device visible"); return OBCA_ERR_NO_DEVICE; }
   const int dev = opts ? opts->device : 0;
-  if (dev < 0 || dev >= ndev) { obca_set_last_error("bad device ordinal"); return OBCA_ERR_ARG; }
+  const int rc = check_device(dev);
+  if (rc) return rc;
   if (plan_seconds) *plan_seconds = 0.0;
   if (B == 0) return 0;
   if (max_nodes <= 0) max_nodes = P3_DEFAULT_NODES;
@@ -103,72 +85,63 @@ extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, con
   C.max_nodes = max_nodes;
   C.max_queue = max_nodes / 4 > 64 ? max_nodes / 4 : 64;
 
-  int rc = 0, sms = 0;
-  cudaStream_t st = nullptr;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  char *dconst = nullptr, *dscr = nullptr, *dio = nullptr;
-  {
-    PCK(cudaSetDevice(dev));
-    PCK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PCK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    PCK(cudaEventCreate(&e0)); PCK(cudaEventCreate(&e1));
-    const int grid = (B + P3_WARPS - 1) / P3_WARPS < sms ? (B + P3_WARPS - 1) / P3_WARPS : sms;
-    const size_t nw = (size_t)grid * P3_WARPS, nmap = S.map.size(), Bs = (size_t)B;
-    // batch constants: the obstacle bitmap, the pairs' cells, the counter
-    PCK(cudaMalloc(&dconst, padded(nmap * 4) + 2 * padded(3 * Bs * 8) + 256));
-    char* q = dconst;
-    uint32_t* dmap = carve<uint32_t>(q, nmap);
-    long long* ds = carve<long long>(q, 3 * Bs);
-    long long* dg = carve<long long>(q, 3 * Bs);
-    int* dcounter = carve<int>(q, 1);
-    PCK(cudaMemcpyAsync(dmap, S.map.data(), nmap * 4, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemcpyAsync(ds, S.s.data(), 3 * Bs * 8, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemcpyAsync(dg, S.g.data(), 3 * Bs * 8, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemsetAsync(dcounter, 0, sizeof(int), st));
-    C.map = dmap;
-    // per warp: cell table, node pool, queue
-    const size_t table_stride = padded((size_t)(S.cells > 0 ? S.cells : 1) * 4) / 4;
-    PCK(cudaMalloc(&dscr, padded(table_stride * 4 * nw) + padded(sizeof(A3Node) * C.max_nodes * nw) +
-                              padded(sizeof(A3Item) * C.max_queue * nw)));
-    q = dscr;
-    A3Scratch W0;
-    W0.table = carve<int>(q, table_stride * nw);
-    W0.pool = carve<A3Node>(q, (size_t)C.max_nodes * nw);
-    W0.queue = carve<A3Item>(q, (size_t)C.max_queue * nw);
-    PCK(cudaMemsetAsync(W0.table, 0xff, table_stride * 4 * nw, st));      // -1: no node
-    // outputs: copied in first, so that the kernel leaves every entry it does not write as the caller had it
-    const size_t cb = Bs * cap;
-    PCK(cudaMalloc(&dio, 3 * padded(cb * 8) + 3 * padded(Bs * 4)));
-    q = dio;
-    double* drx = carve<double>(q, cb); double* dry = carve<double>(q, cb); double* drz = carve<double>(q, cb);
-    int* dN = carve<int>(q, Bs); int* dst = carve<int>(q, Bs); int* dex = carve<int>(q, Bs);
-    PCK(cudaMemcpyAsync(drx, rx, cb * 8, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemcpyAsync(dry, ry, cb * 8, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemcpyAsync(drz, rz, cb * 8, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemcpyAsync(dN, N, Bs * 4, cudaMemcpyHostToDevice, st));
-    if (expansions) PCK(cudaMemcpyAsync(dex, expansions, Bs * 4, cudaMemcpyHostToDevice, st));
-    const A3IO io{ds, dg, drx, dry, drz, dN, dst, expansions ? dex : nullptr, nullptr, nullptr};
-    PCK(cudaEventRecord(e0, st));
-    k_plan3d<<<grid, P3_WARPS * 32, 0, st>>>(B, C, io, W0, table_stride, dcounter);
-    PCK(cudaGetLastError());
-    PCK(cudaEventRecord(e1, st));
-    PCK(cudaMemcpyAsync(rx, drx, cb * 8, cudaMemcpyDeviceToHost, st));
-    PCK(cudaMemcpyAsync(ry, dry, cb * 8, cudaMemcpyDeviceToHost, st));
-    PCK(cudaMemcpyAsync(rz, drz, cb * 8, cudaMemcpyDeviceToHost, st));
-    PCK(cudaMemcpyAsync(N, dN, Bs * 4, cudaMemcpyDeviceToHost, st));
-    PCK(cudaMemcpyAsync(status, dst, Bs * 4, cudaMemcpyDeviceToHost, st));
-    if (expansions) PCK(cudaMemcpyAsync(expansions, dex, Bs * 4, cudaMemcpyDeviceToHost, st));
-    PCK(cudaStreamSynchronize(st));
-    float ms = 0.f;
-    PCK(cudaEventElapsedTime(&ms, e0, e1));
-    if (plan_seconds) *plan_seconds = ms * 1e-3;
-  }
-done:
-  if (dio) cudaFree(dio);
-  if (dscr) cudaFree(dscr);
-  if (dconst) cudaFree(dconst);
-  if (e0) cudaEventDestroy(e0);
-  if (e1) cudaEventDestroy(e1);
-  if (st) cudaStreamDestroy(st);
-  return rc;
+  int sms = 0;
+  Stream st;
+  Event e0, e1;
+  CK(cudaSetDevice(dev));
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CK(cudaStreamCreateWithFlags(&st.h, cudaStreamNonBlocking));
+  CK(cudaEventCreate(&e0.h));
+  CK(cudaEventCreate(&e1.h));
+  const int grid = (B + P3_WARPS - 1) / P3_WARPS < sms ? (B + P3_WARPS - 1) / P3_WARPS : sms;
+  const size_t nw = (size_t)grid * P3_WARPS, nmap = S.map.size(), Bs = (size_t)B;
+  // batch constants: the obstacle bitmap, the pairs' cells, the counter
+  uint32_t* dmap;
+  long long *ds, *dg;
+  int* dcounter;
+  DevLayout cl;
+  cl.in(dmap, S.map.data(), nmap);
+  cl.in(ds, S.s.data(), 3 * Bs);
+  cl.in(dg, S.g.data(), 3 * Bs);
+  cl.add(dcounter, 1);
+  DevBuf dconst;
+  CK(alloc_layout(dconst, cl));
+  CK(cl.copy_in(st.h));
+  CK(cudaMemsetAsync(dcounter, 0, sizeof(int), st.h));
+  C.map = dmap;
+  // per warp: cell table, node pool, queue
+  const size_t table_stride = DevLayout::padded((size_t)(S.cells > 0 ? S.cells : 1) * sizeof(int)) / sizeof(int);
+  A3Scratch W0;
+  DevLayout wl;
+  wl.add(W0.table, table_stride * nw);
+  wl.add(W0.pool, (size_t)C.max_nodes * nw);
+  wl.add(W0.queue, (size_t)C.max_queue * nw);
+  DevBuf dscr;
+  CK(alloc_layout(dscr, wl));
+  CK(cudaMemsetAsync(W0.table, 0xff, table_stride * nw * sizeof(int), st.h));      // -1: no node
+  // outputs: copied in first, so that the kernel leaves every entry it does not write as the caller had it
+  const size_t cb = Bs * cap;
+  double *drx, *dry, *drz;
+  int *dN, *dst, *dex;
+  DevLayout il;
+  il.inout(drx, rx, cb);
+  il.inout(dry, ry, cb);
+  il.inout(drz, rz, cb);
+  il.inout(dN, N, Bs);
+  il.out(dst, status, Bs);
+  il.inout(dex, expansions, Bs);
+  DevBuf dio;
+  CK(alloc_layout(dio, il));
+  CK(il.copy_in(st.h));
+  const A3IO io{ds, dg, drx, dry, drz, dN, dst, expansions ? dex : nullptr, nullptr, nullptr};
+  CK(cudaEventRecord(e0.h, st.h));
+  k_plan3d<<<grid, P3_WARPS * 32, 0, st.h>>>(B, C, io, W0, table_stride, dcounter);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e1.h, st.h));
+  CK(il.copy_out(st.h));
+  CK(cudaStreamSynchronize(st.h));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e0.h, e1.h));
+  if (plan_seconds) *plan_seconds = ms * 1e-3;
+  return 0;
 }
