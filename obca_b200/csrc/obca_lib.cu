@@ -183,7 +183,7 @@ k_quad_solve(const __grid_constant__ QuadProblem P, const __grid_constant__ IpmO
     QOutputs out;
     out.xp = bp.xp + (size_t)12 * NS * b; out.up = bp.up + (size_t)4 * N * b; out.ts = bp.ts + (size_t)NS * b;
     out.lp = bp.lp + (size_t)30 * NS * b; out.slack = bp.slack ? bp.slack + (size_t)5 * NS * b : nullptr;
-    IpmDriver<QuadSolver<SDV> >::solve(C, 0);      // flag = 1 in the reference: a single attempt (QuadcopterSignedDist.jl:227-235)
+    IpmDriver<QuadSolver<SDV> >::solve(C);      // flag = 1 in the reference: a single attempt (QuadcopterSignedDist.jl:227-235)
     __syncthreads();
     double ssum = 0.0;
     const int Np = C.N;

@@ -1,8 +1,8 @@
-// obca_phased.cuh -- phase-split ("lock-step") driver of the batched parking solve.
+// obca_phased.cuh -- phase-split ("lock-step") schedule of the batched parking solve.
 //
-// The interior-point loop of IpmDriver<M>::solve (obca_solver.cuh) restated as a per-problem state machine so that the
-// parallel phases and the serial-in-time KKT sweep of an iteration run as separate kernels over ALL active problems of
-// the batch, each with the launch shape that suits it.  One round = three launches:
+// The phase functions of IpmDriver<M> (obca_solver.cuh: phase_A, phase_B_serial, phase_C), run from separate kernels over
+// ALL active problems of the batch, so that the parallel phases and the serial-in-time KKT sweep of an iteration each get
+// the launch shape that suits them.  One round = three launches:
 //     k_pk_eval    persistent CTAs, one problem at a time: K1 -- item pass (one thread per (obstacle, stage) block:
 //                  evaluation, KKT-error partials, condensation onto the stage pose; hand-over of the 12 doubles per block
 //                  the assembly needs IN THE STAGE SLOT, shared memory), stage pass (dynamics, objective, bounds, assembly
@@ -10,9 +10,9 @@
 //                  was reduced, the re-evaluation, in the same launch.  The finished stage models leave shared memory in
 //                  ONE bulk copy (cp.async.bulk.global.shared::cta, 53 KB per problem).  Also: initial point, end of
 //                  attempt (status / retry / checker), compaction of the active list.
-//     k_pk_sweep   HALF-WARP per problem: K3 stage-banded KKT sweep; the 656-byte stage slots are streamed from HBM through
-//                  a 4-deep ring of bulk copies (cp.async.bulk.shared::cluster.global + mbarrier complete_tx), gains and
-//                  costate rows written back in place; inertia-correction bookkeeping.
+//     k_pk_sweep   one WARP per problem: K3 stage-banded KKT sweep; the 656-byte stage slots are streamed from HBM through
+//                  an 8-deep ring of cp.async (LDGSTS) copies, gains and costate rows written back in place;
+//                  inertia-correction bookkeeping (phase_B_serial).
 //     k_pk_step    persistent CTAs, one problem at a time: K4 -- item pass (steps of the block unknowns from the stored
 //                  local maps) + stage pass (costates, bounds), fraction-to-the-boundary, filter line search (merit
 //                  function: item + stage pass), iterate update.  The step of the block unknowns lives in shared memory.
@@ -20,19 +20,18 @@
 // The iterate, the local maps and the stage slots of every problem live in HBM (layout: problem-major, then [array][stage],
 // so each warp streams contiguous slices); between kernels a problem is described by its ProbState record (phase,
 // iteration, barrier parameter, filter, ...).  When the active set has shrunk far enough the remaining problems are handed to
-//     k_pk_tail    persistent CTA per problem: the same phase functions in a loop, stage slots in shared memory
+//     k_pk_tail    persistent CTA per problem: the phase functions in a loop (the loop of IpmDriver::solve plus the end of
+//                  attempt), stage slots in shared memory
 // which is also the whole solver for small batches.
 //
 // Every floating-point operation of a phase lives in ONE out-of-line device function per template instance
-// (PhasedDriver::phase_A / phase_C and the per-item / per-stage functions of ParkSolver) that all kernels call: the
+// (IpmDriver::phase_A / phase_C and the per-item / per-stage functions of ParkSolver) that all kernels call: the
 // schedules produce bit-identical iterates by construction (tests/test_gpu_parking.py::test_phased_equals_persistent).
 #pragma once
 #include "obca_check.cuh"
 #include "obca_solver.cuh"
 
 namespace obca {
-
-enum { PH_INIT = 0, PH_EVAL = 1, PH_EVAL2 = 2, PH_REASM = 3, PH_KKT = 4, PH_RECOVER = 5, PH_END = 6, PH_DONE = 7 };
 
 struct BatchPtrs {
   const double *x0, *xF, *rx, *ry, *ryaw, *xWS, *uWS, *lWS, *nWS;
@@ -49,32 +48,9 @@ struct BatchPtrs {
 #if defined(__CUDACC__)
 
 // ------------------------------------------------------------------------------------------------------------
-// Bulk-copy (TMA, sm_90) and mbarrier primitives used by the round kernels
+// Bulk copy (sm_90) of the finished stage slots from shared to global memory (k_pk_eval)
 // ------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// global -> shared bulk copy, completion signalled on an mbarrier (bytes: multiple of 16; both addresses 16-byte aligned)
-__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, unsigned bytes, unsigned long long* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(smem_u32(smem_dst)),
-               "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 // shared -> global bulk copy (bulk async-group completion)
 __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, unsigned bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;\n" ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
@@ -83,194 +59,6 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
 // writes of the generic proxy (st.shared) become visible to the async proxy (the bulk copy engine)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-// same for writes to global memory that a later bulk copy of this thread's warp reads back
-__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;\n" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------------------
-// the phase functions (all threads of a CTA call them with the same context; ProbState in shared memory)
-// ------------------------------------------------------------------------------------------------------------
-template <class M>
-struct PhasedDriver {
-  typedef typename M::Ctx Ctx;
-  typedef IpmDriver<M> D;
-
-  // B (serial part, one thread, after the sweep): Ipopt's inertia-correction bookkeeping.  `ok`: 1 if every pivot of
-  // the sweep had the required sign, 0 otherwise (also when the local blocks already failed and the sweep was skipped).
-  __device__ static void phase_B_serial(ProbState& S, const IpmOpts& O, int ok) {
-    S.n_fact++;
-    if (!ok) {
-      if (S.dw == 0.0) S.dw = (S.dw_last == 0.0) ? O.dw_first : dmax(O.dw_min, O.kw_minus * S.dw_last);
-      else S.dw *= (S.dw_last == 0.0) ? O.kw_plus_first : O.kw_plus;
-      if (S.dw > O.dw_max) { S.status = -2; ok = -1; }
-    } else if (S.dw > 0.0) {
-      S.dw_last = S.dw;
-    }
-    S.ok = ok;
-    S.phase = ok > 0 ? PH_RECOVER : (ok == 0 ? PH_REASM : PH_END);
-  }
-
-  // A: [init] -> evaluate at the current iterate, convergence test, barrier update (+ re-evaluation), or re-assembly
-  //    with a larger delta_w.  Leaves phase = PH_KKT (stage models ready) or PH_END (attempt over).
-  __device__ __noinline__ static void phase_A(const Ctx& C) {
-    const IpmOpts& O = CTX_O(C);
-    ProbState& S = *C.S;
-    const int NS = M::n_stages(C);
-    const int ph = S.phase;
-    EvalPart ep;
-    if (ph == PH_REASM) {
-      reassemble(C);
-      return;
-    }
-    if (ph == PH_INIT) {
-      const int restart = S.attempt;
-      OBCA_SERIAL {
-        M::init_scalars(C, restart);
-        S.mu = O.mu_init; S.tau = dmax(O.tau_min, 1.0 - O.mu_init);
-        S.dw = 0.0; S.dw_last = 0.0; S.nfilt = 0; S.status = 0; S.iters = 0; S.n_fact = 0; S.n_kick = 0;
-        S.it = 0; S.first = 1;
-      }
-      OBCA_SYNC();
-      OBCA_FOR_STAGES(k, NS) M::init_stage(C, k, restart);
-      OBCA_SYNC();
-      OBCA_FOR_STAGES(k, NS) M::init_slacks(C, k);
-      // (S.phase may only change behind a barrier: every thread read it on entry)
-      OBCA_SERIAL { S.phase = PH_EVAL; }
-      OBCA_SYNC();
-    }
-    // (PH_EVAL: new iterate -- or a barrier kick: new direction from the same iterate)
-    OBCA_SERIAL { S.dw = 0.0; }
-    OBCA_SYNC();
-    part_init(ep);
-    M::eval_phase(C, true, ep);
-    OBCA_REDUCE(ep);
-    OBCA_SERIAL {
-      S.prof[7]++;
-      D::apply_errors(C, ep);
-      S.ok = ep.ok;
-      if (S.first) {
-        S.theta_max = 1e4 * dmax(1.0, S.th_k);
-        S.theta_min = 1e-4 * dmax(1.0, S.th_k);
-        S.first = 0;
-      }
-      S.e0 = D::err_mu(C, 0.0);
-      S.iters = S.it;
-      S.flag = 0;
-      if (S.e0 <= O.tol && S.e_dual <= O.dual_inf_tol && S.e_pr <= O.constr_viol_tol && S.e_cmax <= O.compl_inf_tol) {
-        S.status = 1; S.flag = 1;
-      } else if (S.it >= O.max_iter) {
-        S.status = 0; S.flag = 1;
-      } else {
-        bool changed = false;
-        while (S.mu > O.mu_min && D::err_mu(C, S.mu) <= O.kappa_eps * S.mu) {
-          S.mu = dmax(O.mu_min, dmin_(O.kappa_mu * S.mu, pow(S.mu, O.theta_mu)));
-          S.tau = dmax(O.tau_min, 1.0 - S.mu);
-          changed = true;
-        }
-        if (changed) { S.nfilt = 0; S.flag = 2; }
-      }
-      S.phase = (S.flag == 1) ? PH_END : PH_KKT;
-    }
-    OBCA_SYNC();
-    if (S.flag == 2) {
-      // mu changed: the barrier terms of the stage models (and phi) are stale
-      part_init(ep);
-      M::eval_phase(C, true, ep);
-      OBCA_REDUCE(ep);
-      OBCA_SERIAL { D::apply_errors(C, ep); S.ok = ep.ok; S.prof[7]++; S.prof[5]++; }
-      OBCA_SYNC();
-    }
-  }
-  // Re-assembly with the current delta_w (inertia correction).  (Inertia failures are found by the sweep: a wrong sign among
-  // the local pivots of the blocks alone is rare -- handling it inside this launch did not change the number of rounds.)
-  __device__ static void reassemble(const Ctx& C) {
-    ProbState& S = *C.S;
-    EvalPart ep;
-    part_init(ep);
-    M::eval_phase(C, false, ep);
-    OBCA_REDUCE(ep);
-    OBCA_SERIAL { S.ok = ep.ok; S.phase = PH_KKT; S.prof[7]++; }
-    OBCA_SYNC();
-  }
-
-  // C: recover the full step, step lengths, filter line search, and -- when a step is accepted -- the iterate update.
-  //    Leaves PH_EVAL (new iterate, or barrier kick: same iterate, new barrier parameter) or PH_END (line-search failure).
-  __device__ __noinline__ static void phase_C(const Ctx& C) {
-    const IpmOpts& O = CTX_O(C);
-    ProbState& S = *C.S;
-    StepPart sp;
-    part_init(sp);
-    M::recover_phase(C, sp);
-    OBCA_REDUCE(sp);
-    OBCA_SERIAL {
-      const double apr = sp.apr, adu = sp.adu, dphi = sp.dphi;
-      S.a_pr = apr; S.a_du = adu; S.dphi = dphi;
-      const double th = S.th_k;
-      if (dphi < 0.0 && th <= S.theta_min)
-        S.a_min = O.gamma_alpha * dmin_(O.gamma_theta, dmin_(O.gamma_phi * th / (-dphi), O.delta * pow(th, O.s_theta) / pow(-dphi, O.s_phi)));
-      else if (dphi < 0.0)
-        S.a_min = O.gamma_alpha * dmin_(O.gamma_theta, O.gamma_phi * th / (-dphi));
-      else
-        S.a_min = O.gamma_alpha * O.gamma_theta;
-      S.alpha = apr;
-      S.flag = 0;
-    }
-    OBCA_SYNC();
-    for (int nbt = 0;; ++nbt) {
-      const double alpha = S.alpha;
-      MeritPart mp;
-      part_init(mp);
-      M::merit_phase(C, alpha, mp);
-      OBCA_REDUCE(mp);
-      OBCA_SERIAL {
-        S.prof[6]++;
-        const double th = mp.th, ph = mp.phi;
-        S.th_t = th; S.ph_t = ph;
-        bool in_filter = th >= S.theta_max || !(ph < 1e299);
-        for (int i = 0; i < S.nfilt && !in_filter; ++i) in_filter = (th >= S.filt_th[i] && ph >= S.filt_ph[i]);
-        bool accepted = false, ftype = false;
-        if (!in_filter) {
-          const bool sw = S.dphi < 0.0 && alpha * pow(-S.dphi, O.s_phi) > O.delta * pow(S.th_k, O.s_theta);
-          if (S.th_k <= S.theta_min && sw) {
-            if (ph <= S.ph_k + O.eta_phi * alpha * S.dphi + 10.0 * 2.220446049250313e-16 * dabs(S.ph_k)) { accepted = true; ftype = true; }
-          } else {
-            if (th <= (1.0 - O.gamma_theta) * S.th_k || ph <= S.ph_k - O.gamma_phi * S.th_k) accepted = true;
-          }
-        }
-        if (accepted) {
-          S.flag = 1;
-          if (!ftype && S.nfilt < 64) {
-            S.filt_th[S.nfilt] = (1.0 - O.gamma_theta) * S.th_k;
-            S.filt_ph[S.nfilt] = S.ph_k - O.gamma_phi * S.th_k;
-            S.nfilt++;
-          }
-        } else {
-          S.alpha = 0.5 * alpha;
-          if (S.alpha < S.a_min || nbt + 1 >= O.max_backtrack) {
-            if (S.n_kick < O.max_kick) {      // barrier kick (restoration substitute), see IpmDriver::solve
-              S.n_kick++;
-              S.nfilt = 0;
-              S.mu = dmin_(O.mu_init, 10.0 * S.mu);
-              S.tau = dmax(O.tau_min, 1.0 - S.mu);
-              S.flag = -2;
-            } else {
-              S.flag = -1; S.status = -1;
-            }
-          }
-        }
-        if (S.flag == 1) S.phase = PH_EVAL;
-        else if (S.flag == -2) { S.it++; S.phase = PH_EVAL; }
-        else if (S.flag == -1) S.phase = PH_END;
-      }
-      OBCA_SYNC();
-      if (S.flag != 0) break;
-    }
-    if (S.flag == 1) {      // accept
-      M::update_phase(C);
-      OBCA_SERIAL { M::update_scalars(C); S.it++; }
-      OBCA_SYNC();
-    }
-  }
-};
 
 // ------------------------------------------------------------------------------------------------------------
 // helpers
@@ -394,17 +182,8 @@ __device__ __forceinline__ void pk_step_A(const PkCtx& C, const PkOutputs& out, 
   for (;;) {
     if (S.phase == PH_END) pk_end_of_attempt<VM, SDV>(C, out, bp, b, F);
     if (S.phase == PH_DONE) return;
-    PhasedDriver<ParkSolver<VM, SDV> >::phase_A(C);
+    IpmDriver<ParkSolver<VM, SDV> >::phase_A(C);
     if (S.phase != PH_END) return;
-  }
-}
-
-__device__ __forceinline__ void state_fresh(ProbState& S, int N) {
-  if (threadIdx.x == 0) {
-    S.N = N;
-    S.phase = PH_INIT; S.attempt = 0; S.iters_total = 0; S.it = 0; S.first = 1; S.status = 0; S.iters = 0;
-    S.t = 1.0; S.e0 = 0.0; S.ok = 0; S.flag = 0;
-    for (int i = 0; i < 8; ++i) S.prof[i] = 0;
   }
 }
 
@@ -580,7 +359,7 @@ k_pk_sweep(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpt
     ok = pk_sweep_warp<VM, SDV>(P, O, L, S->N, Wall + (size_t)b * L.total * L.NSP, slots + (size_t)b * NSL * RSTRIDE, S, hw,
                                 hw + SWEEP_DEPTH * RSTRIDE);
   __syncwarp();
-  if (lane == 0) PhasedDriver<ParkSolver<VM, SDV> >::phase_B_serial(*S, O, ok);
+  if (lane == 0) IpmDriver<ParkSolver<VM, SDV> >::phase_B_serial(*S, O, ok);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -621,7 +400,7 @@ k_pk_step(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpts
     __syncthreads();
     if (threadIdx.x == 0) S.prof[6] = 0;
     __syncthreads();
-    PhasedDriver<ParkSolver<VM, SDV> >::phase_C(C);
+    IpmDriver<ParkSolver<VM, SDV> >::phase_C(C);
     state_store(Sg + b, S);
     if (threadIdx.x == 0) n_merit += (unsigned long long)S.prof[6];
     __syncthreads();
@@ -670,14 +449,10 @@ k_pk_tail(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpts
       const int ph = S.phase;
       __syncthreads();      // every thread has read the phase before thread 0 moves it on (phase_B_serial)
       if (ph == PH_DONE) break;
-      if (threadIdx.x < 32) {
-        int ok = S.ok;
-        if (ok) ok = PS::kkt_solve_warp(C, s_tile);
-        __syncwarp();
-        if (threadIdx.x == 0) PhasedDriver<PS>::phase_B_serial(S, O, ok);
-      }
+      const int ok = PS::factor(C);
+      if (threadIdx.x == 0) IpmDriver<PS>::phase_B_serial(S, O, ok);
       __syncthreads();
-      if (S.phase == PH_RECOVER) PhasedDriver<PS>::phase_C(C);
+      if (S.phase == PH_RECOVER) IpmDriver<PS>::phase_C(C);
     }
     if (threadIdx.x == 0) { n_eval += (unsigned long long)S.prof[7]; n_merit += (unsigned long long)S.prof[6]; }
     __syncthreads();

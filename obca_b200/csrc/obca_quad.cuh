@@ -540,7 +540,20 @@ struct QuadSolver {
     for (int a = 0; a < QNU; ++a) QA(dU, a, N) = 0.0;
     return 1;
   }
-  OBCA_HD static int kkt_host(const QCtx& C) { return kkt_dense(C); }
+  // the KKT solve of an iteration, skipped (0) when the local blocks already failed the inertia test.  All threads call it;
+  // the result is valid in thread 0, which may write S as soon as it returns.  Device: the block-cooperative sweep
+  // (kkt_solve_block); host: kkt_dense.
+  OBCA_HD static int factor(const QCtx& C) {
+#if defined(__CUDA_ARCH__)
+    const int ok = C.S->ok;      // uniform: S.ok was published before the last barrier
+    __syncthreads();             // every thread has read it before thread 0 updates it (phase_B_serial)
+    return ok ? kkt_solve_block(C) : 0;
+#else
+    return C.S->ok ? kkt_dense(C) : 0;
+#endif
+  }
+  // prof[0..5]: clock64 cycles of the driver's phases (eval, kkt, recover, merit, update, serial)
+  static constexpr bool PROF_CYCLES = true;
   static constexpr int STG_N = QNQ + QNYV + QD_NJ + QNX;     // per-stage data of the sweep: Q 231 | q 21 | Jv 66 | r 12
   // shared-memory layout of the tensor-core sweep (kkt_solve_block below)
   static constexpr int V2_LDP = 20, V2_LDF = 24, V2_LDT = 24, V2_LDQ = 24, V2_LDH = 28, V2_LDK = 24;
@@ -554,7 +567,6 @@ struct QuadSolver {
   static_assert((V2_F % 2) == 0 && (V2_Q % 2) == 0 && (V2_T % 2) == 0 && (V2_H % 2) == 0 && (V2_K % 2) == 0, "16-byte alignment");
 
   OBCA_HD static int smem_doubles(int) { return V2_TOTAL; }
-  static constexpr bool KKT_BLOCK = true;
 
 #if defined(__CUDA_ARCH__)
 #ifdef OBCA_QPROF
@@ -862,7 +874,6 @@ struct QuadSolver {
 #endif
     return 1;
   }
-  __device__ static int kkt_solve_warp(const QCtx&, double*) { return 0; }   // unused (KKT_BLOCK)
 #endif
 
   // ---- K4a ----

@@ -22,12 +22,13 @@
 #define OBCA_FOR_ITEMS(i, n) for (int i = threadIdx.x; i < (n); i += blockDim.x)
 #define OBCA_SYNC() __syncthreads()
 #define OBCA_SERIAL if (threadIdx.x == 0)
-// phase profiling: thread 0 charges the cycles since the last mark to counter i (call right after a barrier)
-#define OBCA_PROF(i) do { if (threadIdx.x == 0) { long long t_ = clock64(); S.prof[i] += t_ - S.tmark; S.tmark = t_; } } while (0)
-#define OBCA_PROF_COUNT(i) do { if (threadIdx.x == 0) S.prof[i] += 1; } while (0)
+// phase profiling of the models with M::PROF_CYCLES: thread 0 charges the cycles since the last mark to counter i (call right
+// after a barrier); OBCA_PROF_START() sets the first mark
+#define OBCA_PROF_START() do { if (M::PROF_CYCLES && threadIdx.x == 0) S.tmark = clock64(); } while (0)
+#define OBCA_PROF(i) do { if (M::PROF_CYCLES && threadIdx.x == 0) { long long t_ = clock64(); S.prof[i] += t_ - S.tmark; S.tmark = t_; } } while (0)
 #else
+#define OBCA_PROF_START()
 #define OBCA_PROF(i)
-#define OBCA_PROF_COUNT(i)
 #define OBCA_FOR_STAGES(k, ns) for (int k = 0; k < (ns); ++k)
 #define OBCA_FOR_ITEMS(i, n) for (int i = 0; i < (n); ++i)
 #define OBCA_SYNC()
@@ -112,11 +113,9 @@ __device__ __forceinline__ void block_reduce_warps(T& v, void* scratch, int nw) 
   if (threadIdx.x == 0)
     for (int w = 1; w < nw; ++w) part_merge(v, sc[w]);
 }
-#define OBCA_REDUCE(v) block_reduce(v, C.red_scratch)
-#define OBCA_REDUCE_M(v) M::reduce(v, C)      // IpmDriver<M>: the model's own block reduction
+#define OBCA_REDUCE(v) M::reduce(v, C)      // IpmDriver<M>: the model's own block reduction
 #else
 #define OBCA_REDUCE(v)
-#define OBCA_REDUCE_M(v)
 #endif
 
 // ---- what one (stage, obstacle) OBCA block contributes to its stage (K1).  The blocks are evaluated by the "item" pass of
@@ -189,6 +188,9 @@ constexpr int RSTRIDE = 82;
 constexpr int RQ = 0, Rq = 45, RDYN = 54, RR4 = 74;
 constexpr int RK = 0, RPP = 16, Rpp = 44;   // RPP: rows 0..3 of P_{k+1}, row-major 4x7;  Rpp: p_{k+1}[0..3]
 
+// where the solve of a problem stands between the phase functions of IpmDriver (ProbState::phase)
+enum { PH_INIT = 0, PH_EVAL = 1, PH_EVAL2 = 2, PH_REASM = 3, PH_KKT = 4, PH_RECOVER = 5, PH_END = 6, PH_DONE = 7 };
+
 // per-problem scalar state (shared memory on the device)
 struct ProbState {
   double t, zTL, zTU, dt;           // time scale, its bound multipliers, its step
@@ -211,14 +213,24 @@ struct ProbState {
   int n_kick;     // barrier kicks after line-search failures
   long long prof[8];   // device cycle counters per phase: eval, kkt, recover, merit, update, serial, n_merit, n_eval
   long long tmark;
-  // state machine of the phase-split driver (obca_phased.cuh): where the solve of this problem stands between kernels
-  int phase;        // PH_* below
-  int it;           // iteration counter of the current attempt (the `it` of IpmDriver::solve)
+  // state machine of IpmDriver's phase functions (between kernels in the parking rounds, obca_phased.cuh)
+  int phase;        // PH_* above
+  int it;           // iteration counter of the current attempt
   int attempt;      // 0: from the warm start, 1: the reference's second solve(m) from the last iterate
   int first;        // theta_max / theta_min not yet initialised for this attempt
   int iters_total;  // iterations of the finished attempts
   int N;            // horizon of this problem (set when the problem is picked up fresh; read by the sweep kernel)
 };
+
+// a problem picked up fresh: first attempt from the warm start, profile counters zeroed
+OBCA_HD void state_fresh(ProbState& S, int N) {
+  OBCA_SERIAL {
+    S.N = N;
+    S.phase = PH_INIT; S.attempt = 0; S.iters_total = 0; S.it = 0; S.first = 1; S.status = 0; S.iters = 0;
+    S.t = 1.0; S.e0 = 0.0; S.ok = 0; S.flag = 0;
+    for (int i = 0; i < 8; ++i) S.prof[i] = 0;
+  }
+}
 
 struct PkInputs {
   const double* x0;    // 4
@@ -1526,9 +1538,8 @@ struct ParkSolver {
   }
   // ---- adapters used by the generic interior-point driver (IpmDriver below) ----
   typedef PkCtx Ctx;
-  static constexpr bool KKT_BLOCK = false;   // the KKT sweep is run by warp 0 (kkt_solve_warp)
+  static constexpr bool PROF_CYCLES = false;   // prof[5] counts the re-evaluations after a barrier update
 #if defined(__CUDA_ARCH__)
-  __device__ static int kkt_solve_block(const PkCtx&) { return 0; }
   template <typename T>
   __device__ static void reduce(T& v, const PkCtx& C) { block_reduce(v, C.red_scratch); }   // every warp of the CTA
 #endif
@@ -1549,10 +1560,21 @@ struct ParkSolver {
       S.t = q; S.zTL = zl; S.zTU = zu;
     }
   }
-  OBCA_HD static int kkt_host(const PkCtx& C) {
+  // the KKT solve of an iteration, skipped (0) when the local blocks already failed the inertia test.  All threads call it;
+  // the result is valid in thread 0, which may write S as soon as it returns.  Device: warp 0 runs the sweep over the stage
+  // slots in shared memory (only warp 0 reads S.ok, and its __syncwarp orders those reads before thread 0's writes); host: the
+  // emulation of that warp, or the serial sweep when the context has no tile.
+  OBCA_HD static int factor(const PkCtx& C) {
 #if defined(__CUDA_ARCH__)
-    return 0;
+    int ok = 0;
+    if (threadIdx.x < 32) {
+      ok = C.S->ok;
+      if (ok) ok = kkt_solve_warp(C, C.tile);
+      __syncwarp();
+    }
+    return ok;
 #else
+    if (!C.S->ok) return 0;
     return C.tile ? kkt_solve_warp_emul(C, C.tile) : kkt_solve(C);
 #endif
   }
@@ -1560,7 +1582,8 @@ struct ParkSolver {
 
 // ------------------------------------------------------------------------------------------------------------
 // Generic interior-point driver (Ipopt's algorithm: monotone barrier update, inertia correction, filter line
-// search).  M is the model policy (ParkSolver<VM,SDV>, QuadSolver<SDV>): per-stage phase functions + the KKT sweep.
+// search).  M is the model policy (ParkSolver<VM,SDV>, QuadSolver<SDV>): per-stage phase functions, the block reduction
+// (reduce), the KKT solve (factor) and what prof[5] holds (PROF_CYCLES).
 // ------------------------------------------------------------------------------------------------------------
 template <class M>
 struct IpmDriver {
@@ -1583,194 +1606,220 @@ struct IpmDriver {
   }
 
   // ---------------------------------------------------------------------------------------------------
-  // the solve: all threads of the CTA call this with the same context
+  // The iteration as phase functions: all threads of the CTA call them with the same context; S.phase says where the solve
+  // stands between them.  solve() runs them in one loop, the parking rounds run them from separate kernels (obca_phased.cuh).
+  // On the device phase_A / phase_C are out of line: one copy of their floating-point operations per template instance,
+  // whichever kernel calls them, so that every schedule rounds the same way.
   // ---------------------------------------------------------------------------------------------------
-  OBCA_HD static void solve(const Ctx& C, int restart = 0) {
+  // B (serial part, one thread, after the KKT solve): Ipopt's inertia-correction bookkeeping.  `ok`: 1 if every pivot of
+  // the sweep had the required sign, 0 otherwise (also when the local blocks already failed and the sweep was skipped).
+  OBCA_HD static void phase_B_serial(ProbState& S, const IpmOpts& O, int ok) {
+    S.n_fact++;
+    if (!ok) {
+      if (S.dw == 0.0) S.dw = (S.dw_last == 0.0) ? O.dw_first : dmax(O.dw_min, O.kw_minus * S.dw_last);
+      else S.dw *= (S.dw_last == 0.0) ? O.kw_plus_first : O.kw_plus;
+      if (S.dw > O.dw_max) { S.status = -2; ok = -1; }
+    } else if (S.dw > 0.0) {
+      S.dw_last = S.dw;
+    }
+    S.ok = ok;
+    S.phase = ok > 0 ? PH_RECOVER : (ok == 0 ? PH_REASM : PH_END);
+  }
+
+  // A: [init] -> evaluate at the current iterate, convergence test, barrier update (+ re-evaluation), or re-assembly
+  //    with a larger delta_w.  Leaves phase = PH_KKT (stage models ready) or PH_END (attempt over).
+  OBCA_HD_NI static void phase_A(const Ctx& C) {
     const IpmOpts& O = CTX_O(C);
     ProbState& S = *C.S;
     const int NS = M::n_stages(C);
-
+    const int ph = S.phase;
+    EvalPart ep;
+    if (ph == PH_REASM) {
+      reassemble(C);
+      return;
+    }
+    if (ph == PH_INIT) {
+      const int restart = S.attempt;
+      OBCA_SERIAL {
+        M::init_scalars(C, restart);
+        S.mu = O.mu_init; S.tau = dmax(O.tau_min, 1.0 - O.mu_init);
+        S.dw = 0.0; S.dw_last = 0.0; S.nfilt = 0; S.status = 0; S.iters = 0; S.n_fact = 0; S.n_kick = 0;
+        S.it = 0; S.first = 1;
+      }
+      OBCA_PROF_START();
+      OBCA_SYNC();
+      OBCA_FOR_STAGES(k, NS) M::init_stage(C, k, restart);
+      OBCA_SYNC();
+      OBCA_FOR_STAGES(k, NS) M::init_slacks(C, k);
+      // (S.phase may only change behind a barrier: every thread read it on entry)
+      OBCA_SERIAL { S.phase = PH_EVAL; }
+      OBCA_SYNC();
+    }
+    // (PH_EVAL: new iterate -- or a barrier kick: new direction from the same iterate)
+    OBCA_SERIAL { S.dw = 0.0; }
+    OBCA_SYNC();
+    part_init(ep);
+    M::eval_phase(C, true, ep);
+    OBCA_REDUCE(ep);
+    OBCA_PROF(0);
     OBCA_SERIAL {
-      M::init_scalars(C, restart);
-      S.mu = O.mu_init; S.tau = dmax(O.tau_min, 1.0 - O.mu_init);
-      S.dw = 0.0; S.dw_last = 0.0; S.nfilt = 0; S.status = 0; S.iters = 0; S.n_fact = 0; S.n_kick = 0;
-#if defined(__CUDA_ARCH__)
-      if (!restart) for (int i = 0; i < 8; ++i) S.prof[i] = 0;
-      S.tmark = clock64();
-#endif
+      S.prof[7]++;
+      apply_errors(C, ep);
+      S.ok = ep.ok;
+      if (S.first) {
+        S.theta_max = 1e4 * dmax(1.0, S.th_k);
+        S.theta_min = 1e-4 * dmax(1.0, S.th_k);
+        S.first = 0;
+      }
+      S.e0 = err_mu(C, 0.0);
+      S.iters = S.it;
+      S.flag = 0;
+      if (S.e0 <= O.tol && S.e_dual <= O.dual_inf_tol && S.e_pr <= O.constr_viol_tol && S.e_cmax <= O.compl_inf_tol) {
+        S.status = 1; S.flag = 1;
+      } else if (S.it >= O.max_iter) {
+        S.status = 0; S.flag = 1;
+      } else {
+        // monotone barrier update
+        bool changed = false;
+        while (S.mu > O.mu_min && err_mu(C, S.mu) <= O.kappa_eps * S.mu) {
+          S.mu = dmax(O.mu_min, dmin_(O.kappa_mu * S.mu, pow(S.mu, O.theta_mu)));
+          S.tau = dmax(O.tau_min, 1.0 - S.mu);
+          changed = true;
+        }
+        if (changed) { S.nfilt = 0; S.flag = 2; }
+      }
+      S.phase = (S.flag == 1) ? PH_END : PH_KKT;
     }
     OBCA_SYNC();
-    OBCA_FOR_STAGES(k, NS) M::init_stage(C, k, restart);
-    OBCA_SYNC();
-    OBCA_FOR_STAGES(k, NS) M::init_slacks(C, k);
-    OBCA_SYNC();
-
-    bool first = true;
-    for (int it = 0;; ++it) {
-      // ---- K1: evaluate (errors + assembly with the current mu and dw = 0) ----
-      OBCA_SERIAL { S.dw = 0.0; }
-      OBCA_SYNC();
-      EvalPart ep;
+    OBCA_PROF(5);
+    if (S.flag == 2) {
+      // mu changed: the barrier terms of the stage models (and phi) are stale
       part_init(ep);
       M::eval_phase(C, true, ep);
-      OBCA_REDUCE_M(ep);
-      OBCA_PROF(0); OBCA_PROF_COUNT(7);
-      OBCA_SERIAL {
-        apply_errors(C, ep);
-        S.ok = ep.ok;
-        if (first) {
-          S.theta_max = 1e4 * dmax(1.0, S.th_k);
-          S.theta_min = 1e-4 * dmax(1.0, S.th_k);
-        }
-        S.e0 = err_mu(C, 0.0);
-        S.iters = it;
-        S.flag = 0;
-        if (S.e0 <= O.tol && S.e_dual <= O.dual_inf_tol && S.e_pr <= O.constr_viol_tol && S.e_cmax <= O.compl_inf_tol) {
-          S.status = 1; S.flag = 1;
-        } else if (it >= O.max_iter) {
-          S.status = 0; S.flag = 1;
-        } else {
-          // monotone barrier update
-          bool changed = false;
-          while (S.mu > O.mu_min && err_mu(C, S.mu) <= O.kappa_eps * S.mu) {
-            S.mu = dmax(O.mu_min, dmin_(O.kappa_mu * S.mu, pow(S.mu, O.theta_mu)));
-            S.tau = dmax(O.tau_min, 1.0 - S.mu);
-            changed = true;
-          }
-          if (changed) { S.nfilt = 0; S.flag = 2; }
-        }
-      }
-      first = false;
+      OBCA_REDUCE(ep);
+      OBCA_PROF(0);
+      OBCA_SERIAL { apply_errors(C, ep); S.ok = ep.ok; S.prof[7]++; if (!M::PROF_CYCLES) S.prof[5]++; }
       OBCA_SYNC();
       OBCA_PROF(5);
-      if (S.flag == 1) break;
-      if (S.flag == 2) {   // mu changed: the barrier terms of the stage models (and phi) are stale
-        part_init(ep);
-        M::eval_phase(C, true, ep);
-        OBCA_REDUCE_M(ep);
-        OBCA_PROF(0); OBCA_PROF_COUNT(7);
-        OBCA_SERIAL { apply_errors(C, ep); S.ok = ep.ok; }
-        OBCA_SYNC();
-        OBCA_PROF(5);
-      }
-      // ---- K3 with inertia correction (Ipopt Algorithm IC) ----
-      bool tried0 = false;
-      for (;;) {
-#if defined(__CUDA_ARCH__)
-        if (M::KKT_BLOCK) {
-          if (S.ok) {                                // uniform: S.ok was published before the last barrier
-            const int ok = M::kkt_solve_block(C);
-            __syncthreads();
-            if (threadIdx.x == 0) S.ok = ok;
-          }
-        } else if (S.ok && threadIdx.x < 32) {
-          const int ok = M::kkt_solve_warp(C, C.tile);
-          __syncwarp();
-          if (threadIdx.x == 0) S.ok = ok;
-        }
-#else
-        if (S.ok) S.ok = M::kkt_host(C);
-#endif
-        OBCA_SYNC();
-        OBCA_SERIAL {
-          S.n_fact++;
-          if (!S.ok) {
-            if (S.dw == 0.0) S.dw = (S.dw_last == 0.0) ? O.dw_first : dmax(O.dw_min, O.kw_minus * S.dw_last);
-            else S.dw *= (S.dw_last == 0.0) ? O.kw_plus_first : O.kw_plus;
-            if (S.dw > O.dw_max) { S.status = -2; S.ok = -1; }
-          } else if (S.dw > 0.0) {
-            S.dw_last = S.dw;
-          }
-        }
-        OBCA_SYNC();
-        OBCA_PROF(1);
-        if (S.ok != 0) break;
-        part_init(ep);
-        M::eval_phase(C, false, ep);
-        OBCA_REDUCE_M(ep);
-        OBCA_SERIAL { S.ok = ep.ok; }
-        OBCA_SYNC();
-        OBCA_PROF(0); OBCA_PROF_COUNT(7);
-        (void)tried0;
-      }
-      if (S.ok < 0) break;
-      // ---- K4: recover, step lengths, filter line search ----
-      StepPart sp;
-      part_init(sp);
-      M::recover_phase(C, sp);
-      OBCA_REDUCE_M(sp);
-      OBCA_PROF(2);
+    }
+  }
+  // Re-assembly with the current delta_w (inertia correction).  (Inertia failures are found by the sweep: a wrong sign among
+  // the local pivots of the blocks alone is rare -- handling it inside this launch did not change the number of rounds.)
+  OBCA_HD static void reassemble(const Ctx& C) {
+    ProbState& S = *C.S;
+    EvalPart ep;
+    part_init(ep);
+    M::eval_phase(C, false, ep);
+    OBCA_REDUCE(ep);
+    OBCA_SERIAL { S.ok = ep.ok; S.phase = PH_KKT; S.prof[7]++; }
+    OBCA_SYNC();
+    OBCA_PROF(0);
+  }
+
+  // C: recover the full step, step lengths, filter line search, and -- when a step is accepted -- the iterate update.
+  //    Leaves PH_EVAL (new iterate, or barrier kick: same iterate, new barrier parameter) or PH_END (line-search failure).
+  OBCA_HD_NI static void phase_C(const Ctx& C) {
+    const IpmOpts& O = CTX_O(C);
+    ProbState& S = *C.S;
+    StepPart sp;
+    part_init(sp);
+    M::recover_phase(C, sp);
+    OBCA_REDUCE(sp);
+    OBCA_PROF(2);
+    OBCA_SERIAL {
+      const double apr = sp.apr, adu = sp.adu, dphi = sp.dphi;
+      S.a_pr = apr; S.a_du = adu; S.dphi = dphi;
+      const double th = S.th_k;
+      if (dphi < 0.0 && th <= S.theta_min)
+        S.a_min = O.gamma_alpha * dmin_(O.gamma_theta, dmin_(O.gamma_phi * th / (-dphi), O.delta * pow(th, O.s_theta) / pow(-dphi, O.s_phi)));
+      else if (dphi < 0.0)
+        S.a_min = O.gamma_alpha * dmin_(O.gamma_theta, O.gamma_phi * th / (-dphi));
+      else
+        S.a_min = O.gamma_alpha * O.gamma_theta;
+      S.alpha = apr;
+      S.flag = 0;
+    }
+    OBCA_SYNC();
+    for (int nbt = 0;; ++nbt) {
+      const double alpha = S.alpha;
+      MeritPart mp;
+      part_init(mp);
+      M::merit_phase(C, alpha, mp);
+      OBCA_REDUCE(mp);
+      OBCA_PROF(3);
       OBCA_SERIAL {
-        const double apr = sp.apr, adu = sp.adu, dphi = sp.dphi;
-        S.a_pr = apr; S.a_du = adu; S.dphi = dphi;
-        const double th = S.th_k;
-        if (dphi < 0.0 && th <= S.theta_min)
-          S.a_min = O.gamma_alpha * dmin_(O.gamma_theta, dmin_(O.gamma_phi * th / (-dphi), O.delta * pow(th, O.s_theta) / pow(-dphi, O.s_phi)));
-        else if (dphi < 0.0)
-          S.a_min = O.gamma_alpha * dmin_(O.gamma_theta, O.gamma_phi * th / (-dphi));
-        else
-          S.a_min = O.gamma_alpha * O.gamma_theta;
-        S.alpha = apr;
-        S.flag = 0;
+        S.prof[6]++;
+        const double th = mp.th, ph = mp.phi;
+        S.th_t = th; S.ph_t = ph;
+        bool in_filter = th >= S.theta_max || !(ph < 1e299);
+        for (int i = 0; i < S.nfilt && !in_filter; ++i) in_filter = (th >= S.filt_th[i] && ph >= S.filt_ph[i]);
+        bool accepted = false, ftype = false;
+        if (!in_filter) {
+          const bool sw = S.dphi < 0.0 && alpha * pow(-S.dphi, O.s_phi) > O.delta * pow(S.th_k, O.s_theta);
+          if (S.th_k <= S.theta_min && sw) {
+            if (ph <= S.ph_k + O.eta_phi * alpha * S.dphi + 10.0 * 2.220446049250313e-16 * dabs(S.ph_k)) { accepted = true; ftype = true; }
+          } else {
+            if (th <= (1.0 - O.gamma_theta) * S.th_k || ph <= S.ph_k - O.gamma_phi * S.th_k) accepted = true;
+          }
+        }
+        if (accepted) {
+          S.flag = 1;
+          if (!ftype && S.nfilt < 64) {
+            S.filt_th[S.nfilt] = (1.0 - O.gamma_theta) * S.th_k;
+            S.filt_ph[S.nfilt] = S.ph_k - O.gamma_phi * S.th_k;
+            S.nfilt++;
+          }
+        } else {
+          S.alpha = 0.5 * alpha;
+          if (S.alpha < S.a_min || nbt + 1 >= O.max_backtrack) {
+            // Ipopt would enter its restoration phase here.  Substitute ("barrier kick"): forget the filter,
+            // raise the barrier parameter one decade and recompute the direction from the same iterate; after
+            // max_kick kicks the attempt ends with a line-search failure (the caller's retry logic takes over).
+            if (S.n_kick < O.max_kick) {
+              S.n_kick++;
+              S.nfilt = 0;
+              S.mu = dmin_(O.mu_init, 10.0 * S.mu);
+              S.tau = dmax(O.tau_min, 1.0 - S.mu);
+              S.flag = -2;
+            } else {
+              S.flag = -1; S.status = -1;
+            }
+          }
+        }
+        if (S.flag == 1) S.phase = PH_EVAL;
+        else if (S.flag == -2) { S.it++; S.phase = PH_EVAL; }
+        else if (S.flag == -1) S.phase = PH_END;
       }
       OBCA_SYNC();
-      for (int nbt = 0;; ++nbt) {
-        const double alpha = S.alpha;
-        MeritPart mp;
-        part_init(mp);
-        M::merit_phase(C, alpha, mp);
-        OBCA_REDUCE_M(mp);
-        OBCA_PROF(3); OBCA_PROF_COUNT(6);
-        OBCA_SERIAL {
-          const double th = mp.th, ph = mp.phi;
-          S.th_t = th; S.ph_t = ph;
-          bool in_filter = th >= S.theta_max || !(ph < 1e299);
-          for (int i = 0; i < S.nfilt && !in_filter; ++i) in_filter = (th >= S.filt_th[i] && ph >= S.filt_ph[i]);
-          bool accepted = false, ftype = false;
-          if (!in_filter) {
-            const bool sw = S.dphi < 0.0 && alpha * pow(-S.dphi, O.s_phi) > O.delta * pow(S.th_k, O.s_theta);
-            if (S.th_k <= S.theta_min && sw) {
-              if (ph <= S.ph_k + O.eta_phi * alpha * S.dphi + 10.0 * 2.220446049250313e-16 * dabs(S.ph_k)) { accepted = true; ftype = true; }
-            } else {
-              if (th <= (1.0 - O.gamma_theta) * S.th_k || ph <= S.ph_k - O.gamma_phi * S.th_k) accepted = true;
-            }
-          }
-          if (accepted) {
-            S.flag = 1;
-            if (!ftype && S.nfilt < 64) {
-              S.filt_th[S.nfilt] = (1.0 - O.gamma_theta) * S.th_k;
-              S.filt_ph[S.nfilt] = S.ph_k - O.gamma_phi * S.th_k;
-              S.nfilt++;
-            }
-          } else {
-            S.alpha = 0.5 * alpha;
-            if (S.alpha < S.a_min || nbt + 1 >= O.max_backtrack) {
-              // Ipopt would enter its restoration phase here.  Substitute ("barrier kick"): forget the filter,
-              // raise the barrier parameter one decade and recompute the direction from the same iterate; after
-              // max_kick kicks the attempt ends with a line-search failure (the caller's retry logic takes over).
-              if (S.n_kick < O.max_kick) {
-                S.n_kick++;
-                S.nfilt = 0;
-                S.mu = dmin_(O.mu_init, 10.0 * S.mu);
-                S.tau = dmax(O.tau_min, 1.0 - S.mu);
-                S.flag = -2;
-              } else {
-                S.flag = -1; S.status = -1;
-              }
-            }
-          }
-        }
-        OBCA_SYNC();
-        OBCA_PROF(5);
-        if (S.flag != 0) break;
-      }
-      if (S.flag == -2) continue;     // barrier kick: new direction from the same iterate
-      if (S.flag < 0) break;
-      // ---- accept ----
+      OBCA_PROF(5);
+      if (S.flag != 0) break;
+    }
+    if (S.flag == 1) {      // accept
       M::update_phase(C);
-      OBCA_SERIAL { M::update_scalars(C); }
+      OBCA_SERIAL { M::update_scalars(C); S.it++; }
       OBCA_SYNC();
       OBCA_PROF(4);
+    }
+  }
+
+  // ---------------------------------------------------------------------------------------------------
+  // the solve of one problem from its warm start: all threads of the CTA call this with the same context
+  // ---------------------------------------------------------------------------------------------------
+  OBCA_HD static void solve(const Ctx& C) {
+    ProbState& S = *C.S;
+    state_fresh(S, M::n_stages(C) - 1);
+    OBCA_SYNC();
+    for (;;) {
+      phase_A(C);
+      const int ph = S.phase;
+      OBCA_SYNC();      // every thread has read the phase before thread 0 moves it on (phase_B_serial)
+      if (ph == PH_END) break;
+      const int ok = M::factor(C);
+      OBCA_SERIAL { phase_B_serial(S, CTX_O(C), ok); }
+      OBCA_SYNC();
+      OBCA_PROF(1);
+      if (S.phase == PH_RECOVER) phase_C(C);
+      if (S.phase == PH_END) break;
     }
   }
 };
