@@ -1,0 +1,63 @@
+"""The reverse-parking sweep in a row of a car park (obca_b200.scenarios.parking_lot_scenario: n_cars parked cars + the far wall,
+nOb = n_cars + 1 obstacles): plan every start pose with the GPU Hybrid A* against the lot's point cloud (one call,
+obca_plan_parking_warmstart_batch), solve every pose planned OK -- each with the horizon the planner gave it -- in ONE GPU call
+(obca_parking_solve_mixed), and run the reference's acceptance test on every result in one more call.  Poses the planner does not
+plan (no path, or a search that outgrew the device's scratch) are reported, not planned on the host: the host planner's warm-start
+entry knows only the reference's two scenes.
+
+usage: python examples/sweep_parking_lot.py [B] [n_cars] [seed]      (needs a CUDA device)
+"""
+import os
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import obca_b200                                 # noqa: E402
+from obca_b200 import parking, scenarios         # noqa: E402
+from obca_b200.planner import device             # noqa: E402
+
+
+def run(B=64, seed=0, n_cars=10, signed_dist=1, sampleN=3):
+    sc = scenarios.parking_lot_scenario(n_cars)
+    rng = np.random.default_rng(seed)
+    x0 = np.column_stack([rng.uniform(-9, 9, B), rng.uniform(6.8, 9.3, B), np.zeros(B), np.zeros(B)])      # start poses in the lane, v = 0
+    ox, oy = scenarios.parking_lot_points(n_cars)
+    Ts = sc["Ts"] / 3 * sampleN
+    t0 = time.time()
+    o = device.plan_raw(x0, sc["xF"], ox, oy, Ts, sc["L"], sampleN)
+    t_plan = time.time() - t0
+    idx = np.flatnonzero(o["status"] == 0)
+    out = dict(B=B, n_planned=int(idx.size), status=o["status"].copy(), t_plan=t_plan, t_solve=0.0, n_converged=0, n_clean=0,
+               exitflag=np.zeros(B, int), N=o["N"].copy())
+    if idx.size == 0:
+        return out
+    Ns = o["N"][idx]
+    rx = [o["rx"][i, :n + 1] for i, n in zip(idx, Ns)]; ry = [o["ry"][i, :n + 1] for i, n in zip(idx, Ns)]
+    ryaw = [o["ryaw"][i, :n + 1] for i, n in zip(idx, Ns)]
+    xWS = [o["xWS"][i, :4 * (n + 1)].reshape(4, n + 1).T for i, n in zip(idx, Ns)]
+    uWS = [o["uWS"][i, :2 * n].reshape(2, n).T for i, n in zip(idx, Ns)]
+    r = parking.parking_solve_mixed(x0[idx], sc["xF"], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"], sc["b"],
+                                    rx, ry, ryaw, 0, xWS, uWS, signed_dist)
+    feas, _, _ = parking.check_parking_mixed(x0[idx], sc["xF"], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"],
+                                             sc["b"], r["xp"], r["up"], r["lp"], r["np"], r["ts"], 0, signed_dist, r["sl"])
+    conv = r["exitflag"] == 1
+    out.update(t_solve=float(r["time"]), n_converged=int(conv.sum()), n_clean=int((np.asarray(feas)[conv] == 1).sum()))
+    out["exitflag"][idx] = r["exitflag"]
+    return out
+
+
+if __name__ == "__main__":
+    a = sys.argv
+    try:
+        o = run(int(a[1]) if len(a) > 1 else 64, int(a[3]) if len(a) > 3 else 0, int(a[2]) if len(a) > 2 else 10)
+    except obca_b200.ObcaError as e:
+        print("not run:", e); sys.exit(2)
+    miss = np.flatnonzero(o["status"] != 0)
+    print(f"{o['B']} start poses: {o['n_planned']} planned on the GPU in {o['t_plan']:.2f} s"
+          + (f" (not planned: poses {miss.tolist()}, status {o['status'][miss].tolist()})" if miss.size else "")
+          + f"; solved in one GPU call in {o['t_solve'] * 1e3:.0f} ms device time: {o['n_converged']} converged, "
+          f"{o['n_clean']} of them pass ParkingConstraints")

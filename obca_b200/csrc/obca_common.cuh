@@ -20,8 +20,8 @@
 #define OBCA_HD_NI inline
 #endif
 
-#define OBCA_MAX_OB 5      // obstacles per problem
-#define OBCA_MAX_ROWS 20   // total half-spaces (sum vOb)
+#define OBCA_MAX_OB 16     // obstacles per problem
+#define OBCA_MAX_ROWS 64   // total half-spaces (sum vOb)
 #define OBCA_VMAX 4        // half-spaces per obstacle supported by the kernels (templates instantiate 2 and 4)
 
 namespace obca {

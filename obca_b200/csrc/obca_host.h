@@ -10,6 +10,9 @@
 
 namespace obca {
 
+// the bounds on nOb and vOb[j] bound sum(vOb): no shape that passes them overflows the problem's half-space arrays
+static_assert(OBCA_MAX_OB * OBCA_VMAX <= OBCA_MAX_ROWS, "sum(vOb) is bounded through nOb and vOb[j]");
+
 // Arguments as in ParkingSignedDist.jl:29: vOb = half-space counts per obstacle, A = sum(vOb) x 2 column-major,
 // b = sum(vOb), ego = [x_up, y_up, -x_lo, -y_lo] (main.jl:72-73), XYbounds = [xL, xU, yL, yU] (main.jl:209-210).
 inline int fill_problem(ParkProblem& P, int N, int nOb, const int* vOb, const double* A, const double* b, double Ts,
@@ -23,8 +26,7 @@ inline int fill_problem(ParkProblem& P, int N, int nOb, const int* vOb, const do
     P.vOb[j] = vOb[j]; P.voff[j] = V; V += vOb[j];
   }
   P.voff[nOb] = V;
-  if (V > OBCA_MAX_ROWS) return -3;
-  P.V = V;
+  P.V = V;      // <= OBCA_MAX_OB * OBCA_VMAX <= OBCA_MAX_ROWS (static_assert above)
   for (int r = 0; r < V; ++r) { P.A[r][0] = A[r]; P.A[r][1] = A[V + r]; P.b[r] = b[r]; }
   P.Ts = Ts; P.L = L;
   const double W_ev = ego[1] + ego[3], L_ev = ego[0] + ego[2];           // ParkingSignedDist.jl:182-183
@@ -37,6 +39,17 @@ inline int fill_problem(ParkProblem& P, int N, int nOb, const int* vOb, const do
   P.w_a = (fixTime || !signed_dist) ? 0.5 : 0.1;                          // :79,:86 ; ParkingDist.jl:79,87
   P.w_yaw = fixTime ? 0.01 : 0.0001;                                      // :82,:91
   return 0;
+}
+
+#define OBCA_STR_(x) #x
+#define OBCA_STR(x) OBCA_STR_(x)
+// the message for a nonzero return of fill_problem: the bound the problem breaks
+inline const char* shape_error(int rc) {
+  switch (rc) {
+    case -1: return "unsupported problem shape: need N >= 2 and 1 <= nOb <= " OBCA_STR(OBCA_MAX_OB) " obstacles";
+    case -2: return "unsupported problem shape: need 1 <= vOb[j] <= " OBCA_STR(OBCA_VMAX) " half-spaces per obstacle";
+    default: return "unsupported problem shape";
+  }
 }
 
 // Arguments of QuadcopterSignedDist.jl:25: obs = ob1..ob5 as 6 x 5 column-major; bounds of :78-93 (QuadcopterDist.jl:88).

@@ -340,18 +340,43 @@ static int env_int(const char* name, int dflt) {
   return (v && *v) ? atoi(v) : dflt;
 }
 
+// Where k_pk_step keeps the step rows dLAM .. dRS (V + 10 nOb + 5 rows of NSP doubles): in shared memory while the kernel
+// still has OBCA_STEP_SMEM_MIN_CTAS resident CTAs per SM with them there, else in the workspace (no dynamic shared memory).
+// The default is the kernel's launch bound (the reference's scenes at N = 80 need 40-51 rows and stay in shared memory);
+// profiles/lot_h100.md has the measurement behind the rule.
+#ifndef OBCA_STEP_SMEM_MIN_CTAS
+#define OBCA_STEP_SMEM_MIN_CTAS OBCA_MINB_C
+#endif
+template <class K>
+static cudaError_t step_rows_in_smem(K kernel, const PkLay& L, int* in_smem, size_t* smem) {
+  const size_t need = (size_t)(L.dRS + 1 - L.dLAM) * L.NSP * sizeof(double);
+  int dev = 0, optin = 0, occ = 0;
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, kernel);
+  *in_smem = 0; *smem = 0;
+  // a CTA's dynamic and static shared memory together may not exceed the opt-in limit
+  if (e != cudaSuccess || need + fa.sharedSizeBytes > (size_t)optin) return e;
+  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, PK_THREADS, need);
+  if (e == cudaSuccess && occ >= OBCA_STEP_SMEM_MIN_CTAS) { *in_smem = 1; *smem = need; }
+  return e;
+}
+
 template <int VM, bool SDV>
 static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, const BatchPtrs& bp, int mode) {
   PkLay L = make_layout(P, LocalDims<VM, SDV>::NFAC);
   const int B = bp.B, NS = P.N + 1;
   if (NS > 128) { set_err("horizon too long for this build (N+1 <= 128)"); return OBCA_ERR_UNSUPPORTED; }
   const size_t smem_slots = (size_t)NS * RSTRIDE * sizeof(double);
-  const size_t smem_step = (size_t)(L.dRS + 1 - L.dLAM) * L.NSP * sizeof(double);
   CK(cudaFuncSetAttribute(k_pk_eval<VM, SDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_slots));
   CK(cudaFuncSetAttribute(k_pk_tail<VM, SDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_slots));
-  CK(cudaFuncSetAttribute(k_pk_step<VM, SDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_step));
   const size_t smem_sweep = (size_t)SWEEP_WARPS * SWEEP_WARP_DOUBLES * sizeof(double);
   CK(cudaFuncSetAttribute(k_pk_sweep<VM, SDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sweep));
+  size_t smem_step = 0;
+  int step_smem = 0;
+  CK(step_rows_in_smem(k_pk_step<VM, SDV>, L, &step_smem, &smem_step));
   int occ_t = 0, occ_e = 0, occ_s = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, k_pk_tail<VM, SDV>, PK_THREADS, smem_slots));
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_pk_eval<VM, SDV>, PK_THREADS, smem_slots));
@@ -416,7 +441,8 @@ static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, cons
     mark();
     k_pk_sweep<VM, SDV><<<(nb + SWEEP_WARPS - 1) / SWEEP_WARPS, 32 * SWEEP_WARPS, smem_sweep, st>>>(P, O, L, c.W, c.slots, Sg, a_out, n_out, n_zero);
     mark();
-    k_pk_step<VM, SDV><<<cap(nb, step_cap), PK_THREADS, smem_step, st>>>(P, O, L, bp, c.W, c.slots, Sg, a_out, n_out, q_step, q_eval);
+    k_pk_step<VM, SDV><<<cap(nb, step_cap), PK_THREADS, smem_step, st>>>(P, O, L, bp, c.W, c.slots, Sg, a_out, n_out, q_step, q_eval,
+                                                                          step_smem);
     mark();
     CK(cudaGetLastError());
     if (readback) CK(cudaMemcpyAsync(c.h_n + (rr & 15), n_out, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -506,7 +532,8 @@ static int solve_dev_impl(DevCtx& c, const ParkProblem& P, const IpmOpts& O, Bat
   for (int i = 0; i < 4; ++i) c.phase_ms[i] = 0.0;
   int rc;
   const int mode = env_int("OBCA_MODE", 0);
-  // large batches are solved in chunks so that the per-problem workspace (~0.25 MB) stays within a few GB
+  // large batches are solved in chunks so that the per-problem workspace (0.19 MB for config 2, 0.6 MB at 11 obstacles, N = 80;
+  // INTEGRATION.md section 3a) stays within a few GB
   const int chunk = env_int("OBCA_CHUNK", 16384);
   const int NSc = P.N + 1, Vc = P.V, nObc = P.nOb;
   rc = 0;
@@ -581,9 +608,7 @@ static int parking_solve_dev(int B, int N, const int* Nb, int nOb, const int* vO
   if (B <= 0 || !vOb || !A || !b || !x0 || !xF || !ego || !XYbounds || !rx || !ry || !ryaw || !xWS || !uWS || !xp ||
       !up || !ts || !lp || !np || !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
   ParkProblem P;
-  if (fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) {
-    set_err("unsupported problem shape"); return OBCA_ERR_ARG;
-  }
+  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
   DevCtx* c;
   int rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
@@ -641,11 +666,14 @@ static int parking_solve_host(bool mixed, int B, int N, const int* Nb, int nOb, 
                               int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
                               double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                               double* solve_seconds) {
-  if (B <= 0 || !vOb || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up || !ts || !lp || !np ||
-      !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
+  if (B <= 0 || !vOb || !A || !b || !ego || !XYbounds || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up ||
+      !ts || !lp || !np || !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
   int rc = mixed ? check_horizons(B, Nb, N) : 0;
   if (rc) return rc;
-  if (N < 2 || nOb < 1 || nOb > OBCA_MAX_OB) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  {   // the shape decides the staging sizes below: checked before anything is sized, copied or written
+    ParkProblem P;
+    if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
+  }
   int V = 0;
   for (int j = 0; j < nOb; ++j) V += vOb[j];
   DevCtx* c;
@@ -726,7 +754,7 @@ static int check_parking(int B, int N, const int* Nb, int nOb, const int* vOb, c
     set_err("null argument"); return OBCA_ERR_ARG;
   }
   ParkProblem P;
-  if (fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sd)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sd)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
   DevCtx* c;
   int rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
@@ -963,7 +991,7 @@ int obca_dualmultws_batch(int B, int N, int nOb, const int* vOb, const double* A
   if (B <= 0 || !vOb || !A || !b || !ego || !rx || !ry || !ryaw || !lp || !np) { set_err("null argument"); return OBCA_ERR_ARG; }
   ParkProblem P;
   double xy[4] = {0, 1, 0, 1};
-  if (fill_problem(P, N, nOb, vOb, A, b, 1.0, 1.0, ego, xy, 0, 1)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, 1.0, 1.0, ego, xy, 0, 1)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
   DevCtx* c;
   int rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
@@ -1068,7 +1096,7 @@ int obca_last_times(int device, double* dualws_seconds, double* solve_seconds) {
 int obca_parking_eval_sizes(int N, int nOb, const int* vOb, int signed_dist, long long* n_out, long long* m_out) {
   ParkProblem P;
   double A[2 * OBCA_MAX_ROWS] = {0}, b[OBCA_MAX_ROWS] = {0}, ego[4] = {1, 1, 1, 1}, xy[4] = {0, 1, 0, 1};
-  if (fill_problem(P, N, nOb, vOb, A, b, 1.0, 1.0, ego, xy, 0, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, 1.0, 1.0, ego, xy, 0, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
   if (n_out) *n_out = (long long)eval_n(P);
   if (m_out) *m_out = (long long)eval_m(P);
   return 0;
@@ -1084,7 +1112,7 @@ int obca_parking_eval_batch_dev(int B, int N, int nOb, const int* vOb, const dou
   if (B <= 0 || !vOb || !A || !b || !x0 || !xF || !ego || !XYbounds || !rx || !ry || !ryaw || !xp || !up || !lp || !np ||
       !c_out || !gradL_out || !fk_out || (signed_dist && !sl) || (!fixTime && !ts)) { set_err("null argument"); return OBCA_ERR_ARG; }
   ParkProblem P;
-  if (fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
   DevCtx* c;
   int rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;

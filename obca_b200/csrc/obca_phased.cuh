@@ -5,7 +5,8 @@
 // the launch shape that suits them.  One round = three launches:
 //     k_pk_eval    persistent CTAs, one problem at a time: K1 -- item pass (one thread per (obstacle, stage) block:
 //                  evaluation, KKT-error partials, condensation onto the stage pose; hand-over of the 12 doubles per block
-//                  the assembly needs IN THE STAGE SLOT, shared memory), stage pass (dynamics, objective, bounds, assembly
+//                  the assembly needs IN THE STAGE SLOT, shared memory, for the first six obstacles, in workspace rows for
+//                  the others), stage pass (dynamics, objective, bounds, assembly
 //                  of the stage models), reductions, convergence test, barrier update -- and, when the barrier parameter
 //                  was reduced, the re-evaluation, in the same launch.  The finished stage models leave shared memory in
 //                  ONE bulk copy (cp.async.bulk.global.shared::cta, 53 KB per problem).  Also: initial point, end of
@@ -15,7 +16,8 @@
 //                  inertia-correction bookkeeping (phase_B_serial).
 //     k_pk_step    persistent CTAs, one problem at a time: K4 -- item pass (steps of the block unknowns from the stored
 //                  local maps) + stage pass (costates, bounds), fraction-to-the-boundary, filter line search (merit
-//                  function: item + stage pass), iterate update.  The step of the block unknowns lives in shared memory.
+//                  function: item + stage pass), iterate update.  The step of the block unknowns lives in shared memory
+//                  while the kernel keeps its resident CTAs with it there, else in the workspace.
 // The persistent CTAs of k_pk_eval and k_pk_step take their problems from an atomic work queue (pk_queue_next).
 // The iterate, the local maps and the stage slots of every problem live in HBM (layout: problem-major, then [array][stage],
 // so each warp streams contiguous slices); between kernels a problem is described by its ProbState record (phase,
@@ -364,7 +366,8 @@ k_pk_sweep(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpt
 
 // ------------------------------------------------------------------------------------------------------------
 // K_step: persistent CTAs, one problem at a time.  The rows of the step that the sweep does not produce (block unknowns,
-// new multipliers, slack steps: 40 of 46 rows for config 2) never leave shared memory.
+// new multipliers, slack steps: V + 10 nOb + 5 rows, 40 of 46 for config 2) stay in shared memory when they fit there
+// (step_smem = 1; the host's rule, step_rows_in_smem); otherwise they are the workspace rows dLAM .. dRS, as in k_pk_tail.
 // ------------------------------------------------------------------------------------------------------------
 #ifndef OBCA_MINB_C
 #define OBCA_MINB_C 5
@@ -373,8 +376,9 @@ template <int VM, bool SDV>
 __global__ void __launch_bounds__(PK_THREADS, OBCA_MINB_C)
 k_pk_step(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpts O, const PkLay L, const BatchPtrs bp,
           double* __restrict__ Wall, double* __restrict__ slots, ProbState* __restrict__ Sg,
-          const int* __restrict__ act, const int* __restrict__ n_act, int* __restrict__ queue, int* __restrict__ queue_next) {
-  extern __shared__ __align__(16) double s_step[];      // (dRS + 1 - dLAM) x NSP
+          const int* __restrict__ act, const int* __restrict__ n_act, int* __restrict__ queue, int* __restrict__ queue_next,
+          int step_smem) {
+  extern __shared__ __align__(16) double s_step[];      // step_smem: (dRS + 1 - dLAM) x NSP, else empty
   __shared__ ProbState S;
   __shared__ double s_red[4 * 12];
   __shared__ int s_i;
@@ -394,7 +398,7 @@ k_pk_step(const __grid_constant__ ParkProblem P, const __grid_constant__ IpmOpts
     state_load(S, Sg + b);
     if (threadIdx.x == 0) {
       pk_make_ctx<VM, SDV>(C, out, P, O, L, bp, b, Wall + (size_t)b * L.total * L.NSP);
-      C.Wd = s_step;
+      if (step_smem) C.Wd = s_step;
       C.ric = s_step /* unused here; a shared address as OBCA_LOCALS assumes */; C.pp = slots + (size_t)b * NSL * RSTRIDE; C.red_scratch = s_red; C.tile = nullptr; C.S = &S;
     }
     __syncthreads();

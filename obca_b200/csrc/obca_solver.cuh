@@ -120,15 +120,17 @@ __device__ __forceinline__ void block_reduce_warps(T& v, void* scratch, int nw) 
 
 // ---- what one (stage, obstacle) OBCA block contributes to its stage (K1).  The blocks are evaluated by the "item" pass of
 //      an evaluation (one thread per (obstacle, stage) pair); the 12 doubles the stage assembly needs (Schur complement,
-//      gradient, Lagrangian-gradient rows of the pose) are handed over through the stage's own slot in shared memory, the
-//      KKT-error / merit partials are merged into the thread's running EvalPart ----
+//      gradient, Lagrangian-gradient rows of the pose) are handed over through the stage's own slot in shared memory for
+//      the first HO_SLOT_OB obstacles and through the workspace rows HO for the others, the KKT-error / merit partials are
+//      merged into the thread's running EvalPart ----
 struct BlockOut {
   double Sxx[6], rx3[3];   // Schur complement and gradient on the pose (X, Y, psi)      (assembly)
   double gx[3];            // the block's rows of the Lagrangian gradient on the pose    (errors)
   double e_dual, e_pr, cmax, cmin, sum_y, sum_z, th, lsum, fobj;   // KKT-error / merit partials; lsum = sum of log(gap)
   int ok;                  // 1: every local pivot had the sign required for inertia (n, m, 0)
 };
-constexpr int HO_N = 12;   // doubles per block handed over in the stage slot: Sxx 6 | rx3 3 | gx 3 (slot offset HO_N * j)
+constexpr int HO_N = 12;   // doubles per block handed over: Sxx 6 | rx3 3 | gx 3 (slot offset HO_N * j, or rows HO + HO_N * (j - HO_SLOT_OB))
+constexpr int HO_SLOT_OB = 6;   // obstacles whose hand-over fits in a stage slot: HO_N * HO_SLOT_OB = 72 <= RSTRIDE = 82
 
 // ---- workspace layout: every entry is an array of NSP doubles indexed by stage ----
 struct PkLay {
@@ -144,6 +146,7 @@ struct PkLay {
   // KKT workspace
   int LF;
   int nfac;
+  int HO;      // hand-over of the item pass for obstacles j >= HO_SLOT_OB: HO_N rows each (none with nOb <= HO_SLOT_OB)
   int total;
 };
 
@@ -173,6 +176,7 @@ inline PkLay make_layout(const ParkProblem& P, int nfac) {
   L.dSD = take(P.nOb); L.dSN = take(P.nOb); L.dRS = take(1);
   L.nfac = nfac;
   L.LF = take(P.nOb * nfac);
+  L.HO = take(HO_N * (P.nOb > HO_SLOT_OB ? P.nOb - HO_SLOT_OB : 0));
   L.total = c;
   return L;
 }
@@ -185,6 +189,7 @@ inline PkLay make_layout(const ParkProblem& P, int nfac) {
 // copy (cp.async.bulk) and the sweep kernel streams single slots back with bulk copies; 82 = 2 mod 4 costs a 2-way bank
 // conflict on the thread-per-stage accesses (an odd stride would be conflict-free but misaligns every second slot).
 constexpr int RSTRIDE = 82;
+static_assert(HO_N * HO_SLOT_OB <= RSTRIDE, "the hand-over of the first HO_SLOT_OB obstacles must fit in a stage slot");
 constexpr int RQ = 0, Rq = 45, RDYN = 54, RR4 = 74;
 constexpr int RK = 0, RPP = 16, Rpp = 44;   // RPP: rows 0..3 of P_{k+1}, row-major 4x7;  Rpp: p_{k+1}[0..3]
 
@@ -506,7 +511,8 @@ struct ParkSolver {
   // K1, item pass: item i = (obstacle j, stage k), i = j * (N+1) + k, so that consecutive threads work on consecutive
   // stages (contiguous slices of every stacked array).  Evaluates the block (block_eval), hands the 12 doubles the stage
   // assembly needs over in the stage's own slot (offset HO_N * j; the stage pass reads them before it zeroes its Q / q
-  // area) and merges the block's KKT-error / merit partials into the thread's running EvalPart.
+  // area) or, for j >= HO_SLOT_OB, in the workspace rows HO, and merges the block's KKT-error / merit partials into the
+  // thread's running EvalPart.
   // ---------------------------------------------------------------------------------------------------
   OBCA_HD_NI static void block_item_eval(const PkCtx& C, int i, bool do_err, EvalPart& acc) {
     OBCA_LOCALS(C);
@@ -520,11 +526,19 @@ struct ParkSolver {
     sincos(ps, &sn_, &cs_);
     BlockOut B;
     block_eval(C, k, j, X, Y, cs_, sn_, mu_b, S.dw, do_err, true, B);
-    double* const h = &RIC(HO_N * j, k);
+    if (j < HO_SLOT_OB) {
+      double* const h = &RIC(HO_N * j, k);
 #pragma unroll
-    for (int e = 0; e < 6; ++e) h[e] = B.Sxx[e];
+      for (int e = 0; e < 6; ++e) h[e] = B.Sxx[e];
 #pragma unroll
-    for (int e = 0; e < 3; ++e) { h[6 + e] = B.rx3[e]; h[9 + e] = B.gx[e]; }
+      for (int e = 0; e < 3; ++e) { h[6 + e] = B.rx3[e]; h[9 + e] = B.gx[e]; }
+    } else {
+      const int r = HO_N * (j - HO_SLOT_OB);
+#pragma unroll
+      for (int e = 0; e < 6; ++e) WV(HO, r + e, k) = B.Sxx[e];
+#pragma unroll
+      for (int e = 0; e < 3; ++e) { WV(HO, r + 6 + e, k) = B.rx3[e]; WV(HO, r + 9 + e, k) = B.gx[e]; }
+    }
     acc.ok &= B.ok;
     acc.f += B.fobj;
     if (do_err) {
@@ -533,6 +547,32 @@ struct ParkSolver {
       acc.sy += B.sum_y; acc.sz += B.sum_z; acc.th += B.th;
       acc.phi += B.fobj - mu_b * B.lsum;
     }
+  }
+
+  // ---------------------------------------------------------------------------------------------------
+  // K1 with more than HO_SLOT_OB obstacles, between the item and the stage pass: sums the hand-overs of stage k over all
+  // obstacles in index order (slot offsets of obstacles 0..5, then the workspace rows HO), stores the sum in obstacle 0's place
+  // of the slot and zeroes the places of obstacles 1..5.  stage_eval's sum over the slot then gives the same bits (the sum
+  // starts from +0.0, so it is never -0.0, and adding +0.0 leaves it unchanged), and stage_eval itself stays as small as
+  // for up to six obstacles.
+  // ---------------------------------------------------------------------------------------------------
+  OBCA_HD_NI static void fold_far_handover(const PkCtx& C, int k) {
+    OBCA_LOCALS(C);
+    const ParkProblem& P = CTX_P(C);
+    double hs[HO_N];
+#pragma unroll
+    for (int e = 0; e < HO_N; ++e) hs[e] = 0.0;
+    for (int j = 0; j < HO_SLOT_OB; ++j) {
+#pragma unroll
+      for (int e = 0; e < HO_N; ++e) hs[e] += RIC(HO_N * j + e, k);
+    }
+    for (int j = HO_SLOT_OB; j < P.nOb; ++j) {
+#pragma unroll
+      for (int e = 0; e < HO_N; ++e) hs[e] += WV(HO, HO_N * (j - HO_SLOT_OB) + e, k);
+    }
+#pragma unroll
+    for (int e = 0; e < HO_N; ++e) RIC(e, k) = hs[e];
+    for (int i = HO_N; i < HO_N * HO_SLOT_OB; ++i) RIC(i, k) = 0.0;
   }
 
   // ---------------------------------------------------------------------------------------------------
@@ -557,7 +597,8 @@ struct ParkSolver {
     double hs[HO_N];
 #pragma unroll
     for (int e = 0; e < HO_N; ++e) hs[e] = 0.0;
-    for (int j = 0; j < P.nOb; ++j) {
+    const int n_slot = P.nOb < HO_SLOT_OB ? P.nOb : HO_SLOT_OB;      // more obstacles: folded into slot 0 (fold_far_handover)
+    for (int j = 0; j < n_slot; ++j) {
 #pragma unroll
       for (int e = 0; e < HO_N; ++e) hs[e] += RIC(HO_N * j + e, k);
     }
@@ -1482,6 +1523,8 @@ struct ParkSolver {
     const int NS = CTX_N(C) + 1, NI = CTX_P(C).nOb * NS;
     OBCA_FOR_ITEMS(i, NI) block_item_eval(C, i, do_err, ep);
     OBCA_SYNC();
+    // (the same thread handles stage k in both stage loops: no barrier between them)
+    if (CTX_P(C).nOb > HO_SLOT_OB) OBCA_FOR_STAGES(k, NS) fold_far_handover(C, k);
     OBCA_FOR_STAGES(k, NS) { EvalPart e1; stage_eval(C, k, do_err, true, e1); part_merge(ep, e1); }
   }
   OBCA_HD static void recover_phase(const PkCtx& C, StepPart& sp) {

@@ -8,6 +8,7 @@
   artefacts main.jl hands to ParkingSignedDist: rx, ry, ryaw (N+1), xWS (N+1)x4, uWS Nx2.
 * ``reverse_parking_batch`` -- BASELINE config 2: randomised start poses, numpy default_rng(seed).
 * ``reverse_parking_mixed_batch`` -- the same with a seeded horizon per problem (input of parking_solve_mixed).
+* ``parking_lot_*``       -- the reverse-parking slot in a row of parked cars (n_cars + 1 obstacles): scene, batch, point cloud.
 * ``quadcopter_mixed_batch`` -- BASELINE config 4 with a seeded horizon and its sampling time per problem (input of
   quadcopter_solve_mixed).
 """
@@ -172,6 +173,66 @@ def reverse_parking_batch(B, N=80, seed=0):
         rx[i], ry[i], ryaw[i], xWS[i], uWS[i] = warmstart_reverse(x0[i], sc["xF"], N, sc["Ts"], sc["L"])
     sc.update(B=B, N=N, x0=x0, rx=rx, ry=ry, ryaw=ryaw, xWS=xWS, uWS=uWS)
     return sc
+
+
+# ----------------------------------------------------------------------------------------------
+# a row of a car park: the reverse-parking slot between parked cars
+# ----------------------------------------------------------------------------------------------
+LOT_SLOT = 2.6                  # slot width: the target slot is [-1.3, 1.3]
+LOT_CAR = (1.9, 4.6)            # parked car: width, length
+LOT_KERB = 5.0                  # the cars' fronts are on y = 5 (the kerb line of main.jl:99-101)
+
+
+def parking_lot_cars(n_cars):
+    """The parked cars as clockwise rectangles [x_lo, x_hi, y_lo, y_hi], centred in the slots that alternate right and
+    left of the target slot (x = 2.6, -2.6, 5.2, -5.2, ...)."""
+    w, l = LOT_CAR
+    cars = []
+    for i in range(n_cars):
+        c = LOT_SLOT * (i // 2 + 1) * (1 if i % 2 == 0 else -1)
+        cars.append((c - w / 2, c + w / 2, LOT_KERB - l, LOT_KERB))
+    return cars
+
+
+def parking_lot_scenario(n_cars=10):
+    """The "backwards" scene of main.jl:99-108 in a row of a car park: obstacles 1 and 2 (the half-planes beside the slot) are
+    replaced by n_cars parked cars (4 half-spaces each), the far wall (obstacle 3, y >= 11) stays; goal, Ts, XYbounds as in
+    reverse_parking_scenario.  nOb = n_cars + 1, sum(vOb) = 4 n_cars + 1.  Every car lies inside the region of the reference's
+    obstacles 1 and 2, so the start poses and warm starts of reverse_parking_batch stay collision-free."""
+    lOb = [[[x0, y1], [x1, y1], [x1, y0], [x0, y0], [x0, y1]] for x0, x1, y0, y1 in parking_lot_cars(n_cars)]
+    lOb.append([[20, 11], [-20, 11]])
+    vOb = [5] * n_cars + [2]
+    nOb = n_cars + 1
+    A, b = obst_hrep(nOb, vOb, lOb)
+    sc = reverse_parking_scenario()
+    sc.update(nOb=nOb, vOb=np.array(vOb) - 1, A=A, b=b, lOb=lOb)
+    return sc
+
+
+def parking_lot_batch(B, N=80, seed=0, n_cars=10):
+    """reverse_parking_batch (start poses, warm starts) with the obstacles of parking_lot_scenario(n_cars)."""
+    sc = reverse_parking_batch(B, N, seed)
+    lot = parking_lot_scenario(n_cars)
+    for k in ("nOb", "vOb", "A", "b", "lOb"):
+        sc[k] = lot[k]
+    return sc
+
+
+def parking_lot_points(n_cars=10):
+    """The point cloud Hybrid A* plans against in the lot: every car outline sampled at 0.1 m, and the far wall y = 11 at
+    1 m spacing, as main.jl:111-142 samples the reference's obstacles."""
+    ox, oy = [], []
+
+    def line(a, b, n):
+        for t in np.linspace(0.0, 1.0, n + 1):
+            ox.append(a[0] + t * (b[0] - a[0])); oy.append(a[1] + t * (b[1] - a[1]))
+    for x0, x1, y0, y1 in parking_lot_cars(n_cars):
+        nx, ny = int(round((x1 - x0) / 0.1)), int(round((y1 - y0) / 0.1))
+        line((x0, y1), (x1, y1), nx); line((x1, y0), (x0, y0), nx)
+        line((x0, y0), (x0, y1), ny); line((x1, y1), (x1, y0), ny)
+    for i in range(-12, 13):
+        ox.append(float(i)); oy.append(11.0)
+    return np.array(ox), np.array(oy)
 
 
 def reverse_parking_mixed_batch(B, N_range=(40, 80), seed=0, Ns=None):
