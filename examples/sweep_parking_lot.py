@@ -1,11 +1,13 @@
 """The reverse-parking sweep in a row of a car park (obca_b200.scenarios.parking_lot_scenario: n_cars parked cars + the far wall,
 nOb = n_cars + 1 obstacles): plan every start pose with the GPU Hybrid A* against the lot's point cloud (one call,
-obca_plan_parking_warmstart_batch), solve every pose planned OK -- each with the horizon the planner gave it -- in ONE GPU call
-(obca_parking_solve_mixed), and run the reference's acceptance test on every result in one more call.  Poses the planner does not
-plan (no path, or a search that outgrew the device's scratch) are reported, not planned on the host: the host planner's warm-start
-entry knows only the reference's two scenes.
+obca_plan_parking_warmstart_goals), solve every pose planned OK -- each with the horizon the planner gave it -- in ONE GPU call
+(obca_parking_solve_mixed), and run the reference's acceptance test on every result in one more call.  Poses whose search outgrew the
+device's scratch are planned by the host twin (obca_plan_warmstart_cloud_batch); poses without a path are reported.
 
-usage: python examples/sweep_parking_lot.py [B] [n_cars] [seed]      (needs a CUDA device)
+--free-slots: the row of scenarios.parking_lot_free_slots instead -- some parked cars left out -- and each car is sent to one of the
+free slots (car i to slot i mod the number of slots): the planner takes a goal per pose, the solve and the check xF of shape (B, 4).
+
+usage: python examples/sweep_parking_lot.py [B] [n_cars] [seed] [--free-slots]      (needs a CUDA device)
 """
 import os
 import sys
@@ -21,18 +23,23 @@ from obca_b200 import parking, scenarios         # noqa: E402
 from obca_b200.planner import device             # noqa: E402
 
 
-def run(B=64, seed=0, n_cars=10, signed_dist=1, sampleN=3):
-    sc = scenarios.parking_lot_scenario(n_cars)
+def run(B=64, seed=0, n_cars=10, signed_dist=1, sampleN=3, free_slots=False):
+    sc = scenarios.parking_lot_free_slots(n_cars) if free_slots else scenarios.parking_lot_scenario(n_cars)
     rng = np.random.default_rng(seed)
     x0 = np.column_stack([rng.uniform(-9, 9, B), rng.uniform(6.8, 9.3, B), np.zeros(B), np.zeros(B)])      # start poses in the lane, v = 0
-    ox, oy = scenarios.parking_lot_points(n_cars)
+    if free_slots:
+        ox, oy = sc["ox"], sc["oy"]
+        xF = sc["goals"][np.arange(B) % len(sc["goals"])]                                           # car i -> free slot i mod n_slots
+    else:
+        ox, oy = scenarios.parking_lot_points(n_cars)
+        xF = np.tile(sc["xF"], (B, 1))
     Ts = sc["Ts"] / 3 * sampleN
     t0 = time.time()
-    o = device.plan_raw(x0, sc["xF"], ox, oy, Ts, sc["L"], sampleN)
+    o = device.plan_goals_raw(x0, xF, ox, oy, Ts, sc["L"], sampleN, host_fallback=True)
     t_plan = time.time() - t0
     idx = np.flatnonzero(o["status"] == 0)
     out = dict(B=B, n_planned=int(idx.size), status=o["status"].copy(), t_plan=t_plan, t_solve=0.0, n_converged=0, n_clean=0,
-               exitflag=np.zeros(B, int), N=o["N"].copy())
+               exitflag=np.zeros(B, int), N=o["N"].copy(), per_slot=np.bincount(np.arange(B) % len(sc["goals"])).tolist() if free_slots else None)
     if idx.size == 0:
         return out
     Ns = o["N"][idx]
@@ -40,9 +47,9 @@ def run(B=64, seed=0, n_cars=10, signed_dist=1, sampleN=3):
     ryaw = [o["ryaw"][i, :n + 1] for i, n in zip(idx, Ns)]
     xWS = [o["xWS"][i, :4 * (n + 1)].reshape(4, n + 1).T for i, n in zip(idx, Ns)]
     uWS = [o["uWS"][i, :2 * n].reshape(2, n).T for i, n in zip(idx, Ns)]
-    r = parking.parking_solve_mixed(x0[idx], sc["xF"], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"], sc["b"],
+    r = parking.parking_solve_mixed(x0[idx], xF[idx], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"], sc["b"],
                                     rx, ry, ryaw, 0, xWS, uWS, signed_dist)
-    feas, _, _ = parking.check_parking_mixed(x0[idx], sc["xF"], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"],
+    feas, _, _ = parking.check_parking_mixed(x0[idx], xF[idx], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"],
                                              sc["b"], r["xp"], r["up"], r["lp"], r["np"], r["ts"], 0, signed_dist, r["sl"])
     conv = r["exitflag"] == 1
     out.update(t_solve=float(r["time"]), n_converged=int(conv.sum()), n_clean=int((np.asarray(feas)[conv] == 1).sum()))
@@ -51,13 +58,14 @@ def run(B=64, seed=0, n_cars=10, signed_dist=1, sampleN=3):
 
 
 if __name__ == "__main__":
-    a = sys.argv
+    free = "--free-slots" in sys.argv
+    a = [v for v in sys.argv if v != "--free-slots"]
     try:
-        o = run(int(a[1]) if len(a) > 1 else 64, int(a[3]) if len(a) > 3 else 0, int(a[2]) if len(a) > 2 else 10)
+        o = run(int(a[1]) if len(a) > 1 else 64, int(a[3]) if len(a) > 3 else 0, int(a[2]) if len(a) > 2 else 10, free_slots=free)
     except obca_b200.ObcaError as e:
         print("not run:", e); sys.exit(2)
     miss = np.flatnonzero(o["status"] != 0)
     print(f"{o['B']} start poses: {o['n_planned']} planned on the GPU in {o['t_plan']:.2f} s"
           + (f" (not planned: poses {miss.tolist()}, status {o['status'][miss].tolist()})" if miss.size else "")
           + f"; solved in one GPU call in {o['t_solve'] * 1e3:.0f} ms device time: {o['n_converged']} converged, "
-          f"{o['n_clean']} of them pass ParkingConstraints")
+          f"{o['n_clean']} of them pass ParkingConstraints" + (f"; cars per free slot {o['per_slot']}" if free else ""))

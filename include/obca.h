@@ -187,34 +187,55 @@ int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x,
                                 const double* x0, const double* xF, const double* Tsb, const double* lambda,
                                 const double* ob, double R, const obca_opts* opts, int* feasible, double* worst);
 
-/* Hybrid A* warm starts on the GPU: B start poses x0 (3 x B column-major: x, y, yaw) towards one goal xF (x, y, yaw) among the obstacle
- * points (ox[i], oy[i]), i < n_ob, in ONE call -- main.jl:215-248 for each pose, as obca_plan_warmstart_batch of include/obca_planner.h
- * does on host threads, with the same search decisions (the same heuristic map, priorities, insertion order and expansion budget) and
- * the same outputs up to the last bits of sin / cos / atan2 / acos / tan / atan.  One CTA plans one pose at a time (k_plan).
+/* Hybrid A* warm starts on the GPU: B start poses x0 and a goal per pose xF (both 3 x B column-major: x, y, yaw) among the obstacle
+ * points (ox[i], oy[i]), i < n_ob, in ONE call -- main.jl:215-248 for each pose, as obca_plan_warmstart_cloud_batch of
+ * include/obca_planner.h does on host threads, with the same search decisions (the same heuristic maps, priorities, insertion order and
+ * expansion budget) and the same outputs up to the last bits of sin / cos / atan2 / acos / tan / atan.  The heuristic map depends on the
+ * goal only through its grid cell (round(gx / 0.3), round(gy / 0.3)): one CTA per distinct goal cell builds that cell's map on the device
+ * (k_plan_hmap), bit for bit the host's Dijkstra, then one CTA plans one pose at a time (k_plan) against its goal's map.
  *   Ts: the sampling time (> 0) of the warm start; L: wheelbase of the steering extraction; sampleN: down-sampling of the 0.1 m path.
  *   max_expansions <= 0: 200000 (obca_plan_warmstart's budget).
  *   max_nodes: node pool per resident CTA; <= 0 selects 32768 (the demo sweeps insert at most ~4500 nodes per plan).  Device scratch per
  *     resident CTA (4 per SM): max_nodes x 176 bytes + a 4-byte cell table over the search grid (~1 MB for the demo clouds)
  *     + ~0.2 MB of course buffers + 96 x cap x sampleN bytes; about 7.1 MB at the defaults, cap = 512, sampleN = 3.
- *     Device memory of one call: min(B, 4 x SMs) x that scratch -- about 3.7 GB on a 132-SM H100 for B >= 528 at the defaults --
- *     plus the batch's outputs, 72 x B x cap bytes (151 MB at B = 4096, cap = 512), which are copied to the device first (so that
- *     the entries the planner does not write keep the caller's values) and back after the kernel.  All of it is freed before the
- *     call returns.
+ *     Device memory of one call: min(B, 4 x SMs) x that scratch -- about 3.7 GB on a 132-SM H100 for B >= 528 at the defaults --,
+ *     the heuristic maps, distinct goal cells x hxw x hyw x 8 bytes (hxw x hyw: the cloud's extent in 0.3 m cells; 3520 cells, 28 KB per
+ *     goal cell, for the demo "backwards" cloud, 3384 / 27 KB for the 10-car lot), plus the batch's goals and outputs,
+ *     72 x B x cap + 64 x B bytes (151 MB at B = 4096, cap = 512), which are copied to the device first (so that the entries the planner
+ *     does not write keep the caller's values) and back after the kernel.  All of it is freed before the call returns.
  * Outputs, with the stride cap, in the layout of obca_plan_warmstart_batch: rx / ry / ryaw [i*cap ..] (N[i]+1 values), xWS [i*4*cap ..]
  * as (N[i]+1) x 4, uWS [i*2*cap ..] as N[i] x 2 column-major.  Nothing past a problem's own N[i]+1 stages is written.
  * status[i]: OBCA_PLAN_OK (0), OBCA_PLAN_NO_PATH (1), OBCA_PLAN_CAPACITY (2; N[i] holds the horizon, nothing else written), or
  * OBCA_PLAN_POOL_FULL (4): the search outgrew its device scratch and was stopped: it needed more than max_nodes nodes, or -- only for
  * a start pose hundreds of metres from the goal -- an analytic expansion longer than the kernel's 4096-point course buffer (409.6 m).
- * That pose is NOT planned (nothing else written, never a partial path); the host planner can plan it (obca_b200.planner.device.plan_batch
- * does so).
- * expansions[i] (may be NULL): nodes expanded.  plan_seconds (may be NULL): device time of the search kernel.
+ * That pose is NOT planned (nothing else written, never a partial path); the host planner can plan it
+ * (obca_b200.planner.device.plan_goals_batch does so).
+ * expansions[i] (may be NULL): nodes expanded.  plan_seconds (may be NULL): device time of the search kernel k_plan.
  * Return: 0, OBCA_ERR_ARG (B < 0, a null array, n_ob <= 0, Ts <= 0, sampleN < 1, cap < 2; reason in obca_last_error()),
  * OBCA_ERR_NO_DEVICE, OBCA_ERR_CUDA. */
 #define OBCA_PLAN_POOL_FULL 4
+int obca_plan_parking_warmstart_goals(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob,
+                                      double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap,
+                                      const obca_opts* opts, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
+                                      int* N, int* status, int* expansions, double* plan_seconds);
+
+/* The same with ONE goal xF (x, y, yaw) for the whole batch -- the randomised sweeps of main.jl:165-168, as obca_plan_warmstart_batch of
+ * include/obca_planner.h plans them on host threads: obca_plan_parking_warmstart_goals with xF repeated for every pose (one heuristic
+ * map), same outputs, status codes and device memory. */
 int obca_plan_parking_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob,
                                       double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap,
                                       const obca_opts* opts, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
                                       int* N, int* status, int* expansions, double* plan_seconds);
+
+/* The heuristic maps the two entries above build on the device (k_plan_hmap), read back; used by tests and tools/bench_plan_goals.py.
+ * For the cloud (ox, oy, n_ob > 0): mn[2] = (minx, miny), w[2] = (xw, yw) (the map's cell (i, j), 1 <= i <= xw, 1 <= j <= yw, is the grid cell
+ * (i + minx, j + miny)); then, one map per goal g < G (goals: 2 x G column-major, gx, gy), maps[(g * xw + i-1) * yw + j-1] = the 8-connected
+ * distance of that cell from the goal's cell, INF where unreachable -- calc_dist_policy of obca_b200/planner/csrc/obca_plan_core.h, bit
+ * for bit.  map_seconds (may be NULL): device time of k_plan_hmap.  Return: 0, OBCA_ERR_ARG (G < 0, a null array, n_ob <= 0, or fewer
+ * than G x xw x yw entries in cap -- mn and w are written first, so a call with maps = NULL reads the size), OBCA_ERR_NO_DEVICE,
+ * OBCA_ERR_CUDA. */
+int obca_plan_parking_heuristic_maps(int G, const double* goals, const double* ox, const double* oy, int n_ob, const obca_opts* opts,
+                                     long long* mn, int* w, double* maps, long long cap, double* map_seconds);
 
 /* 3-D A* warm starts of the quadcopter flow on the GPU: B start / goal pairs (x0, xF: 3 x B column-major positions, each pair its own)
  * among one obstacle point cloud (ox, oy, oz, n_ob >= 0 points; lo, hi: the bound corners in raw units; reso > 0: the cell size) in ONE

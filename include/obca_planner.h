@@ -6,8 +6,8 @@
  *   the warm-start extraction               main.jl:215-248
  * Same algorithms as the Python restatement obca_b200/planner/ (which documents the reference line by line); the two are tested to
  * produce the same paths (tests/test_planner_native.py).  The reference's planner is host code as well and runs once per problem.
- * GPU twin: obca_plan_parking_warmstart_batch in include/obca.h (libobca.so) plans a batch of start poses in one call with the same search
- * decisions; both libraries compile the algorithm from one source, obca_b200/planner/csrc/obca_plan_core.h.
+ * GPU twins: obca_plan_parking_warmstart_goals / _batch in include/obca.h (libobca.so) plan a batch of start poses in one call with the same
+ * search decisions; both libraries compile the algorithm from one source, obca_b200/planner/csrc/obca_plan_core.h.
  *
  * All arrays are Float64, owned by the caller, column-major where two-dimensional (Julia layout).
  */
@@ -47,6 +47,17 @@ int obca_plan_warmstart(const double* x0, const double* xF, int scenario, double
  * rx / ry / ryaw [i*cap ..], xWS [i*4*cap ..] as (N[i]+1) x 4 column-major, uWS [i*2*cap ..] as N[i] x 2 column-major. */
 int obca_plan_warmstart_batch(int B, const double* x0, const double* xF, int scenario, double Ts, double L, int sampleN, int cap, int nthreads,
                               double* rx, double* ry, double* ryaw, double* xWS, double* uWS, int* N, int* status);
+
+/* The per-pose body of obca_plan_warmstart among any obstacle point cloud (ox[i], oy[i]), i < n_ob, for B start poses x0 and a goal per
+ * pose xF (both 3 x B column-major: x, y, yaw), on nthreads host threads (<= 0: hardware concurrency).  Ts > 0 is the sampling time of the
+ * warm start and L the wheelbase of the steering extraction, both used as given.  Outputs as obca_plan_warmstart_batch, plus
+ * expansions[i] (may be NULL): the nodes pose i's search expanded.  The heuristic's obstacle map is built once per call; its distances
+ * once per pose.  Return OBCA_PLAN_BAD_ARG (nothing written) for B < 0, a null array, n_ob <= 0, Ts <= 0, sampleN < 1 or cap < 2, else
+ * OBCA_PLAN_OK.  With one goal repeated and a demo cloud it writes what obca_plan_warmstart_batch writes, byte for byte.
+ * GPU twin: obca_plan_parking_warmstart_goals in include/obca.h, with the same search decisions and expansion counts. */
+int obca_plan_warmstart_cloud_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L,
+                                    int sampleN, int cap, int nthreads, double* rx, double* ry, double* ryaw, double* xWS, double* uWS, int* N,
+                                    int* status, int* expansions);
 
 /* 3-D grid A* of the quadcopter flow (a_star_3D.jl:49-154, mainQuadcopter.jl:122-135) for B start / goal pairs among one obstacle point
  * cloud, on nthreads host threads (<= 0: hardware concurrency).  The decisions are those of the Python restatement

@@ -15,7 +15,8 @@ SYMBOLS = ["obca_version", "obca_device_count", "obca_last_error", "obca_default
            "obca_parking_eval_batch_dev", "obca_parking_eval_sizes", "obca_last_profile", "obca_last_schedule",
            "obca_last_times", "obca_parking_solve_mixed", "obca_check_parking_mixed",
            "obca_quadcopter_solve_batch", "obca_check_quadcopter", "obca_quadcopter_solve_mixed",
-           "obca_check_quadcopter_mixed", "obca_plan_parking_warmstart_batch", "obca_plan_quadcopter_warmstart_batch"]
+           "obca_check_quadcopter_mixed", "obca_plan_parking_warmstart_batch", "obca_plan_quadcopter_warmstart_batch",
+           "obca_plan_parking_warmstart_goals", "obca_plan_parking_heuristic_maps"]
 
 
 class ObcaOpts(C.Structure):

@@ -1,12 +1,15 @@
-// obca_plan.cu -- the GPU Hybrid A* warm-start producer (obca_plan_parking_warmstart_batch of include/obca.h): k_plan and its entry.
-// Built as its own translation unit WITHOUT FMA contraction (-fmad=false), because the host planner it reproduces is built with
-// -ffp-contract=off; linked into libobca.so next to obca_lib.cu (see __graft_entry__.build()).
+// obca_plan.cu -- the GPU Hybrid A* warm-start producer (obca_plan_parking_warmstart_goals / _batch of include/obca.h): k_plan_hmap,
+// k_plan and their entries.  Built as its own translation unit WITHOUT FMA contraction (-fmad=false), because the host planner it
+// reproduces is built with -ffp-contract=off; linked into libobca.so next to obca_lib.cu (see __graft_entry__.build()).
 //
+// k_plan_hmap: one CTA per distinct goal cell of the call relaxes that cell's heuristic map (hmap_one) in shared memory when it fits,
+// else in place in global memory, and leaves it in global memory for k_plan.
 // k_plan: persistent CTAs of PLAN_THREADS threads take start poses from an atomic counter, so that the short plans (the median plan is
 // about 100 times shorter than the longest) do not wait for the long ones.  Each resident CTA owns its scratch in global memory (cell ->
-// node table, node pool, heap, course and path buffers), reused pose after pose.
+// node table, node pool, heap, course and path buffers), reused pose after pose; each pose reads the map of its own goal cell.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -25,12 +28,27 @@ namespace {
 constexpr int PLAN_THREADS = 128;
 constexpr int PLAN_CTAS_PER_SM = 4;
 constexpr int PLAN_DEFAULT_NODES = 32768;      // 7x the most nodes a plan of the demo sweeps inserts (4493)
+constexpr int HMAP_THREADS = 512;
 
 struct CtaDev {
   __device__ int tid() const { return threadIdx.x; }
   __device__ int nth() const { return blockDim.x; }
   __device__ void sync() const { __syncthreads(); }
+  __device__ int sync_or(int v) const { return __syncthreads_or(v); }
 };
+
+// The heuristic maps: map g from the goal cell (gcell[2g], gcell[2g+1]) into maps + g * xw * yw.  smem: relax in dynamic shared memory
+// (xw * yw doubles) and copy the result out, else relax in place.
+__global__ void __launch_bounds__(HMAP_THREADS) k_plan_hmap(const char* obmap, long minx, long miny, int xw, int yw, const long* gcell,
+                                                            double sqrt2, bool smem, double* maps) {
+  extern __shared__ double hs[];
+  const size_t cells = (size_t)xw * yw;
+  double* out = maps + blockIdx.x * cells;
+  double* d = smem ? hs : out;
+  hmap_one(CtaDev(), obmap, xw, yw, gcell[2 * blockIdx.x] - minx, gcell[2 * blockIdx.x + 1] - miny, sqrt2, d);
+  if (smem)
+    for (size_t k = threadIdx.x; k < cells; k += blockDim.x) out[k] = d[k];
+}
 
 __global__ void __launch_bounds__(PLAN_THREADS) k_plan(int B, PlanConst C, PlanIO io, PlanScratch W0, int* counter) {
   __shared__ PlanSmem sm;
@@ -49,12 +67,37 @@ __global__ void __launch_bounds__(PLAN_THREADS) k_plan(int B, PlanConst C, PlanI
   }
 }
 
+// The maps of the goal cells gcell (2 per map) into dmaps on the stream st, with the obstacle map H copied to the device first (into
+// dbuf, which the caller keeps until the stream is done).  ev0 / ev1 (may be null): recorded around the kernel.
+int launch_hmaps(const HeurGrid& H, const std::vector<long>& gcell, double* dmaps, int dev, cudaStream_t st, DevBuf& dbuf, cudaEvent_t ev0,
+                 cudaEvent_t ev1) {
+  const size_t cells = (size_t)H.xw * H.yw, G = gcell.size() / 2;
+  if (G == 0 || cells == 0) return 0;
+  char* dob;
+  long* dg;
+  DevLayout l;
+  l.in(dob, H.obmap.data(), cells);
+  l.in(dg, gcell.data(), gcell.size());
+  CK(alloc_layout(dbuf, l));
+  CK(l.copy_in(st));
+  int optin = 0;
+  CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const size_t bytes = cells * sizeof(double);
+  const bool smem = bytes <= (size_t)optin;
+  if (smem) CK(cudaFuncSetAttribute(k_plan_hmap, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  if (ev0) CK(cudaEventRecord(ev0, st));
+  k_plan_hmap<<<(unsigned)G, HMAP_THREADS, smem ? bytes : 0, st>>>(dob, H.minx, H.miny, H.xw, H.yw, dg, std::sqrt(2.0), smem, dmaps);
+  CK(cudaGetLastError());
+  if (ev1) CK(cudaEventRecord(ev1, st));
+  return 0;
+}
+
 }  // namespace
 
-extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob,
-                                                 double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap,
-                                                 const obca_opts* opts, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
-                                                 int* N, int* status, int* expansions, double* plan_seconds) {
+// Both warm-start entries: B start poses, goal p at xF + goal_stride * p (3: a goal per pose, 0: one goal for the batch).
+static int plan_warmstart(int B, const double* x0, const double* xF, size_t goal_stride, const double* ox, const double* oy, int n_ob,
+                          double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap, const obca_opts* opts, double* rx,
+                          double* ry, double* ryaw, double* xWS, double* uWS, int* N, int* status, int* expansions, double* plan_seconds) {
   if (B < 0) { obca_set_last_error("B < 0"); return OBCA_ERR_ARG; }
   if (!x0 || !xF || !ox || !oy || !rx || !ry || !ryaw || !xWS || !uWS || !N || !status) {
     obca_set_last_error("null argument"); return OBCA_ERR_ARG;
@@ -71,8 +114,11 @@ extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const 
   if (B == 0) return 0;
   if (max_nodes <= 0) max_nodes = PLAN_DEFAULT_NODES;
 
+  std::vector<double> xFs(3 * (size_t)B);
+  for (int p = 0; p < B; ++p)
+    for (int r = 0; r < 3; ++r) xFs[3 * (size_t)p + r] = xF[goal_stride * p + r];
   PlanSetup S;
-  plan_setup(S, xF, ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap);
+  plan_setup(S, B, xFs.data(), ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap);
   int sms = 0;
   Stream st;
   Event e0, e1;
@@ -82,8 +128,9 @@ extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const 
   CK(cudaEventCreate(&e0.h));
   CK(cudaEventCreate(&e1.h));
   const int grid = B < sms * PLAN_CTAS_PER_SM ? B : sms * PLAN_CTAS_PER_SM;
-  const size_t P = plan_path_max(cap, sampleN), nc = (size_t)S.ob.start.size(), ni = S.ob.ids.size(), nh = S.H.pmap.size();
-  // batch constants: obstacle points, cell grid (CSR), heuristic map, counter
+  const size_t P = plan_path_max(cap, sampleN), nc = (size_t)S.ob.start.size(), ni = S.ob.ids.size();
+  const size_t nh = S.C.hcells * (S.gcell.size() / 2);
+  // batch constants: obstacle points, cell grid (CSR), one heuristic map per distinct goal cell, counter
   double *dox, *doy, *dpmap;
   int *dstart, *dids, *dcounter;
   DevLayout cl;
@@ -91,14 +138,16 @@ extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const 
   cl.in(doy, S.ob.oy.data(), n_ob);
   cl.in(dstart, S.ob.start.data(), nc);
   cl.in(dids, ni > 0 ? S.ob.ids.data() : nullptr, ni > 0 ? ni : 1);
-  cl.in(dpmap, nh > 0 ? S.H.pmap.data() : nullptr, nh > 0 ? nh : 1);
+  cl.add(dpmap, nh > 0 ? nh : 1);
   cl.add(dcounter, 1);
-  DevBuf dconst;
+  DevBuf dconst, dhmap;
   CK(alloc_layout(dconst, cl));
   CK(cl.copy_in(st.h));
   CK(cudaMemsetAsync(dcounter, 0, sizeof(int), st.h));
+  const int hrc = launch_hmaps(S.H, S.gcell, dpmap, dev, st.h, dhmap, nullptr, nullptr);
+  if (hrc) return hrc;
   PlanConst C = S.C;
-  C.grid.start = dstart; C.grid.ids = dids; C.grid.ox = dox; C.grid.oy = doy; C.pmap = dpmap;
+  C.grid.start = dstart; C.grid.ids = dids; C.grid.ox = dox; C.grid.oy = doy; C.pmap = dpmap;      // C.goals / C.hidx below
   // per resident CTA: cell table, node pool, heap, course and path buffers
   PlanScratch W0;
   DevLayout wl;
@@ -119,10 +168,12 @@ extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const 
   CK(cudaMemsetAsync(W0.table, 0xff, C.table_size * grid * sizeof(int), st.h));      // -1: no node
   // inputs / outputs: outputs are copied in first, so that the kernel leaves every entry it does not write as the caller had it
   const size_t cb = (size_t)B * cap;
-  double *dx0, *drx, *dry, *dryaw, *dxWS, *duWS;
-  int *dN, *dst, *dex;
+  double *dx0, *dxF, *drx, *dry, *dryaw, *dxWS, *duWS;
+  int *dhidx, *dN, *dst, *dex;
   DevLayout il;
   il.in(dx0, x0, 3 * (size_t)B);
+  il.in(dxF, xFs.data(), 3 * (size_t)B);
+  il.in(dhidx, S.hidx.data(), B);
   il.inout(drx, rx, cb);
   il.inout(dry, ry, cb);
   il.inout(dryaw, ryaw, cb);
@@ -134,6 +185,7 @@ extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const 
   DevBuf dio;
   CK(alloc_layout(dio, il));
   CK(il.copy_in(st.h));
+  C.goals = dxF; C.hidx = dhidx;
   PlanIO io{dx0, drx, dry, dryaw, dxWS, duWS, dN, dst, dex};
   CK(cudaEventRecord(e0.h, st.h));
   k_plan<<<grid, PLAN_THREADS, 0, st.h>>>(B, C, io, W0, dcounter);
@@ -144,5 +196,59 @@ extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const 
   float ms = 0.f;
   CK(cudaEventElapsedTime(&ms, e0.h, e1.h));
   if (plan_seconds) *plan_seconds = ms * 1e-3;
+  return 0;
+}
+
+extern "C" int obca_plan_parking_warmstart_goals(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob,
+                                                 double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap,
+                                                 const obca_opts* opts, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
+                                                 int* N, int* status, int* expansions, double* plan_seconds) {
+  return plan_warmstart(B, x0, xF, 3, ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap, opts, rx, ry, ryaw, xWS, uWS, N, status,
+                        expansions, plan_seconds);
+}
+
+extern "C" int obca_plan_parking_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob,
+                                                 double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap,
+                                                 const obca_opts* opts, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
+                                                 int* N, int* status, int* expansions, double* plan_seconds) {
+  return plan_warmstart(B, x0, xF, 0, ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap, opts, rx, ry, ryaw, xWS, uWS, N, status,
+                        expansions, plan_seconds);
+}
+
+extern "C" int obca_plan_parking_heuristic_maps(int G, const double* goals, const double* ox, const double* oy, int n_ob, const obca_opts* opts,
+                                                long long* mn, int* w, double* maps, long long cap, double* map_seconds) {
+  if (G < 0) { obca_set_last_error("G < 0"); return OBCA_ERR_ARG; }
+  if (!goals || !ox || !oy || !mn || !w) { obca_set_last_error("null argument"); return OBCA_ERR_ARG; }
+  if (n_ob <= 0) { obca_set_last_error("n_ob <= 0: the planner needs obstacle points"); return OBCA_ERR_ARG; }
+  const std::vector<double> vx(ox, ox + n_ob), vy(oy, oy + n_ob);
+  const HeurGrid H = calc_heur_grid(vx, vy, XY_GRID_RESOLUTION, VEHICLE_RADIUS);
+  mn[0] = H.minx; mn[1] = H.miny; w[0] = H.xw; w[1] = H.yw;
+  const size_t cells = (size_t)H.xw * H.yw;
+  if (!maps || (long long)(cells * G) > cap) { obca_set_last_error("maps: fewer than G x xw x yw entries"); return OBCA_ERR_ARG; }
+  const int dev = opts ? opts->device : 0;
+  const int rc = check_device(dev);
+  if (rc) return rc;
+  if (map_seconds) *map_seconds = 0.0;
+  if (G == 0 || cells == 0) return 0;
+  std::vector<long> gcell(2 * (size_t)G);
+  for (int g = 0; g < G; ++g) heur_goal_cell(goals[2 * (size_t)g], goals[2 * (size_t)g + 1], XY_GRID_RESOLUTION, gcell[2 * g], gcell[2 * g + 1]);
+  Stream st;
+  Event e0, e1;
+  CK(cudaSetDevice(dev));
+  CK(cudaStreamCreateWithFlags(&st.h, cudaStreamNonBlocking));
+  CK(cudaEventCreate(&e0.h));
+  CK(cudaEventCreate(&e1.h));
+  double* dmaps;
+  DevLayout l;
+  l.out(dmaps, maps, cells * G);
+  DevBuf dbuf, dhmap;
+  CK(alloc_layout(dbuf, l));
+  const int hrc = launch_hmaps(H, gcell, dmaps, dev, st.h, dhmap, e0.h, e1.h);
+  if (hrc) return hrc;
+  CK(l.copy_out(st.h));
+  CK(cudaStreamSynchronize(st.h));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e0.h, e1.h));
+  if (map_seconds) *map_seconds = ms * 1e-3;
   return 0;
 }

@@ -1,7 +1,8 @@
 // obca_plan.cuh -- the GPU Hybrid A* search: one CTA plans one start pose at a time (obca_plan.cu), reproducing the host planner's
 // decisions (obca_b200/planner/csrc/obca_planner.cpp) with a binary heap, a cell -> node table and a node pool instead of its hash maps.
-// Written once for a CTA policy `Cta` (tid / nth / sync): the kernel runs it with the threads of a CTA, the development emulation
-// (tests/emul/emul_plan.cpp) with one host thread, so the emulation checks this very source against the host planner bit for bit.
+// Written once for a CTA policy `Cta` (tid / nth / sync / sync_or): the kernel runs it with the threads of a CTA, the development emulation
+// (tests/emul/emul_plan.cpp for one goal, tests/emul/emul_plan_goals.cpp for a goal per pose and the heuristic-map relaxation) with one
+// host thread, so the emulation checks this very source against the host planner bit for bit.
 //
 // One expansion:
 //   1. thread 0 pops the heap (priority cost + H_COST * h, then insertion tick; no trig, so the pops are those of std::priority_queue);
@@ -42,12 +43,15 @@ OBCA_PHD bool heap_less(const HeapItem& a, const HeapItem& b) { return a.pr < b.
 struct PlanConst {
   Config cfg;
   ObGridView grid;
-  const double* pmap;
+  const double* pmap;              // the heuristic maps of the call's distinct goal cells, hcells entries each
   long hminx, hminy;
   int hxw, hyw;
+  size_t hcells;                   // hxw * hyw
+  const double* goals;             // the goals (x, y, yaw): pose p's at goals + 3 * per_pose * p
+  const int* hidx;                 // hidx[per_pose * p]: the heuristic map of pose p's goal cell
+  int per_pose;                    // 1: a goal per pose; 0: goals[0..2] and map 0 for every pose
   double maxc;
   double us[N_MOTION], ds[N_MOTION], tanu[N_MOTION];
-  double goal[3];                  // (gx, gy, pi_2_pi(gyaw))
   long max_expansions;
   int max_nodes;
   long table_size;                 // cells of the cell -> node table
@@ -72,29 +76,84 @@ struct PlanScratch {
 };
 OBCA_PHD size_t plan_path_max(int cap, int sampleN) { return (size_t)cap * sampleN; }
 
-// Host set-up of one call, shared by the batch: obstacle cell grid, heuristic map, primitives.  S.C points into S.ob / S.H (host memory).
+// Host set-up of one call, shared by the batch: obstacle cell grid, the heuristic's obstacle map, the distinct goal cells, primitives.
+// S.C points into S (host memory).  plan_setup(S, B, xF, ...): a goal per pose (xF 3 x B); S.C.pmap is left to the caller, who builds
+// one map per goal cell (hmap_one) in goal-cell order.  plan_setup(S, xF, ...): one goal for every pose, its map built here by the host's
+// Dijkstra (dist_from_goal).
 struct PlanSetup {
   Obstacles ob;
-  DistPolicy H;
+  HeurGrid H;
+  std::vector<double> goals;       // 3 per goal
+  std::vector<long> gcell;         // (g0, g1) of each distinct goal cell, in order of first appearance
+  std::vector<int> hidx;           // the goal cell of each goal
+  std::vector<double> map;         // the one-goal set-up's heuristic map
   PlanConst C;
 };
-inline void plan_setup(PlanSetup& S, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L, int sampleN,
+inline void plan_setup(PlanSetup& S, int B, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L, int sampleN,
                        int max_expansions, int max_nodes, int cap) {
   S.ob.ox.assign(ox, ox + n_ob); S.ob.oy.assign(oy, oy + n_ob); S.ob.build();
   PlanConst& C = S.C;
   C.cfg = calc_config(S.ob.ox, S.ob.oy, XY_GRID_RESOLUTION, YAW_GRID_RESOLUTION);
   C.grid = S.ob.view();
-  S.H = calc_dist_policy(xF[0], xF[1], S.ob.ox, S.ob.oy, XY_GRID_RESOLUTION, VEHICLE_RADIUS);
-  C.pmap = S.H.pmap.data(); C.hminx = S.H.minx; C.hminy = S.H.miny; C.hxw = S.H.xw; C.hyw = S.H.yw;
+  S.H = calc_heur_grid(S.ob.ox, S.ob.oy, XY_GRID_RESOLUTION, VEHICLE_RADIUS);
+  S.goals.assign(xF, xF + 3 * (size_t)B);
+  S.gcell.clear(); S.hidx.assign(B, 0);
+  std::unordered_map<uint64_t, int> seen;
+  for (int p = 0; p < B; ++p) {
+    long g0, g1;
+    heur_goal_cell(xF[3 * (size_t)p], xF[3 * (size_t)p + 1], XY_GRID_RESOLUTION, g0, g1);
+    const uint64_t key = ((uint64_t)(uint32_t)(int32_t)g0 << 32) | (uint32_t)(int32_t)g1;
+    auto f = seen.find(key);
+    if (f == seen.end()) { f = seen.emplace(key, (int)(S.gcell.size() / 2)).first; S.gcell.push_back(g0); S.gcell.push_back(g1); }
+    S.hidx[p] = f->second;
+  }
+  C.pmap = nullptr; C.hminx = S.H.minx; C.hminy = S.H.miny; C.hxw = S.H.xw; C.hyw = S.H.yw; C.hcells = (size_t)S.H.xw * S.H.yw;
+  C.goals = S.goals.data(); C.hidx = S.hidx.data(); C.per_pose = 1;
   C.maxc = max_curvature();
   std::vector<double> us, ds, tanu;
   motion_inputs(us, ds, tanu);
   for (int m = 0; m < N_MOTION; ++m) { C.us[m] = us[m]; C.ds[m] = ds[m]; C.tanu[m] = tanu[m]; }
-  C.goal[0] = xF[0]; C.goal[1] = xF[1]; C.goal[2] = pi_2_pi(xF[2]);
   C.max_expansions = max_expansions > 0 ? max_expansions : 200000;      // obca_plan_warmstart's budget
   C.max_nodes = max_nodes;
   C.table_size = (C.cfg.yaww + 1) * C.cfg.xw * C.cfg.yw;
   C.dt = Ts / sampleN; C.L = L; C.sampleN = sampleN; C.cap = cap;
+}
+inline void plan_setup(PlanSetup& S, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L, int sampleN,
+                       int max_expansions, int max_nodes, int cap) {
+  plan_setup(S, 1, xF, ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap);
+  S.map = dist_from_goal(S.H, S.gcell[0], S.gcell[1]).pmap;
+  S.C.pmap = S.map.data(); S.C.per_pose = 0;
+}
+
+// The heuristic map of one goal cell into d (xw * yw entries, the layout of DistPolicy::pmap); (gi, gj) = the goal cell - (minx, miny),
+// its map coordinates.  d is the fixed point of d(v) = min(d(v), d(u) + c) over the 8 neighbours u of every target v, c = 1 or sqrt2 (the
+// host libm's sqrt(2.0)), relaxed sweep after sweep until a sweep changes nothing.  Round-to-nearest addition is monotone and c >= 1, so
+// the fixed point is unique -- every cell gets the smallest left-to-right sum over its paths from the goal -- and it is what
+// dist_from_goal's Dijkstra computes, bit for bit, whatever the order of the updates.  The goal is a source even when it is blocked or
+// outside the map; targets are the free cells of the strict interior (dist_from_goal's ok()); every other entry stays INF, the goal's
+// own entry 0 when it lies in the map.  Every thread calls it.
+template <class Cta>
+OBCA_PHD void hmap_one(const Cta& cta, const char* obmap, int xw, int yw, long gi, long gj, double sqrt2, double* d) {
+  const int t = cta.tid(), nt = cta.nth(), cells = xw * yw;
+  for (int k = t; k < cells; k += nt) d[k] = (k / yw + 1 == gi && k % yw + 1 == gj) ? 0.0 : pinf();
+  cta.sync();
+  const int MX[8] = {1, 0, -1, 0, -1, -1, 1, 1}, MY[8] = {0, 1, 0, -1, -1, 1, -1, 1};
+  for (;;) {
+    int changed = 0;
+    for (int k = t; k < cells; k += nt) {
+      const int i = k / yw + 1, j = k % yw + 1;
+      if (!(i < xw && j < yw) || obmap[k]) continue;
+      double best = d[k];
+      for (int m = 0; m < 8; ++m) {
+        const int ni = i + MX[m], nj = j + MY[m];
+        const double du = (ni == gi && nj == gj) ? 0.0 : ((1 <= ni && ni <= xw && 1 <= nj && nj <= yw) ? d[(ni - 1) * yw + (nj - 1)] : pinf());
+        const double nc = du + (m < 4 ? 1.0 : sqrt2);
+        if (nc < best) best = nc;
+      }
+      if (best < d[k]) { d[k] = best; changed = 1; }
+    }
+    if (!cta.sync_or(changed)) break;
+  }
 }
 
 // CTA-shared state of one problem.
@@ -102,7 +161,8 @@ struct PlanSmem {
   int status;                      // -1 while searching, else OBCA_PLAN_* / PLAN_NODE_POOL
   int cur, heap_n, n_nodes, rs_n, rs_hit, have_rs, len;
   long tick, expansions, sid;
-  double q[3];
+  double q[3], goal[3];             // goal: (gx, gy, pi_2_pi(gyaw)) of this pose
+  const double* hmap;              // its heuristic map
   RsCand cand[RS_NCAND];
   bool cand_ok[RS_NCAND];
   RsSet set;
@@ -135,17 +195,19 @@ OBCA_PHD HeapItem heap_pop(HeapItem* h, int& n) {
   return top;
 }
 
-OBCA_PHD double node_priority(const PlanConst& C, const PNode& n) {
-  return n.cost + H_COST * heuristic(C.pmap, C.hminx, C.hminy, C.hxw, C.hyw, n.xind, n.yind);
+OBCA_PHD double node_priority(const PlanConst& C, const double* hmap, const PNode& n) {
+  return n.cost + H_COST * heuristic(hmap, C.hminx, C.hminy, C.hxw, C.hyw, n.xind, n.yind);
 }
 
-// Plan problem p: main.jl:215-248 for start pose x0[:, p].  Every thread of the CTA calls it; it ends with a sync.
+// Plan problem p: main.jl:215-248 for start pose x0[:, p] and its goal.  Every thread of the CTA calls it; it ends with a sync.
 template <class Cta>
 OBCA_PHD void plan_one(const Cta& cta, const PlanConst& C, const PlanScratch& W, PlanSmem& sm, const PlanIO& io, int p) {
   const int t = cta.tid(), nt = cta.nth();
   const Config& c = C.cfg;
   if (t == 0) {
-    const double* x0 = io.x0 + 3 * (size_t)p;
+    const double *x0 = io.x0 + 3 * (size_t)p, *xF = C.goals + 3 * (size_t)C.per_pose * p;
+    sm.goal[0] = xF[0]; sm.goal[1] = xF[1]; sm.goal[2] = pi_2_pi(xF[2]);
+    sm.hmap = C.pmap + (size_t)C.hidx[(size_t)C.per_pose * p] * C.hcells;
     PNode& n = W.pool[0];
     const double syaw = pi_2_pi(x0[2]);
     n.np = 1; n.x[0] = x0[0]; n.y[0] = x0[1]; n.yaw[0] = syaw;
@@ -155,7 +217,7 @@ OBCA_PHD void plan_one(const Cta& cta, const PlanConst& C, const PlanScratch& W,
     sm.sid = n.id;
     if (n.id >= 0 && n.id < C.table_size) W.table[n.id] = 0;
     sm.n_nodes = 1; sm.heap_n = 0; sm.tick = 0; sm.expansions = 0; sm.status = -1;
-    heap_push(W.heap, sm.heap_n, HeapItem{node_priority(C, n), 0, 0});
+    heap_push(W.heap, sm.heap_n, HeapItem{node_priority(C, sm.hmap, n), 0, 0});
   }
   for (;;) {
     // Every thread has read sm.status / sm.cur of the previous step (and thread 0's set-up) before thread 0 writes them again: without
@@ -183,7 +245,7 @@ OBCA_PHD void plan_one(const Cta& cta, const PlanConst& C, const PlanScratch& W,
     // ---- 2. analytic expansion: candidate words ----
     {
       double x, y, phi, xb, yb;
-      rs_frame(sm.q, C.goal, C.maxc, x, y, phi, xb, yb);
+      rs_frame(sm.q, sm.goal, C.maxc, x, y, phi, xb, yb);
       for (int j = t; j < RS_NCAND; j += nt) sm.cand_ok[j] = rs_candidate(j, x, y, phi, xb, yb, sm.cand[j]);
     }
     cta.sync();
@@ -266,7 +328,7 @@ OBCA_PHD void plan_one(const Cta& cta, const PlanConst& C, const PlanScratch& W,
         n.parent = sm.cur; n.id = nid; n.state = NODE_OPEN;
         if (nid >= 0 && nid < C.table_size) W.table[nid] = k;
         ++sm.tick;
-        heap_push(W.heap, sm.heap_n, HeapItem{node_priority(C, n), sm.tick, k});
+        heap_push(W.heap, sm.heap_n, HeapItem{node_priority(C, sm.hmap, n), sm.tick, k});
       }
     }
     cta.sync();
@@ -294,7 +356,7 @@ OBCA_PHD void plan_one(const Cta& cta, const PlanConst& C, const PlanScratch& W,
     }
     if (sm.status == OBCA_PLAN_OK) {
       int e = len - 1;
-      W.px[e] = C.goal[0]; W.py[e] = C.goal[1]; W.pyaw[e] = C.goal[2];
+      W.px[e] = sm.goal[0]; W.py[e] = sm.goal[1]; W.pyaw[e] = sm.goal[2];
       for (int i = nrs; i >= 1; --i) { --e; W.px[e] = W.rsx[i]; W.py[e] = W.rsy[i]; W.pyaw[e] = W.rsyaw[i]; }
       for (k = sm.cur;; k = W.pool[k].parent) {
         const PNode& n = W.pool[k];

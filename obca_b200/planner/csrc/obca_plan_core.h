@@ -539,22 +539,30 @@ inline Config calc_config(const std::vector<double>& ox, const std::vector<doubl
   return c;
 }
 
-// grid heuristic (obca_b200/planner/grid_policy.py): exact 8-connected shortest distances from the goal
+// grid heuristic (obca_b200/planner/grid_policy.py): exact 8-connected shortest distances from the goal.  Two parts: the obstacle map,
+// which does not depend on the goal (HeurGrid, built once per cloud), and the distances from one goal cell (dist_from_goal);
+// calc_dist_policy is their composition.  The distances depend on the goal only through its cell heur_goal_cell(gx, gy, reso).
+struct HeurGrid {
+  std::vector<char> obmap;       // [xw][yw], 1 = blocked; entry (i-1, j-1) <-> cell (i + minx, j + miny)
+  long minx = 0, miny = 0;
+  int xw = 0, yw = 0;
+};
 struct DistPolicy {
   std::vector<double> pmap;      // [xw][yw], INF where unreachable; entry (i-1, j-1) <-> cell (i + minx, j + miny)
   long minx = 0, miny = 0;
   int xw = 0, yw = 0;
 };
-inline DistPolicy calc_dist_policy(double gx, double gy, const std::vector<double>& ox, const std::vector<double>& oy, double reso, double vr) {
+OBCA_PHD void heur_goal_cell(double gx, double gy, double reso, long& g0, long& g1) { g0 = jround(gx / reso); g1 = jround(gy / reso); }
+inline HeurGrid calc_heur_grid(const std::vector<double>& ox, const std::vector<double>& oy, double reso, double vr) {
   using std::vector;
-  DistPolicy P;
+  HeurGrid G;
   vector<double> oxs(ox.size()), oys(oy.size());
   for (size_t i = 0; i < ox.size(); ++i) { oxs[i] = ox[i] / reso; oys[i] = oy[i] / reso; }
   const long minx = jround(*std::min_element(oxs.begin(), oxs.end())), miny = jround(*std::min_element(oys.begin(), oys.end()));
   const long maxx = jround(*std::max_element(oxs.begin(), oxs.end())), maxy = jround(*std::max_element(oys.begin(), oys.end()));
   const int xw = (int)(maxx - minx), yw = (int)(maxy - miny);
-  P.minx = minx; P.miny = miny; P.xw = xw; P.yw = yw;
-  vector<char> obmap((size_t)xw * yw, 0);
+  G.minx = minx; G.miny = miny; G.xw = xw; G.yw = yw;
+  G.obmap.assign((size_t)xw * yw, 0);
   const double lim = vr / reso;
   for (int ix = 1; ix <= xw; ++ix)
     for (int iy = 1; iy <= yw; ++iy) {
@@ -564,10 +572,20 @@ inline DistPolicy calc_dist_policy(double gx, double gy, const std::vector<doubl
         const double dx = oxs[k] - cx, dy = oys[k] - cy, d2 = dx * dx + dy * dy;
         if (d2 < best) best = d2;
       }
-      obmap[(size_t)(ix - 1) * yw + (iy - 1)] = std::sqrt(best) <= lim;
+      G.obmap[(size_t)(ix - 1) * yw + (iy - 1)] = std::sqrt(best) <= lim;
     }
+  return G;
+}
+// Dijkstra from the goal cell (g0, g1).  The goal is a source even when it is blocked or outside the map; a target must lie in the strict
+// interior 0 < ix < xw, 0 < iy < yw and be free; pmap is written only inside 1..xw x 1..yw.
+inline DistPolicy dist_from_goal(const HeurGrid& G, long g0, long g1) {
+  using std::vector;
+  DistPolicy P;
+  const long minx = G.minx, miny = G.miny;
+  const int xw = G.xw, yw = G.yw;
+  const vector<char>& obmap = G.obmap;
+  P.minx = minx; P.miny = miny; P.xw = xw; P.yw = yw;
   P.pmap.assign((size_t)xw * yw, pinf());
-  const long g0 = jround(gx / reso), g1 = jround(gy / reso);
   auto ok = [&](long x, long y) {
     const long ix = x - minx, iy = y - miny;
     return 0 < ix && ix < xw && 0 < iy && iy < yw && !obmap[(size_t)(ix - 1) * yw + (iy - 1)];
@@ -599,6 +617,11 @@ inline DistPolicy calc_dist_policy(double gx, double gy, const std::vector<doubl
     }
   }
   return P;
+}
+inline DistPolicy calc_dist_policy(double gx, double gy, const std::vector<double>& ox, const std::vector<double>& oy, double reso, double vr) {
+  long g0, g1;
+  heur_goal_cell(gx, gy, reso, g0, g1);
+  return dist_from_goal(calc_heur_grid(ox, oy, reso, vr), g0, g1);
 }
 
 // The motion primitives (u, d) of hybrid_a_star.jl:402-414 in the order successors are generated, and tan(u) of each.

@@ -83,15 +83,20 @@ struct Node {
   double steer, cost;
   long pind;
 };
+// HG: the heuristic's obstacle map of (ox, oy) at xyreso (calc_heur_grid), which does not depend on the goal; expansions: the nodes
+// expanded, on every outcome.
 int hybrid_astar(double sx, double sy, double syaw, double gx, double gy, double gyaw, const vector<double>& ox, const vector<double>& oy,
-                 double xyreso, double yawreso, long max_expansions, vector<double>& rx, vector<double>& ry, vector<double>& ryaw) {
+                 const HeurGrid& HG, double xyreso, double yawreso, long max_expansions, vector<double>& rx, vector<double>& ry,
+                 vector<double>& ryaw, long& expansions) {
   syaw = pi_2_pi(syaw); gyaw = pi_2_pi(gyaw);
   const Config c = calc_config(ox, oy, xyreso, yawreso);
   Obstacles ob; ob.ox = ox; ob.oy = oy; ob.build();
   const ObGridView grid = ob.view();
   Node nstart{jround(sx / xyreso), jround(sy / xyreso), jround(syaw / yawreso), true, {sx}, {sy}, {syaw}, 0.0, 0.0, -1};
   Node ngoal{jround(gx / xyreso), jround(gy / xyreso), jround(gyaw / yawreso), true, {gx}, {gy}, {gyaw}, 0.0, 0.0, -1};
-  const DistPolicy H = calc_dist_policy(gx, gy, ox, oy, xyreso, VEHICLE_RADIUS);
+  long g0, g1;
+  heur_goal_cell(gx, gy, xyreso, g0, g1);
+  const DistPolicy H = dist_from_goal(HG, g0, g1);
   auto cost_of = [&](const Node& n) { return n.cost + H_COST * heuristic(H.pmap.data(), H.minx, H.miny, H.xw, H.yw, n.xind, n.yind); };
   std::unordered_map<long, Node> open_, closed;
   const long sid = calc_index(nstart.xind, nstart.yind, nstart.yawind, c);
@@ -105,7 +110,7 @@ int hybrid_astar(double sx, double sy, double syaw, double gx, double gy, double
   const int nlist = motion_nlist();
   const double maxc = max_curvature();
   Node final_node;
-  long expansions = 0;
+  expansions = 0;
   for (;;) {
     if (open_.empty() || pq.empty() || expansions > max_expansions) return OBCA_PLAN_NO_PATH;
     const long c_id = std::get<2>(pq.top());
@@ -189,6 +194,56 @@ int obstacle_points(int scenario, vector<double>& ox, vector<double>& oy) {
   return OBCA_PLAN_OK;
 }
 
+// main.jl:215-248 for one start pose x0 and goal xF among the points (ox, oy) whose heuristic obstacle map is HG: Hybrid A*, speed profile,
+// veloSmooth, steering, down-sampling by sampleN.  *expanded (may be null): the nodes expanded.
+int plan_warmstart_one(const double* x0, const double* xF, const vector<double>& ox, const vector<double>& oy, const HeurGrid& HG, double Ts,
+                       double L, int sampleN, int cap, double* rx, double* ry, double* ryaw, double* xWS, double* uWS, int* N_out, int* expanded) {
+  vector<double> px, py, pyaw;
+  long nexp = 0;
+  const int rc = hybrid_astar(x0[0], x0[1], x0[2], xF[0], xF[1], xF[2], ox, oy, HG, XY_GRID_RESOLUTION, YAW_GRID_RESOLUTION, 200000, px, py, pyaw,
+                              nexp);
+  if (expanded) *expanded = (int)nexp;
+  if (rc) return rc;
+  // main.jl:222-248
+  const int n = (int)px.size();
+  const double dt = Ts / sampleN;
+  vector<double> rv(n, 0.0), v(n), a(n > 0 ? n - 1 : 0), work(5 * (size_t)(n + 40));
+  for (int i = 0; i + 1 < n; ++i) rv[i] = ws_speed(px.data(), py.data(), pyaw.data(), i, dt);
+  velo_smooth(rv.data(), n, WS_AMAX, dt, work.data(), v.data(), a.data());
+  vector<double> delta(n > 0 ? n - 1 : 0);
+  for (int i = 0; i + 1 < n; ++i) delta[i] = ws_steer(pyaw.data(), v.data(), i, L);
+  const int ns = (n + sampleN - 1) / sampleN;      // len(rx[::sampleN])
+  *N_out = ns - 1;
+  if (ns > cap || !rx || !ry || !ryaw || !xWS || !uWS) return OBCA_PLAN_CAPACITY;
+  ws_store(px.data(), py.data(), pyaw.data(), v.data(), a.data(), delta.data(), n, sampleN, rx, ry, ryaw, xWS, uWS);
+  return OBCA_PLAN_OK;
+}
+
+// plan_warmstart_one for B poses on nthreads host threads (<= 0: hardware concurrency); pose i's goal is xF + goal_stride * i.  The
+// heuristic's obstacle map is built once for the batch.
+void plan_warmstart_many(int B, const double* x0, const double* xF, size_t goal_stride, const vector<double>& ox, const vector<double>& oy,
+                         double Ts, double L, int sampleN, int cap, int nthreads, double* rx, double* ry, double* ryaw, double* xWS, double* uWS,
+                         int* N, int* status, int* expansions) {
+  const HeurGrid HG = calc_heur_grid(ox, oy, XY_GRID_RESOLUTION, VEHICLE_RADIUS);
+  if (nthreads <= 0) nthreads = (int)std::thread::hardware_concurrency();
+  if (nthreads < 1) nthreads = 1;
+  if (nthreads > B) nthreads = B > 0 ? B : 1;
+  std::atomic<int> next(0);
+  auto work = [&]() {
+    for (;;) {
+      const int i = next.fetch_add(1);
+      if (i >= B) break;
+      status[i] = plan_warmstart_one(x0 + 3 * (size_t)i, xF + goal_stride * i, ox, oy, HG, Ts, L, sampleN, cap, rx + (size_t)i * cap,
+                                     ry + (size_t)i * cap, ryaw + (size_t)i * cap, xWS + (size_t)i * 4 * cap, uWS + (size_t)i * 2 * cap, N + i,
+                                     expansions ? expansions + i : nullptr);
+    }
+  };
+  vector<std::thread> pool;
+  for (int t = 1; t < nthreads; ++t) pool.emplace_back(work);
+  work();
+  for (auto& t : pool) t.join();
+}
+
 }  // namespace
 
 extern "C" {
@@ -199,8 +254,10 @@ int obca_hybrid_astar(double sx, double sy, double syaw, double gx, double gy, d
                       double xyreso, double yawreso, int max_expansions, int cap, double* rx, double* ry, double* ryaw, int* n_out) {
   if (!ox || !oy || n_ob <= 0 || !n_out) return OBCA_PLAN_BAD_ARG;
   vector<double> vx(ox, ox + n_ob), vy(oy, oy + n_ob), px, py, pyaw;
-  const int rc = hybrid_astar(sx, sy, syaw, gx, gy, gyaw, vx, vy, xyreso > 0 ? xyreso : XY_GRID_RESOLUTION, yawreso > 0 ? yawreso : YAW_GRID_RESOLUTION,
-                              max_expansions > 0 ? max_expansions : 200000, px, py, pyaw);
+  const double xy = xyreso > 0 ? xyreso : XY_GRID_RESOLUTION;
+  long nexp;
+  const int rc = hybrid_astar(sx, sy, syaw, gx, gy, gyaw, vx, vy, calc_heur_grid(vx, vy, xy, VEHICLE_RADIUS), xy,
+                              yawreso > 0 ? yawreso : YAW_GRID_RESOLUTION, max_expansions > 0 ? max_expansions : 200000, px, py, pyaw, nexp);
   if (rc) return rc;
   *n_out = (int)px.size();
   if ((int)px.size() > cap || !rx || !ry || !ryaw) return OBCA_PLAN_CAPACITY;
@@ -224,45 +281,36 @@ int obca_plan_warmstart(const double* x0, const double* xF, int scenario, double
   if (!x0 || !xF || !N_out || sampleN < 1) return OBCA_PLAN_BAD_ARG;
   if (Ts <= 0) Ts = (scenario == 0 ? 0.6 : 0.9) / 3 * sampleN;
   if (L <= 0) L = 2.7;
-  vector<double> ox, oy, px, py, pyaw;
-  int rc = obstacle_points(scenario, ox, oy);
+  vector<double> ox, oy;
+  const int rc = obstacle_points(scenario, ox, oy);
   if (rc) return rc;
-  rc = hybrid_astar(x0[0], x0[1], x0[2], xF[0], xF[1], xF[2], ox, oy, XY_GRID_RESOLUTION, YAW_GRID_RESOLUTION, 200000, px, py, pyaw);
-  if (rc) return rc;
-  // main.jl:222-248
-  const int n = (int)px.size();
-  const double dt = Ts / sampleN;
-  vector<double> rv(n, 0.0), v(n), a(n > 0 ? n - 1 : 0), work(5 * (size_t)(n + 40));
-  for (int i = 0; i + 1 < n; ++i) rv[i] = ws_speed(px.data(), py.data(), pyaw.data(), i, dt);
-  velo_smooth(rv.data(), n, WS_AMAX, dt, work.data(), v.data(), a.data());
-  vector<double> delta(n > 0 ? n - 1 : 0);
-  for (int i = 0; i + 1 < n; ++i) delta[i] = ws_steer(pyaw.data(), v.data(), i, L);
-  const int ns = (n + sampleN - 1) / sampleN;      // len(rx[::sampleN])
-  *N_out = ns - 1;
-  if (ns > cap || !rx || !ry || !ryaw || !xWS || !uWS) return OBCA_PLAN_CAPACITY;
-  ws_store(px.data(), py.data(), pyaw.data(), v.data(), a.data(), delta.data(), n, sampleN, rx, ry, ryaw, xWS, uWS);
-  return OBCA_PLAN_OK;
+  return plan_warmstart_one(x0, xF, ox, oy, calc_heur_grid(ox, oy, XY_GRID_RESOLUTION, VEHICLE_RADIUS), Ts, L, sampleN, cap, rx, ry, ryaw, xWS,
+                            uWS, N_out, nullptr);
 }
 
 int obca_plan_warmstart_batch(int B, const double* x0, const double* xF, int scenario, double Ts, double L, int sampleN, int cap, int nthreads,
                               double* rx, double* ry, double* ryaw, double* xWS, double* uWS, int* N, int* status) {
   if (B < 0 || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !N || !status || cap < 2) return OBCA_PLAN_BAD_ARG;
-  if (nthreads <= 0) nthreads = (int)std::thread::hardware_concurrency();
-  if (nthreads < 1) nthreads = 1;
-  if (nthreads > B) nthreads = B > 0 ? B : 1;
-  std::atomic<int> next(0);
-  auto work = [&]() {
-    for (;;) {
-      const int i = next.fetch_add(1);
-      if (i >= B) break;
-      status[i] = obca_plan_warmstart(x0 + 3 * (size_t)i, xF, scenario, Ts, L, sampleN, cap, rx + (size_t)i * cap, ry + (size_t)i * cap,
-                                      ryaw + (size_t)i * cap, xWS + (size_t)i * 4 * cap, uWS + (size_t)i * 2 * cap, N + i);
-    }
-  };
-  vector<std::thread> pool;
-  for (int t = 1; t < nthreads; ++t) pool.emplace_back(work);
-  work();
-  for (auto& t : pool) t.join();
+  vector<double> ox, oy;
+  const int rc = sampleN < 1 ? OBCA_PLAN_BAD_ARG : obstacle_points(scenario, ox, oy);
+  if (rc) {      // what obca_plan_warmstart reports for every pose
+    for (int i = 0; i < B; ++i) status[i] = rc;
+    return OBCA_PLAN_OK;
+  }
+  if (Ts <= 0) Ts = (scenario == 0 ? 0.6 : 0.9) / 3 * sampleN;
+  if (L <= 0) L = 2.7;
+  plan_warmstart_many(B, x0, xF, 0, ox, oy, Ts, L, sampleN, cap, nthreads, rx, ry, ryaw, xWS, uWS, N, status, nullptr);
+  return OBCA_PLAN_OK;
+}
+
+int obca_plan_warmstart_cloud_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L,
+                                    int sampleN, int cap, int nthreads, double* rx, double* ry, double* ryaw, double* xWS, double* uWS, int* N,
+                                    int* status, int* expansions) {
+  if (B < 0 || !x0 || !xF || !ox || !oy || n_ob <= 0 || !(Ts > 0) || sampleN < 1 || cap < 2 || !rx || !ry || !ryaw || !xWS || !uWS || !N ||
+      !status)
+    return OBCA_PLAN_BAD_ARG;
+  plan_warmstart_many(B, x0, xF, 3, vector<double>(ox, ox + n_ob), vector<double>(oy, oy + n_ob), Ts, L, sampleN, cap, nthreads, rx, ry, ryaw,
+                      xWS, uWS, N, status, expansions);
   return OBCA_PLAN_OK;
 }
 

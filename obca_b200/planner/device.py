@@ -1,5 +1,6 @@
 """The GPU warm-start producers of libobca.so (include/obca.h), with the search decisions of the host planners (obca_b200.planner.native):
   - obca_plan_parking_warmstart_batch, Hybrid A*: B start poses towards one goal in one call (plan_raw, plan_batch);
+  - obca_plan_parking_warmstart_goals, the same with a goal per pose among any point cloud (plan_goals_raw, plan_goals_batch);
   - obca_plan_quadcopter_warmstart_batch, the 3-D A* of the quadcopter flow: B start / goal pairs in one call (plan_quadcopter_raw,
     plan_quadcopter_batch).
 Without a CUDA device the calls raise.  A search that outgrows the device's scratch comes back as POOL_FULL in `status` (the *_raw
@@ -16,18 +17,15 @@ from . import native
 POOL_FULL = 4
 
 
-def plan_raw(x0s, xF, ox, oy, Ts, L=2.7, sampleN=3, cap=512, max_nodes=0, max_expansions=0, opts=None):
-    """The entry's outputs as arrays (rx, ry, ryaw (B, cap), xWS (B, 4 cap), uWS (B, 2 cap), N, status, expansions, seconds).  The
-    output buffers start as NaN (N as -1): entries the planner does not write stay so."""
+def _plan_call(entry, x0s, xF, ox, oy, Ts, L, sampleN, cap, max_nodes, max_expansions, opts):
     x0s = np.ascontiguousarray(np.asarray(x0s, float)[:, :3]); B = x0s.shape[0]
-    xF = np.ascontiguousarray(np.asarray(xF, float)[:3]); ox = np.ascontiguousarray(ox, float); oy = np.ascontiguousarray(oy, float)
+    ox = np.ascontiguousarray(ox, float); oy = np.ascontiguousarray(oy, float)
     o = dict(rx=np.full((B, cap), np.nan), ry=np.full((B, cap), np.nan), ryaw=np.full((B, cap), np.nan), xWS=np.full((B, 4 * cap), np.nan),
              uWS=np.full((B, 2 * cap), np.nan), N=np.full(B, -1, np.int32), status=np.full(B, -1, np.int32), expansions=np.zeros(B, np.int32))
     secs = C.c_double(0.0)
     opts = opts if opts is not None else _lib.default_opts()
     p = _lib.ptr
-    L_ = _lib.lib()
-    f = L_.obca_plan_parking_warmstart_batch
+    f = getattr(_lib.lib(), entry)
     f.restype = C.c_int
     f.argtypes = [C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 10
     rc = f(B, p(x0s), p(xF), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(cap),
@@ -36,6 +34,58 @@ def plan_raw(x0s, xF, ox, oy, Ts, L=2.7, sampleN=3, cap=512, max_nodes=0, max_ex
     _lib.check(rc)
     o["seconds"] = secs.value
     return o
+
+
+def plan_raw(x0s, xF, ox, oy, Ts, L=2.7, sampleN=3, cap=512, max_nodes=0, max_expansions=0, opts=None):
+    """The entry's outputs as arrays (rx, ry, ryaw (B, cap), xWS (B, 4 cap), uWS (B, 2 cap), N, status, expansions, seconds).  The
+    output buffers start as NaN (N as -1): entries the planner does not write stay so."""
+    xF = np.ascontiguousarray(np.asarray(xF, float)[:3])
+    return _plan_call("obca_plan_parking_warmstart_batch", x0s, xF, ox, oy, Ts, L, sampleN, cap, max_nodes, max_expansions, opts)
+
+
+def plan_goals_raw(x0s, xFs, ox, oy, Ts, L=2.7, sampleN=3, cap=512, max_nodes=0, max_expansions=0, opts=None, host_fallback=False):
+    """obca_plan_parking_warmstart_goals's outputs as arrays, as plan_raw: start poses x0s (B, >= 3), goals xFs (B, >= 3) or one goal
+    (>= 3,) for all.  host_fallback: poses whose search outgrew the device's scratch (POOL_FULL) are planned by the host twin
+    (native.plan_cloud_raw, the same decisions) and their entries replaced by its outputs."""
+    B = np.shape(x0s)[0]
+    xFs = np.asarray(xFs, float)
+    xFs = np.ascontiguousarray(np.broadcast_to(xFs[:3], (B, 3)) if xFs.ndim == 1 else xFs.reshape(B, -1)[:, :3])
+    o = _plan_call("obca_plan_parking_warmstart_goals", x0s, xFs, ox, oy, Ts, L, sampleN, cap, max_nodes, max_expansions, opts)
+    full = np.nonzero(o["status"] == POOL_FULL)[0]
+    if host_fallback and full.size:
+        h = native.plan_cloud_raw(np.asarray(x0s, float)[full], xFs[full], ox, oy, Ts, L, sampleN, cap)
+        for k in ("rx", "ry", "ryaw", "xWS", "uWS", "N", "status", "expansions"):
+            o[k][full] = h[k]
+    return o
+
+
+def plan_goals_batch(x0s, xFs, ox, oy, Ts, L=2.7, sampleN=3, cap=512, max_nodes=0, opts=None):
+    """native.plan_cloud_batch on the GPU: for every start pose x0s[i] and its goal xFs[i] ((B, >= 3), or one goal for all) among the
+    cloud (ox, oy), the dictionary of plan_batch (None where no path was found).  Poses whose search outgrew the device's scratch
+    (POOL_FULL) are planned by the host twin, which makes the same decisions; raises if a pose did not fit `cap`."""
+    o = plan_goals_raw(x0s, xFs, ox, oy, Ts, L, sampleN, cap, max_nodes, 0, opts, host_fallback=True)
+    st = o["status"]
+    if (st > 1).any():
+        raise native.PlannerError(f"obca_plan_parking_warmstart_goals: status {st[st > 1][:5]} at poses {np.nonzero(st > 1)[0][:5]}")
+    return native.warm_starts(o, Ts)
+
+
+def heuristic_maps(goals, ox, oy, opts=None):
+    """The heuristic maps k_plan_hmap builds for the goals (G, >= 2) among the cloud, read back (obca_plan_parking_heuristic_maps):
+    (maps (G, xw, yw), (minx, miny), device seconds of the kernel)."""
+    g = np.ascontiguousarray(np.asarray(goals, float).reshape(len(goals), -1)[:, :2]); G = g.shape[0]
+    ox = np.ascontiguousarray(ox, float); oy = np.ascontiguousarray(oy, float)
+    mn = np.zeros(2, np.int64); w = np.zeros(2, np.int32); secs = C.c_double(0.0)
+    opts = opts if opts is not None else _lib.default_opts()
+    p = _lib.ptr
+    f = _lib.lib().obca_plan_parking_heuristic_maps
+    f.restype = C.c_int
+    f.argtypes = [C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 4 + [C.c_longlong, C.c_void_p]
+    f(G, p(g), p(ox), p(oy), int(ox.size), C.cast(C.byref(opts), C.c_void_p), p(mn), p(w), None, 0, None)      # reads the size
+    m = np.zeros(G * int(w[0]) * int(w[1]))
+    rc = f(G, p(g), p(ox), p(oy), int(ox.size), C.cast(C.byref(opts), C.c_void_p), p(mn), p(w), p(m), m.size, C.cast(C.byref(secs), C.c_void_p))
+    _lib.check(rc)
+    return m.reshape(G, int(w[0]), int(w[1])), (int(mn[0]), int(mn[1])), secs.value
 
 
 def plan_quadcopter_raw(starts, goals, ox, oy, oz, lo, hi, reso, cap=1024, max_nodes=0, opts=None):

@@ -33,6 +33,8 @@ def lib():
         L.obca_plan_warmstart.argtypes = [p, p, i, d, d, i, i, p, p, p, p, p, p]
         L.obca_plan_warmstart_batch.restype = i
         L.obca_plan_warmstart_batch.argtypes = [i, p, p, i, d, d, i, i, i] + [p] * 7
+        L.obca_plan_warmstart_cloud_batch.restype = i
+        L.obca_plan_warmstart_cloud_batch.argtypes = [i, p, p, p, p, i, d, d, i, i, i] + [p] * 8
         L.obca_reeds_shepp_length.restype = d
         L.obca_reeds_shepp_length.argtypes = [d] * 7
         L.obca_astar3d_batch.restype = i
@@ -108,6 +110,46 @@ def plan_batch(x0s, xF, scenario="backwards", workers=0, Ts=None, L=2.7, sampleN
         out.append(dict(rx=rx[i, :n + 1].copy(), ry=ry[i, :n + 1].copy(), ryaw=ryaw[i, :n + 1].copy(), xWS=xWS[i, :4 * (n + 1)].reshape(4, n + 1).T.copy(),
                         uWS=uWS[i, :2 * n].reshape(2, n).T.copy(), N=n, Ts=Ts))
     return out
+
+
+def plan_cloud_raw(x0s, xFs, ox, oy, Ts, L=2.7, sampleN=3, cap=512, workers=0):
+    """obca_plan_warmstart_cloud_batch's outputs as arrays: rx, ry, ryaw (B, cap), xWS (B, 4 cap), uWS (B, 2 cap), N, status, expansions --
+    the layout of device.plan_goals_raw.  x0s (B, >= 3) start poses, xFs (B, >= 3) or (>= 3,) goals, (ox, oy) any point cloud.  The output
+    buffers start as NaN (N as -1)."""
+    x0s = np.ascontiguousarray(np.asarray(x0s, float)[:, :3]); B = x0s.shape[0]
+    xFs = np.asarray(xFs, float)
+    xFs = np.ascontiguousarray(np.broadcast_to(xFs[:3], (B, 3)) if xFs.ndim == 1 else xFs.reshape(B, -1)[:, :3])
+    ox = np.ascontiguousarray(ox, float); oy = np.ascontiguousarray(oy, float)
+    o = dict(rx=np.full((B, cap), np.nan), ry=np.full((B, cap), np.nan), ryaw=np.full((B, cap), np.nan), xWS=np.full((B, 4 * cap), np.nan),
+             uWS=np.full((B, 2 * cap), np.nan), N=np.full(B, -1, np.int32), status=np.full(B, -1, np.int32), expansions=np.zeros(B, np.int32))
+    rc = lib().obca_plan_warmstart_cloud_batch(B, _p(x0s), _p(xFs), _p(ox), _p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(cap),
+                                               int(workers), *[_p(o[k]) for k in ("rx", "ry", "ryaw", "xWS", "uWS", "N", "status", "expansions")])
+    if rc:
+        raise PlannerError(f"obca_plan_warmstart_cloud_batch: {rc}")
+    return o
+
+
+def warm_starts(o, Ts):
+    """The list of dictionaries of plan_batch from raw planner outputs (plan_cloud_raw, device.plan_goals_raw): None where the status is
+    not OK."""
+    out = []
+    for i in range(len(o["status"])):
+        if o["status"][i]:
+            out.append(None); continue
+        n = int(o["N"][i])
+        out.append(dict(rx=o["rx"][i, :n + 1].copy(), ry=o["ry"][i, :n + 1].copy(), ryaw=o["ryaw"][i, :n + 1].copy(),
+                        xWS=o["xWS"][i, :4 * (n + 1)].reshape(4, n + 1).T.copy(), uWS=o["uWS"][i, :2 * n].reshape(2, n).T.copy(), N=n, Ts=Ts))
+    return out
+
+
+def plan_cloud_batch(x0s, xFs, ox, oy, Ts, L=2.7, sampleN=3, cap=512, workers=0):
+    """Hybrid A* warm starts for many start poses, each with its own goal, among any point cloud, on a pool of host threads: the list
+    of dictionaries of plan_batch (None where no path was found).  Ts: the warm start's sampling time (> 0)."""
+    o = plan_cloud_raw(x0s, xFs, ox, oy, Ts, L, sampleN, cap, workers)
+    st = o["status"]
+    if (st > 1).any():
+        raise PlannerError(f"obca_plan_warmstart_cloud_batch: status {st[st > 1][:5]} at poses {np.nonzero(st > 1)[0][:5]}")
+    return warm_starts(o, Ts)
 
 
 def reeds_shepp_length(sx, sy, syaw, gx, gy, gyaw, maxc):

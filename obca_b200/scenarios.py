@@ -8,7 +8,8 @@
   artefacts main.jl hands to ParkingSignedDist: rx, ry, ryaw (N+1), xWS (N+1)x4, uWS Nx2.
 * ``reverse_parking_batch`` -- BASELINE config 2: randomised start poses, numpy default_rng(seed).
 * ``reverse_parking_mixed_batch`` -- the same with a seeded horizon per problem (input of parking_solve_mixed).
-* ``parking_lot_*``       -- the reverse-parking slot in a row of parked cars (n_cars + 1 obstacles): scene, batch, point cloud.
+* ``parking_lot_*``       -- the reverse-parking slot in a row of parked cars (n_cars + 1 obstacles): scene, batch, point cloud;
+                            parking_lot_free_slots: the same row with some cars left out, a goal per free slot.
 * ``quadcopter_mixed_batch`` -- BASELINE config 4 with a seeded horizon and its sampling time per problem (input of
   quadcopter_solve_mixed).
 """
@@ -199,10 +200,14 @@ def parking_lot_scenario(n_cars=10):
     replaced by n_cars parked cars (4 half-spaces each), the far wall (obstacle 3, y >= 11) stays; goal, Ts, XYbounds as in
     reverse_parking_scenario.  nOb = n_cars + 1, sum(vOb) = 4 n_cars + 1.  Every car lies inside the region of the reference's
     obstacles 1 and 2, so the start poses and warm starts of reverse_parking_batch stay collision-free."""
-    lOb = [[[x0, y1], [x1, y1], [x1, y0], [x0, y0], [x0, y1]] for x0, x1, y0, y1 in parking_lot_cars(n_cars)]
+    return _lot_scene(parking_lot_cars(n_cars))
+
+
+def _lot_scene(cars):
+    lOb = [[[x0, y1], [x1, y1], [x1, y0], [x0, y0], [x0, y1]] for x0, x1, y0, y1 in cars]
     lOb.append([[20, 11], [-20, 11]])
-    vOb = [5] * n_cars + [2]
-    nOb = n_cars + 1
+    vOb = [5] * len(cars) + [2]
+    nOb = len(cars) + 1
     A, b = obst_hrep(nOb, vOb, lOb)
     sc = reverse_parking_scenario()
     sc.update(nOb=nOb, vOb=np.array(vOb) - 1, A=A, b=b, lOb=lOb)
@@ -221,18 +226,36 @@ def parking_lot_batch(B, N=80, seed=0, n_cars=10):
 def parking_lot_points(n_cars=10):
     """The point cloud Hybrid A* plans against in the lot: every car outline sampled at 0.1 m, and the far wall y = 11 at
     1 m spacing, as main.jl:111-142 samples the reference's obstacles."""
+    return _lot_points(parking_lot_cars(n_cars))
+
+
+def _lot_points(cars):
     ox, oy = [], []
 
     def line(a, b, n):
         for t in np.linspace(0.0, 1.0, n + 1):
             ox.append(a[0] + t * (b[0] - a[0])); oy.append(a[1] + t * (b[1] - a[1]))
-    for x0, x1, y0, y1 in parking_lot_cars(n_cars):
+    for x0, x1, y0, y1 in cars:
         nx, ny = int(round((x1 - x0) / 0.1)), int(round((y1 - y0) / 0.1))
         line((x0, y1), (x1, y1), nx); line((x1, y0), (x0, y0), nx)
         line((x0, y0), (x0, y1), ny); line((x1, y1), (x1, y0), ny)
     for i in range(-12, 13):
         ox.append(float(i)); oy.append(11.0)
     return np.array(ox), np.array(oy)
+
+
+def parking_lot_free_slots(n_cars=10, free=(0, 3, 5)):
+    """The row of parking_lot_scenario(n_cars) with the parked cars of index `free` left out: several free slots.  The scene
+    (nOb, vOb, A, b, lOb) and the point cloud (ox, oy) hold only the cars that remain.  slots: the x of every free slot, the
+    target slot x = 0 first, then the slots of the cars left out in the order of `free`; goals (n_slots, 4): the goal pose
+    [x_slot, 1.3, pi/2, 0] of each, the reverse-parking goal moved to that slot."""
+    cars = parking_lot_cars(n_cars)
+    kept = [c for i, c in enumerate(cars) if i not in set(free)]
+    sc = _lot_scene(kept)
+    sc["ox"], sc["oy"] = _lot_points(kept)
+    sc["slots"] = np.array([0.0] + [(cars[i][0] + cars[i][1]) / 2 for i in free])
+    sc["goals"] = np.array([[x, 1.3, np.pi / 2, 0.0] for x in sc["slots"]])
+    return sc
 
 
 def reverse_parking_mixed_batch(B, N_range=(40, 80), seed=0, Ns=None):
