@@ -5,7 +5,10 @@ has no Julia; julia/OBCA.jl holds the equivalent ccall shims for the reference t
     down-sampling (main.jl:222-248)  ->  obstHrep (main.jl:252)  ->  ParkingDist and ParkingSignedDist (main.jl:258, 269) on the GPU
     ->  ParkingConstraints (the reference's acceptance test)
 
-usage: python examples/main_parking.py [backwards|parallel] [x0 y0 yaw0]          (needs a CUDA device for the two solves)
+sampleN (last argument, default 3) is the warm-start sampling of main.jl:46-57: Ts = 0.6 / 3 * sampleN ("backwards", 0.9 for
+"parallel").  The reference's own pose at sampleN = 1 gives N = 192.
+
+usage: python examples/main_parking.py [backwards|parallel] [x0 y0 yaw0] [sampleN]          (needs a CUDA device for the two solves)
 """
 import math
 import os
@@ -26,11 +29,12 @@ def main(argv):
     scenario = argv[1] if len(argv) > 1 else "backwards"
     sc = scenarios.reverse_parking_scenario() if scenario == "backwards" else scenarios.parallel_parking_scenario(4)
     x0 = np.array([float(v) for v in argv[2:5]] + [0.0]) if len(argv) >= 5 else np.array([-6.0, 9.5, 0.0, 0.0])       # main.jl:213
+    sampleN = int(argv[-1]) if len(argv) in (3, 6) else 3                                                             # main.jl:46
     xF, L, fixTime = sc["xF"], 2.7, 0
     ego = np.array([3.7, 1.0, 1.0, 1.0])                     # main.jl:72-73
     XYbounds = np.array([-15.0, 15.0, 1.0, 10.0])            # main.jl:209-210
     t0 = time.time()
-    w = warmstart.plan_warm_start(x0, xF, scenario)          # Hybrid A* + main.jl:222-248
+    w = warmstart.plan_warm_start(x0, xF, scenario, sampleN=sampleN)      # Hybrid A* + main.jl:222-248
     if w is None:
         print("Hybrid A*: no path found"); return 1
     N, Ts = w["N"], w["Ts"]

@@ -2,9 +2,11 @@
 solved) as a batch: plan every pose on the host threads (libobca_planner.so), solve all planned problems -- each with the horizon
 N the planner gave it -- in ONE GPU call (obca_parking_solve_mixed), run the reference's acceptance test on every result in one
 more call.  With planner="gpu" (4th argument `gpu`) the poses are planned on the GPU as well, in one call
-(obca_plan_parking_warmstart_batch), with the host planner's search decisions.
+(obca_plan_parking_warmstart_batch), with the host planner's search decisions.  sampleN (5th argument, default 3) is the
+warm-start sampling of main.jl:46-57: Ts = 0.6 / 3 * sampleN ("backwards", 0.9 for "parallel"); sampleN = 1 gives horizons past 127
+steps (the solver takes N <= 319), still solved in one call.
 
-usage: python examples/sweep_parking.py [B] [backwards|parallel] [seed] [host|gpu]      (needs a CUDA device for the solves)
+usage: python examples/sweep_parking.py [B] [backwards|parallel] [seed] [host|gpu] [sampleN]      (needs a CUDA device for the solves)
 """
 import os
 import sys
@@ -20,13 +22,14 @@ from obca_b200 import parking, scenarios                    # noqa: E402
 from obca_b200.planner import device, native, warmstart     # noqa: E402
 
 
-def sweep(B=256, scenario="backwards", seed=0, signed_dist=1, workers=0, planner="host"):
+def sweep(B=256, scenario="backwards", seed=0, signed_dist=1, workers=0, planner="host", sampleN=3):
     sc = scenarios.reverse_parking_scenario() if scenario == "backwards" else scenarios.parallel_parking_scenario(4)
     rng = np.random.default_rng(seed)
     x0 = np.column_stack([rng.uniform(-9, 9, B), rng.uniform(6.8, 9.3, B), np.zeros(B), np.zeros(B)])      # start poses in the lane, v = 0
     ego = np.array([3.7, 1.0, 1.0, 1.0]); XYbounds = np.array([-15.0, 15.0, 1.0, 10.0]); L = 2.7
     t0 = time.time()
-    plans = native.plan_batch(x0, sc["xF"], scenario, workers) if planner == "host" else device.plan_batch(x0, sc["xF"], scenario)
+    plans = (native.plan_batch(x0, sc["xF"], scenario, workers, sampleN=sampleN) if planner == "host" else
+             device.plan_batch(x0, sc["xF"], scenario, sampleN=sampleN))
     t_plan = time.time() - t0
     groups = warmstart.group_by_horizon(plans)
     out = dict(B=B, planned=sum(w is not None for w in plans), groups=len(groups), t_plan=t_plan, t_solve=0.0, converged=0, feasible=0,
@@ -51,7 +54,8 @@ if __name__ == "__main__":
     a = sys.argv
     try:
         planner = a[4] if len(a) > 4 else "host"
-        o = sweep(int(a[1]) if len(a) > 1 else 256, a[2] if len(a) > 2 else "backwards", int(a[3]) if len(a) > 3 else 0, planner=planner)
+        o = sweep(int(a[1]) if len(a) > 1 else 256, a[2] if len(a) > 2 else "backwards", int(a[3]) if len(a) > 3 else 0, planner=planner,
+                  sampleN=int(a[5]) if len(a) > 5 else 3)
     except obca_b200.ObcaError as e:
         print("solve not run:", e); sys.exit(2)
     print(f"{o['B']} start poses: {o['planned']} planned in {o['t_plan']:.2f} s ({'host threads' if planner == 'host' else 'GPU'}), {o['groups']} horizons "

@@ -7,7 +7,10 @@ device's scratch are planned by the host twin (obca_plan_warmstart_cloud_batch);
 --free-slots: the row of scenarios.parking_lot_free_slots instead -- some parked cars left out -- and each car is sent to one of the
 free slots (car i to slot i mod the number of slots): the planner takes a goal per pose, the solve and the check xF of shape (B, 4).
 
-usage: python examples/sweep_parking_lot.py [B] [n_cars] [seed] [--free-slots]      (needs a CUDA device)
+sampleN (4th argument, default 3) is the warm-start sampling of main.jl:46-57: Ts = 0.6 / 3 * sampleN; sampleN = 1 gives horizons
+past 127 steps (the solver takes N <= 319), still solved in one call.
+
+usage: python examples/sweep_parking_lot.py [B] [n_cars] [seed] [sampleN] [--free-slots]      (needs a CUDA device)
 """
 import os
 import sys
@@ -61,7 +64,8 @@ if __name__ == "__main__":
     free = "--free-slots" in sys.argv
     a = [v for v in sys.argv if v != "--free-slots"]
     try:
-        o = run(int(a[1]) if len(a) > 1 else 64, int(a[3]) if len(a) > 3 else 0, int(a[2]) if len(a) > 2 else 10, free_slots=free)
+        o = run(int(a[1]) if len(a) > 1 else 64, int(a[3]) if len(a) > 3 else 0, int(a[2]) if len(a) > 2 else 10,
+                sampleN=int(a[4]) if len(a) > 4 else 3, free_slots=free)
     except obca_b200.ObcaError as e:
         print("not run:", e); sys.exit(2)
     miss = np.flatnonzero(o["status"] != 0)

@@ -82,9 +82,9 @@ void obca_default_opts(obca_opts* o);
  *                        exitflag (1 = converged, 0 = not), iters, kkt_err (Ipopt's scaled NLP error E_0),
  *                        solve_seconds[1] = device time of the solve alone -- the reference's `time` (:239-241, :297) is
  *                        the wall time of solve(m), which excludes DualMultWS (:219); obca_last_times() gives both.
- * shape bounds: 1 <= nOb <= 16 obstacles, 1 <= vOb[j] <= 4 half-spaces per obstacle, sum(vOb) <= 64, 2 <= N, N + 1 <= 128;
- *                        another shape returns OBCA_ERR_ARG (OBCA_ERR_UNSUPPORTED for a longer horizon) with the bound in
- *                        obca_last_error() and writes no output.  */
+ * shape bounds: 1 <= nOb <= 16 obstacles, 1 <= vOb[j] <= 4 half-spaces per obstacle, sum(vOb) <= 64, 2 <= N <= 319
+ *                        (N + 1 <= 320 stages); another shape returns OBCA_ERR_ARG (OBCA_ERR_UNSUPPORTED for a longer horizon)
+ *                        with the bound in obca_last_error(), before any device work, and writes no output.  */
 int obca_parking_solve_batch(int B, int N, int nOb, const int* vOb, const double* A, const double* b,
                              const double* x0, const double* xF, double Ts, double L, const double* ego,
                              const double* XYbounds, const double* rx, const double* ry, const double* ryaw,
@@ -110,7 +110,8 @@ int obca_parking_solve_batch_dev(int B, int N, int nOb, const int* vOb, const do
  * the first Nb[b] control rows of them.  The solver never reads input entries past that point and never writes output
  * entries past it.  Problem b's results (outputs over its own horizon, exitflag, iters, kkt_err) are bit-identical to
  * solving it with obca_parking_solve_batch at N = Nb[b] and the same options.  Nb = NULL or an Nb[b] outside [2, Nmax]:
- * OBCA_ERR_ARG.  Shape bounds as for obca_parking_solve_batch (nOb <= 16, vOb[j] <= 4, sum(vOb) <= 64, Nmax + 1 <= 128).
+ * OBCA_ERR_ARG.  Shape bounds as for obca_parking_solve_batch (nOb <= 16, vOb[j] <= 4, sum(vOb) <= 64); Nmax > 319 returns
+ * OBCA_ERR_UNSUPPORTED whatever the problems' own horizons, before any device work and with no output written.
  * obca_last_times / obca_last_schedule / obca_last_profile report this call like any other. */
 int obca_parking_solve_mixed(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
                              const double* x0, const double* xF, double Ts, double L, const double* ego,

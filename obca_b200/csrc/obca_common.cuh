@@ -23,6 +23,9 @@
 #define OBCA_MAX_OB 16     // obstacles per problem
 #define OBCA_MAX_ROWS 64   // total half-spaces (sum vOb)
 #define OBCA_VMAX 4        // half-spaces per obstacle supported by the kernels (templates instantiate 2 and 4)
+// parking horizon: k_pk_eval and k_pk_tail hold the N + 1 stage slots of a problem (656 bytes each) in dynamic shared memory;
+// 320 of them (210 KB) leave room for the kernels' static shared memory under the H100's 227 KB per CTA
+#define OBCA_PK_NMAX 319
 
 namespace obca {
 

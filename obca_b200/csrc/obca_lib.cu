@@ -368,8 +368,21 @@ template <int VM, bool SDV>
 static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, const BatchPtrs& bp, int mode) {
   PkLay L = make_layout(P, LocalDims<VM, SDV>::NFAC);
   const int B = bp.B, NS = P.N + 1;
-  if (NS > 128) { set_err("horizon too long for this build (N+1 <= 128)"); return OBCA_ERR_UNSUPPORTED; }
   const size_t smem_slots = (size_t)NS * RSTRIDE * sizeof(double);
+  {   // the entries check N <= OBCA_PK_NMAX, which is sized for the H100: a device with less shared memory per CTA refuses here
+    int dev = 0, optin = 0;
+    cudaFuncAttributes fe, ft;
+    CK(cudaGetDevice(&dev));
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    CK(cudaFuncGetAttributes(&fe, k_pk_eval<VM, SDV>));
+    CK(cudaFuncGetAttributes(&ft, k_pk_tail<VM, SDV>));
+    const size_t st = fe.sharedSizeBytes > ft.sharedSizeBytes ? fe.sharedSizeBytes : ft.sharedSizeBytes;
+    if (smem_slots + st > (size_t)optin) {
+      set_err("horizon too long for this device: N + 1 = " + std::to_string(NS) + " stage slots need " + std::to_string(smem_slots + st) +
+              " bytes of shared memory per CTA, the device allows " + std::to_string(optin));
+      return OBCA_ERR_UNSUPPORTED;
+    }
+  }
   CK(cudaFuncSetAttribute(k_pk_eval<VM, SDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_slots));
   CK(cudaFuncSetAttribute(k_pk_tail<VM, SDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_slots));
   const size_t smem_sweep = (size_t)SWEEP_WARPS * SWEEP_WARP_DOUBLES * sizeof(double);
@@ -521,20 +534,20 @@ static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, cons
 }
 
 static int solve_dev_impl(DevCtx& c, const ParkProblem& P, const IpmOpts& O, BatchPtrs bp, double* seconds) {
-  {  // problem, options and workspace layout -> __constant__ memory (stream-ordered with the kernels below)
-    const PkLay Lc = make_layout(P, nfac_for(P));
-    CK(cudaMemcpyToSymbolAsync(c_pkP, &P, sizeof(P), 0, cudaMemcpyHostToDevice, c.st));
-    CK(cudaMemcpyToSymbolAsync(c_pkO, &O, sizeof(O), 0, cudaMemcpyHostToDevice, c.st));
-    CK(cudaMemcpyToSymbolAsync(c_pkL, &Lc, sizeof(Lc), 0, cudaMemcpyHostToDevice, c.st));
-  }
+  // problem, options and workspace layout -> __constant__ memory (stream-ordered with the kernels below)
+  const PkLay Lc = make_layout(P, nfac_for(P));
+  CK(cudaMemcpyToSymbolAsync(c_pkP, &P, sizeof(P), 0, cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyToSymbolAsync(c_pkO, &O, sizeof(O), 0, cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyToSymbolAsync(c_pkL, &Lc, sizeof(Lc), 0, cudaMemcpyHostToDevice, c.st));
   CK(cudaMemsetAsync(c.prof, 0, 8 * sizeof(unsigned long long), c.st));
   bp.prof = c.prof;
   for (int i = 0; i < 4; ++i) c.phase_ms[i] = 0.0;
   int rc;
   const int mode = env_int("OBCA_MODE", 0);
   // large batches are solved in chunks so that the per-problem workspace (0.19 MB for config 2, 0.6 MB at 11 obstacles, N = 80;
-  // INTEGRATION.md section 3a) stays within a few GB
-  const int chunk = env_int("OBCA_CHUNK", 16384);
+  // INTEGRATION.md section 3a) stays within a few GB.  Past NSP = 128 doubles per row the chunk shrinks with the row length, so
+  // that no shape needs more memory per chunk than it does at N = 127.
+  const int chunk = env_int("OBCA_CHUNK", Lc.NSP > 128 ? 16384 * 128 / Lc.NSP : 16384);
   const int NSc = P.N + 1, Vc = P.V, nObc = P.nOb;
   rc = 0;
   for (int b0 = 0; b0 < bp.B && rc == 0; b0 += chunk) {
@@ -596,6 +609,15 @@ static int launch_quad(DevCtx& c, const QuadProblem& P, const IpmOpts& O, const 
   return 0;
 }
 
+// The parking solver's horizon bound, checked by every solve entry before any device work: a refused call launches nothing and
+// writes no output.
+static int check_park_horizon(int N) {
+  if (N <= OBCA_PK_NMAX) return 0;
+  set_err("horizon too long for the parking solver: N = " + std::to_string(N) + " > " + std::to_string(OBCA_PK_NMAX) +
+          " (N + 1 <= " + std::to_string(OBCA_PK_NMAX + 1) + " stages)");
+  return OBCA_ERR_UNSUPPORTED;
+}
+
 // The parking solve behind the device- and host-pointer entries.  Every per-problem array is laid out for the horizon N;
 // Nb (device pointer, optional): per-problem horizons <= N, problem b uses the first Nb[b] + 1 stages of its arrays.
 static int parking_solve_dev(int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b,
@@ -609,8 +631,10 @@ static int parking_solve_dev(int B, int N, const int* Nb, int nOb, const int* vO
       !up || !ts || !lp || !np || !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
   ParkProblem P;
   if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
+  int rc = check_park_horizon(N);
+  if (rc) return rc;
   DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
+  rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
   IpmOpts O = to_ipm(opts);
@@ -674,6 +698,8 @@ static int parking_solve_host(bool mixed, int B, int N, const int* Nb, int nOb, 
     ParkProblem P;
     if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
   }
+  rc = check_park_horizon(N);
+  if (rc) return rc;
   int V = 0;
   for (int j = 0; j < nOb; ++j) V += vOb[j];
   DevCtx* c;
