@@ -72,6 +72,13 @@ class IpmOptions:
     freeze_degenerate: float = 0.0      # > 0: an always-regularised row whose Jacobian row is below this threshold
                                         # keeps its multiplier this iteration (its linearisation carries no information;
                                         # Newton on |p|^2 = 1 from p = 0, QuadcopterSignedDist.jl:169 with l = 0.05)
+    # index arrays of variables that a solver may carry as ONE variable (the time scale tied by the chain rows
+    # timeScale[k] == timeScale[k+1], which the CUDA solver eliminates, DESIGN.md section 3): their dual residuals count as one
+    # entry, their sum -- the dual infeasibility of the eliminated formulation.  The Newton steps of the two formulations are
+    # the same; only the optimality error, and so the barrier updates and the stopping test, differ.
+    dual_sum_groups: list | None = None
+    snapshots: tuple = ()               # iteration counts K at which IpmResult.snaps[K] keeps the primal z: the z that a run
+                                        # with max_iter = K returns, so one run pins several K
 
 
 @dataclass
@@ -88,6 +95,7 @@ class IpmResult:
     err: float
     mu: float
     log: list = field(default_factory=list)
+    snaps: dict = field(default_factory=dict)
 
 
 class _SparseLDL:
@@ -216,6 +224,12 @@ def solve(nlp, z0, opt: IpmOptions | None = None, yE0=None) -> IpmResult:
         zsum = zLm.sum() + zUm.sum() + vL.sum() + vU.sum()
         sd = max(o.s_max, (ysum + zsum) / max(n_mult, 1)) / o.s_max
         sc = max(o.s_max, zsum / max(n_bmult, 1)) / o.s_max
+        if o.dual_sum_groups:
+            rz = rz.copy()
+            tied = [rz[g].sum() for g in o.dual_sum_groups]
+            for g in o.dual_sum_groups:
+                rz[g] = 0.0
+            rz = np.concatenate([rz, tied])
         dinf = np.abs(rz).max() if n else 0.0
         cinf = max(np.abs(cE).max() if mE else 0.0, np.abs(cI).max() if mI else 0.0)
         pinf = np.abs(comp).max() if comp.size else 0.0
@@ -227,10 +241,13 @@ def solve(nlp, z0, opt: IpmOptions | None = None, yE0=None) -> IpmResult:
     theta_max = 1e4 * max(1.0, th0); theta_min = 1e-4 * max(1.0, th0)
     dw_last = 0.0
     log = []
+    snaps = {}
     status = 0
     err = np.inf
     it = 0
     for it in range(o.max_iter + 1):
+        if it in o.snapshots:
+            snaps[it] = z.copy()
         e0, dinf, cinf, pinf = errors(z, s, yE, zLm, zUm, vL, vU, 0.0)
         err = e0
         if o.verbose:
@@ -394,4 +411,4 @@ def solve(nlp, z0, opt: IpmOptions | None = None, yE0=None) -> IpmResult:
         vL = np.where(sHasL, np.clip(vL, mu / (ks * c), ks * mu / c), 0.0)
         vU = np.where(sHasU, np.clip(vU, mu / (ks * d), ks * mu / d), 0.0)
         log.append(dict(it=it, mu=mu, alpha=alpha, a_du=a_du, dw=dw, nbt=nbt, th=th_k, e0=e0))
-    return IpmResult(z, s, yE, vL, vU, zLm, zUm, status, it, err, mu, log)
+    return IpmResult(z, s, yE, vL, vU, zLm, zUm, status, it, err, mu, log, snaps)

@@ -58,7 +58,9 @@ def stage_order(nlp):
 
 
 def solve_parking(x0, xF, N, Ts, L, ego, XYbounds, nOb, vOb, A, b, rx, ry, ryaw, fixTime, xWS, uWS,
-                  variant="sd", lWS=None, nWS=None, opts=None, verbose=False):
+                  variant="sd", lWS=None, nWS=None, opts=None, verbose=False, one_time_scale=False):
+    """one_time_scale: measure the dual infeasibility of the time scales as that of the one variable t the CUDA solver carries
+    (ipm_ref.IpmOptions.dual_sum_groups): the same Newton steps, and the barrier updates and the stopping test of the kernels."""
     nlp = solver_view(build_parking_nlp(x0, xF, N, Ts, L, ego, XYbounds, nOb, vOb, A, b, rx, ry, ryaw,
                                         fixTime, variant))
     if lWS is None:
@@ -68,6 +70,8 @@ def solve_parking(x0, xF, N, Ts, L, ego, XYbounds, nOb, vOb, A, b, rx, ry, ryaw,
     o.dc_rows = dc_mask(nlp)
     if o.linsolve == "sparse":
         o.order = stage_order(nlp)
+    if one_time_scale and not fixTime:
+        o.dual_sum_groups = [nlp.lay.ts(np.arange(N + 1))]
     o.verbose = verbose
     t0 = time.time()
     res = ipm_ref.solve(nlp, z0, o)

@@ -41,10 +41,49 @@ def test_dualws_kernel_math_vs_oracle(cfg2):
                 assert np.abs(lam - lp[i, k, vo[j]:vo[j + 1]]).max() < 2e-3 and np.abs(mu - npp[i, k, 4 * j:4 * j + 4]).max() < 2e-3
 
 
-@pytest.mark.parametrize("variant,fix", [("sd", 0), ("d", 0), ("sd", 1), ("d", 1)])
-def test_iterates_track_generic_dense_ipm(variant, fix):
+def _oracle_factorizations(log):
+    """Factorizations the oracle's inertia correction needed in the logged iterations (Algorithm IC of ipm_ref.solve with
+    the default dw_first, kw_minus, kw_plus, kw_plus_first), to set against the emulation's count."""
+    n, last = 0, 0.0
+    for e in log:
+        if e["dw"] > 0:
+            start, grow = (1e-4, 100.0) if last == 0.0 else (max(1e-12, last / 3.0), 8.0)
+            n += 1 + int(round(np.log(e["dw"] / start) / np.log(grow)))
+            last = e["dw"]
+        n += 1
+    return n
+
+
+# the shapes of tests/test_gpu_newton_iterates.py (scene, N): its problem 0 against the sparse oracle for K <= 3
+GPU_SHAPES = [("sd", 0, s) for s in (("cfg2", 4), ("cfg2", 7), ("par4", 128), ("lot", 80), ("lot", 200), ("cfg2", 319), ("x16", 319))] + \
+             [("d", 1, ("cfg2", 80)), ("d", 0, ("lot", 200)), ("d", 1, ("par4", 128))]
+
+
+@pytest.mark.parametrize("variant,fix,shape", [pytest.param(v, f, None, id=f"{v}-{f}") for v, f in (("sd", 0), ("d", 0), ("sd", 1), ("d", 1))] +
+                         [pytest.param(v, f, s, id=f"{v}-{f}-{s[0]}{s[1]}") for v, f, s in GPU_SHAPES])
+def test_iterates_track_generic_dense_ipm(variant, fix, shape):
     """K1+K3+K4 (fused eval, condensation, Riccati KKT solve, line search) against the oracle's generic dense
-    Bunch-Kaufman KKT solve: same iterates for the first iterations, same solution at convergence."""
+    Bunch-Kaufman KKT solve: same iterates for the first iterations, same solution at convergence.  With a shape: the
+    first three iterates at the shapes the GPU pins (the sparse oracle, the same inertia corrections)."""
+    if shape is not None:
+        from test_gpu_newton_iterates import scene
+        sc = scene(*shape)
+        sc.update({k: sc[k][:1] for k in ("x0", "rx", "ry", "ryaw", "xWS", "uWS")}, B=1)     # problem 0 alone
+        lp, npp, _, _ = emul.dualmultws_batch(sc)
+        Ts = sc["Ts_fix"] if fix else sc["Ts"]
+        _, res, nlp = solve_parking(sc["x0"][0], sc["xF"], sc["N"], Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"],
+                                    sc["b"], sc["rx"][0], sc["ry"][0], sc["ryaw"][0], fix, sc["xWS"][0], sc["uWS"][0], variant, lp[0], npp[0],
+                                    ipm_ref.IpmOptions(max_iter=3, linsolve="sparse", snapshots=(1, 2, 3)), one_time_scale=True)
+        for K in (1, 2, 3):
+            o = emul.default_opts(); o.max_iter = K
+            r = emul.solve_batch(sc, fix, variant, o, lp, npp)
+            xp, up, ts, lpo, npo, _ = nlp.lay.unpack(res.snaps[K])
+            sp = 1 + max(np.abs(xp).max(), np.abs(up).max(), np.abs(ts).max())
+            sd = 1 + max(np.abs(lpo).max(), np.abs(npo).max())
+            assert max(np.abs(xp - r["xp"][0].T).max(), np.abs(up - r["up"][0].T).max(), np.abs(ts - r["ts"][0]).max()) < 1e-7 * sp, K
+            assert max(np.abs(lpo - r["lp"][0].T).max(), np.abs(npo - r["np"][0].T).max()) < 1e-6 * sd, K
+            assert r["nfact"][0] == _oracle_factorizations(res.log[:K]), K
+        return
     sc = small_batch()
     lp, npp, _, _ = emul.dualmultws_batch(sc)
     i = 0
