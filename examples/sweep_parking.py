@@ -1,8 +1,8 @@
 """The randomised sweep of the reference's AutonomousParking/main.jl:165-168 (many start poses, each planned by Hybrid A* and then
 solved) as a batch: plan every pose on the host threads (libobca_planner.so), solve all planned problems -- each with the horizon
 N the planner gave it -- in ONE GPU call (obca_parking_solve_mixed), run the reference's acceptance test on every result in one
-more call.  With planner="gpu" (4th argument `gpu`) the poses are planned on the GPU as well, in one call
-(obca_plan_parking_warmstart_batch), with the host planner's search decisions.  sampleN (5th argument, default 3) is the
+more call.  With planner="gpu" (4th argument `gpu`) the poses are planned on the GPU as well, with the host planner's search
+decisions, and planned, solved and checked in ONE call (obca_parking_plan_solve_goals) that keeps everything on the device.  sampleN (5th argument, default 3) is the
 warm-start sampling of main.jl:46-57: Ts = 0.6 / 3 * sampleN ("backwards", 0.9 for "parallel"); sampleN = 1 gives horizons past 127
 steps (the solver takes N <= 319), still solved in one call.
 
@@ -27,9 +27,15 @@ def sweep(B=256, scenario="backwards", seed=0, signed_dist=1, workers=0, planner
     rng = np.random.default_rng(seed)
     x0 = np.column_stack([rng.uniform(-9, 9, B), rng.uniform(6.8, 9.3, B), np.zeros(B), np.zeros(B)])      # start poses in the lane, v = 0
     ego = np.array([3.7, 1.0, 1.0, 1.0]); XYbounds = np.array([-15.0, 15.0, 1.0, 10.0]); L = 2.7
+    if planner == "gpu":
+        r = device.plan_solve_batch(x0, sc["xF"], sc["nOb"], sc["vOb"], sc["A"], sc["b"], ego, XYbounds, scenario, sampleN=sampleN, L=L,
+                                    signed_dist=signed_dist, host_fallback=True)
+        ok = r["status"] == 0
+        return dict(B=B, planned=int(ok.sum()), groups=len(set(r["N"][ok].tolist())), t_plan=r["plan_seconds"], t_solve=r["time"],
+                    converged=int((r["exitflag"] == 1).sum()), feasible=int((r["feasible"][ok] == 1).sum()),
+                    exitflag=r["exitflag"].astype(int), N=np.where(ok, r["N"], -1))
     t0 = time.time()
-    plans = (native.plan_batch(x0, sc["xF"], scenario, workers, sampleN=sampleN) if planner == "host" else
-             device.plan_batch(x0, sc["xF"], scenario, sampleN=sampleN))
+    plans = native.plan_batch(x0, sc["xF"], scenario, workers, sampleN=sampleN)
     t_plan = time.time() - t0
     groups = warmstart.group_by_horizon(plans)
     out = dict(B=B, planned=sum(w is not None for w in plans), groups=len(groups), t_plan=t_plan, t_solve=0.0, converged=0, feasible=0,
@@ -58,6 +64,7 @@ if __name__ == "__main__":
                   sampleN=int(a[5]) if len(a) > 5 else 3)
     except obca_b200.ObcaError as e:
         print("solve not run:", e); sys.exit(2)
-    print(f"{o['B']} start poses: {o['planned']} planned in {o['t_plan']:.2f} s ({'host threads' if planner == 'host' else 'GPU'}), {o['groups']} horizons "
-          f"N = {o['N'][o['N'] >= 0].min()}..{o['N'].max()}; solved in one GPU call in {o['t_solve'] * 1e3:.0f} ms device time: "
+    print(f"{o['B']} start poses: {o['planned']} planned in {o['t_plan']:.2f} s ({'host threads' if planner == 'host' else 'GPU device time'}), "
+          f"{o['groups']} horizons N = {o['N'][o['N'] >= 0].min()}..{o['N'].max()}; solved in {'one' if planner == 'host' else 'the same'} GPU "
+          f"call in {o['t_solve'] * 1e3:.0f} ms device time: "
           f"{o['converged']} converged, {o['feasible']} pass ParkingConstraints")

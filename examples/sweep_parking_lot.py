@@ -1,8 +1,8 @@
 """The reverse-parking sweep in a row of a car park (obca_b200.scenarios.parking_lot_scenario: n_cars parked cars + the far wall,
-nOb = n_cars + 1 obstacles): plan every start pose with the GPU Hybrid A* against the lot's point cloud (one call,
-obca_plan_parking_warmstart_goals), solve every pose planned OK -- each with the horizon the planner gave it -- in ONE GPU call
-(obca_parking_solve_mixed), and run the reference's acceptance test on every result in one more call.  Poses whose search outgrew the
-device's scratch are planned by the host twin (obca_plan_warmstart_cloud_batch); poses without a path are reported.
+nOb = n_cars + 1 obstacles), in ONE GPU call that keeps everything on the device (obca_parking_plan_solve_goals): plan every start pose
+with the GPU Hybrid A* against the lot's point cloud, solve every pose planned OK -- each with the horizon the planner gave it -- and
+run the reference's acceptance test on every result.  Poses whose search outgrew the device's scratch are planned by the host twin
+(obca_plan_warmstart_cloud_batch) and solved and checked after the call; poses without a path are reported.
 
 --free-slots: the row of scenarios.parking_lot_free_slots instead -- some parked cars left out -- and each car is sent to one of the
 free slots (car i to slot i mod the number of slots): the planner takes a goal per pose, the solve and the check xF of shape (B, 4).
@@ -22,7 +22,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import obca_b200                                 # noqa: E402
-from obca_b200 import parking, scenarios         # noqa: E402
+from obca_b200 import scenarios                  # noqa: E402
 from obca_b200.planner import device             # noqa: E402
 
 
@@ -38,26 +38,13 @@ def run(B=64, seed=0, n_cars=10, signed_dist=1, sampleN=3, free_slots=False):
         xF = np.tile(sc["xF"], (B, 1))
     Ts = sc["Ts"] / 3 * sampleN
     t0 = time.time()
-    o = device.plan_goals_raw(x0, xF, ox, oy, Ts, sc["L"], sampleN, host_fallback=True)
-    t_plan = time.time() - t0
-    idx = np.flatnonzero(o["status"] == 0)
-    out = dict(B=B, n_planned=int(idx.size), status=o["status"].copy(), t_plan=t_plan, t_solve=0.0, n_converged=0, n_clean=0,
-               exitflag=np.zeros(B, int), N=o["N"].copy(), per_slot=np.bincount(np.arange(B) % len(sc["goals"])).tolist() if free_slots else None)
-    if idx.size == 0:
-        return out
-    Ns = o["N"][idx]
-    rx = [o["rx"][i, :n + 1] for i, n in zip(idx, Ns)]; ry = [o["ry"][i, :n + 1] for i, n in zip(idx, Ns)]
-    ryaw = [o["ryaw"][i, :n + 1] for i, n in zip(idx, Ns)]
-    xWS = [o["xWS"][i, :4 * (n + 1)].reshape(4, n + 1).T for i, n in zip(idx, Ns)]
-    uWS = [o["uWS"][i, :2 * n].reshape(2, n).T for i, n in zip(idx, Ns)]
-    r = parking.parking_solve_mixed(x0[idx], xF[idx], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"], sc["b"],
-                                    rx, ry, ryaw, 0, xWS, uWS, signed_dist)
-    feas, _, _ = parking.check_parking_mixed(x0[idx], xF[idx], Ns, Ts, sc["L"], sc["ego"], sc["XYbounds"], sc["nOb"], sc["vOb"], sc["A"],
-                                             sc["b"], r["xp"], r["up"], r["lp"], r["np"], r["ts"], 0, signed_dist, r["sl"])
-    conv = r["exitflag"] == 1
-    out.update(t_solve=float(r["time"]), n_converged=int(conv.sum()), n_clean=int((np.asarray(feas)[conv] == 1).sum()))
-    out["exitflag"][idx] = r["exitflag"]
-    return out
+    r = device.plan_solve_goals(x0, xF, ox, oy, Ts, sc["nOb"], sc["vOb"], sc["A"], sc["b"], sc["ego"], sc["XYbounds"], sc["L"], sampleN,
+                                signed_dist=signed_dist, host_fallback=True)
+    ok = r["status"] == 0
+    conv = ok & (r["exitflag"] == 1)
+    return dict(B=B, n_planned=int(ok.sum()), status=r["status"].copy(), t_call=time.time() - t0, t_plan=r["plan_seconds"], t_solve=r["time"],
+                n_converged=int(conv.sum()), n_clean=int((r["feasible"][conv] == 1).sum()), exitflag=r["exitflag"].astype(int), N=r["N"].copy(),
+                per_slot=np.bincount(np.arange(B) % len(sc["goals"])).tolist() if free_slots else None)
 
 
 if __name__ == "__main__":
@@ -69,7 +56,8 @@ if __name__ == "__main__":
     except obca_b200.ObcaError as e:
         print("not run:", e); sys.exit(2)
     miss = np.flatnonzero(o["status"] != 0)
-    print(f"{o['B']} start poses: {o['n_planned']} planned on the GPU in {o['t_plan']:.2f} s"
+    print(f"{o['B']} start poses: {o['n_planned']} planned on the GPU in {o['t_plan']:.2f} s device time"
           + (f" (not planned: poses {miss.tolist()}, status {o['status'][miss].tolist()})" if miss.size else "")
-          + f"; solved in one GPU call in {o['t_solve'] * 1e3:.0f} ms device time: {o['n_converged']} converged, "
+          + f"; solved in the same GPU call in {o['t_solve'] * 1e3:.0f} ms device time ({o['t_call']:.2f} s wall clock for the call): "
+          f"{o['n_converged']} converged, "
           f"{o['n_clean']} of them pass ParkingConstraints" + (f"; cars per free slot {o['per_slot']}" if free else ""))

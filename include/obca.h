@@ -12,6 +12,7 @@
  *   obca_check_parking        <- ParkingConstraints.jl:29-149  called from ParkingSignedDist.jl:253,278, ParkingDist.jl:259,277
  *   obca_parking_solve_mixed / obca_check_parking_mixed: the same two for a batch whose problems have different horizons
  *                                 (the Hybrid A* warm starts of main.jl:215-248 each come with their own N)
+ *   obca_parking_plan_solve_goals: main.jl:215-269 (plan -> solve -> accept) for a batch of start poses in one call
  *   obca_quadcopter_solve_batch / obca_check_quadcopter  <- QuadcopterSignedDist.jl / QuadcopterDist.jl / constrSatisfaction.jl
  *   obca_quadcopter_solve_mixed / obca_check_quadcopter_mixed: the same two for a batch whose problems have different
  *                                 horizons and sampling times (the 3-D A* warm starts of mainQuadcopter.jl:122-137 each
@@ -237,6 +238,44 @@ int obca_plan_parking_warmstart_batch(int B, const double* x0, const double* xF,
  * OBCA_ERR_CUDA. */
 int obca_plan_parking_heuristic_maps(int G, const double* goals, const double* ox, const double* oy, int n_ob, const obca_opts* opts,
                                      long long* mn, int* w, double* maps, long long cap, double* map_seconds);
+
+/* main.jl:215-269 for a batch: plan every start pose towards its goal (obca_plan_parking_warmstart_goals), solve every pose that planned
+ * (obca_parking_solve_mixed, DualMultWS inside) and run ParkingConstraints on the results (obca_check_parking_mixed) in ONE call, with
+ * nothing leaving the device between the stages.  All on the library's stream of opts->device:
+ *   1. plan (k_plan_hmap, k_plan) with the stride Ncap + 1 into device buffers, then free the planner's scratch;
+ *   2. list the poses planned OK to a horizon 2 <= N[i] <= Ncap, in pose order; their count and longest horizon Nmax are the only values
+ *      read back before the solve, which is laid out for that Nmax, not for Ncap;
+ *   3. gather those poses' warm starts, x0 and xF into the inputs of the mixed solve;  4. solve;  5. check;
+ *   6. scatter the results to the caller's pose order and copy them back once.
+ * Inputs: the planner's (x0 4 x B: x, y, yaw, v -- the planner reads x, y, yaw and the solve starts from all four --; xF 4 x B, the
+ * planner reads x, y, yaw; the cloud ox, oy, n_ob; Ts, L, sampleN, max_expansions, max_nodes as for obca_plan_parking_warmstart_goals)
+ * and the solve's (nOb, vOb, A, b, ego, XYbounds, fixTime, signed_dist, opts; Ts and L are the solve's too).
+ * Ncap: 2 <= Ncap <= 319, the horizon the caller's arrays hold.  Outputs, in the caller's pose order, in the layout of
+ * obca_parking_solve_mixed with Nmax = Ncap: xp, up, ts, lp, np, sl (may be NULL); kkt_err, exitflag, iters and feasible (the return
+ * value of ParkingConstraints), strict (may be NULL) one per pose; N[i], status[i] and expansions[i] (may be NULL) as the planner writes
+ * them.  status[i]:
+ *   OBCA_PLAN_OK (0)         planned and solved: every output of pose i over its own horizon N[i] is written, nothing past it;
+ *   OBCA_PLAN_NO_PATH (1)    no path: only status and N (as the planner leaves it) are written;
+ *   OBCA_PLAN_POOL_FULL (4)  the search outgrew its device scratch: the same (no host fallback here; obca_b200.planner.device plans such
+ *                            poses on the host);
+ *   OBCA_PLAN_CAPACITY (2)   the planned horizon N[i] is greater than Ncap (or below the solver's 2): N[i] holds it, nothing else.
+ * A pose that is not solved leaves every other output entry as the caller had it.  Pose i's solve, check and outputs are bit-identical
+ * to obca_parking_solve_mixed followed by obca_check_parking_mixed (with sl) on the planner's output for it.  plan_seconds (may be NULL):
+ * device time of k_plan; solve_seconds (may be NULL): as for obca_parking_solve_mixed; obca_last_times / obca_last_schedule report the
+ * solve.  Device memory, freed before the call returns apart from the solve's workspace, which stays with the library as after any
+ * solve: the planner's buffers, 72 x B x (Ncap + 1) + 84 x B bytes; while planning, the planner's scratch on top (about 3.7 GB on a
+ * 132-SM H100 for B >= 528, see obca_plan_parking_warmstart_goals), freed before the solve allocates; then the solve's inputs and outputs
+ * for the Bs poses it takes, about 8 x Bs x (Nmax + 1) x (16 + V + 5 nOb) bytes, its workspace (as obca_parking_solve_mixed at Nmax), and at
+ * the end the caller's outputs, about 8 x B x (Ncap + 1) x (7 + V + 5 nOb) bytes, which are copied to the device first.
+ * Return: 0, OBCA_ERR_ARG (the planner's: B < 0, a null required array, n_ob <= 0, Ts <= 0, sampleN < 1; Ncap < 2; the solver's shape
+ * errors), OBCA_ERR_UNSUPPORTED (Ncap > 319, the bound in obca_last_error()), all before any device work and with nothing written;
+ * OBCA_ERR_NO_DEVICE, OBCA_ERR_CUDA.  B = 0, or a batch in which no pose is solved, returns 0 without launching the solve. */
+int obca_parking_plan_solve_goals(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts,
+                                  double L, int sampleN, int max_expansions, int max_nodes, int nOb, const int* vOb, const double* A,
+                                  const double* b, const double* ego, const double* XYbounds, int fixTime, int signed_dist,
+                                  const obca_opts* opts, int Ncap, double* xp, double* up, double* ts, double* lp, double* np, double* sl,
+                                  int* N, int* status, int* expansions, int* exitflag, int* iters, double* kkt_err, int* feasible,
+                                  int* strict, double* plan_seconds, double* solve_seconds);
 
 /* 3-D A* warm starts of the quadcopter flow on the GPU: B start / goal pairs (x0, xF: 3 x B column-major positions, each pair its own)
  * among one obstacle point cloud (ox, oy, oz, n_ob >= 0 points; lo, hi: the bound corners in raw units; reso > 0: the cell size) in ONE

@@ -146,3 +146,36 @@ function plan_warm_start(x0::AbstractVector, xF::AbstractVector, scenario::Int; 
     n = Int(N[])
     return (rx = rx[1:n+1], ry = ry[1:n+1], ryaw = ryaw[1:n+1], xWS = reshape(xWS[1:4*(n+1)], n + 1, 4), uWS = reshape(uWS[1:2*n], n, 2), N = n)
 end
+
+# ---- plan -> solve -> check for a batch of start poses in one call (include/obca.h: obca_parking_plan_solve_goals) -------------------
+# main.jl:215-269 for B start poses at once, nothing leaving the GPU between the stages.  x0s, xFs: B x 4 matrices (row i = pose i's
+# x0 / xF as main.jl holds them); ox, oy: the planner's obstacle points; the NLP scene as for ParkingSignedDist.  Returns per-pose
+# vectors in main.jl's shapes (xp[i] 4 x (N[i]+1), up[i] 2 x N[i], timeScale[i], lp[i], np[i]) with `nothing` where the pose was not
+# solved, and status (0 solved, 1 no path, 2 horizon over Ncap, 4 planner scratch full), N, exitflag, iters, feasible.
+# Like every stub in this file it is not executed in this repository (no Julia in the build image); the tested twin is
+# obca_b200.planner.device.plan_solve_goals (tests/test_gpu_plan_solve.py).
+function plan_solve_goals(x0s::AbstractMatrix, xFs::AbstractMatrix, ox::AbstractVector, oy::AbstractVector, Ts, L, nOb, vOb, A, b,
+                          ego, XYbounds; sampleN::Int = 3, Ncap::Int = 319, fixTime::Int = 0, signed_dist::Int = 1,
+                          max_nodes::Int = 0, max_expansions::Int = 0)
+    B = size(x0s, 1); V = Int(sum(vOb)); NS = Ncap + 1
+    xp = zeros(4, NS, B); up = zeros(2, Ncap, B); ts = zeros(NS, B); lp = zeros(V, NS, B); np = zeros(4 * nOb, NS, B)
+    sl = zeros(nOb, NS, B); kkt = zeros(B); ps = Ref{Cdouble}(0.0); ss = Ref{Cdouble}(0.0)
+    N = fill(Cint(-1), B); status = fill(Cint(-1), B); expansions = zeros(Cint, B); flag = zeros(Cint, B); iters = zeros(Cint, B)
+    feasible = zeros(Cint, B); strict = zeros(Cint, B)
+    rc = ccall((:obca_parking_plan_solve_goals, LIBOBCA), Cint,
+               (Cint, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint, Cdouble, Cdouble, Cint, Cint, Cint, Cint, Ptr{Cint},
+                Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint, Cint, Ref{ObcaOpts}, Cint, Ptr{Cdouble}, Ptr{Cdouble},
+                Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cint}, Ptr{Cint}, Ptr{Cint}, Ptr{Cint}, Ptr{Cint},
+                Ptr{Cdouble}, Ptr{Cint}, Ptr{Cint}, Ref{Cdouble}, Ref{Cdouble}),
+               B, _f64(permutedims(x0s[:, 1:4])), _f64(permutedims(xFs[:, 1:4])), _f64(ox), _f64(oy), length(ox), Ts, L, sampleN,
+               max_expansions, max_nodes, nOb, Cint.(vec(vOb)), _f64(A), _f64(vec(b)), _f64(vec(ego)), _f64(vec(XYbounds)), fixTime,
+               signed_dist, obca_default_opts(), Ncap, xp, up, ts, lp, np, sl, N, status, expansions, flag, iters, kkt, feasible, strict,
+               ps, ss)
+    rc == 0 || error("obca_parking_plan_solve_goals: ", rc, " ", unsafe_string(ccall((:obca_last_error, LIBOBCA), Cstring, ())))
+    ok = status .== 0
+    cut(a, i, n) = ok[i] ? a[:, 1:n, i] : nothing
+    return (xp = [cut(xp, i, N[i] + 1) for i in 1:B], up = [cut(up, i, N[i]) for i in 1:B],
+            timeScale = [ok[i] ? ts[1:N[i]+1, i] : nothing for i in 1:B], lp = [cut(lp, i, N[i] + 1) for i in 1:B],
+            np = [cut(np, i, N[i] + 1) for i in 1:B], status = status, N = N, exitflag = flag, iters = iters, feasible = feasible,
+            plan_time = ps[], solve_time = ss[])
+end

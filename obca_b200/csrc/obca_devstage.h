@@ -132,3 +132,19 @@ inline cudaError_t alloc_layout(DevBuf& buf, DevLayout& lay) {
 }
 
 }  // namespace obca
+
+// The GPU Hybrid A* of obca_plan.cu, for the entries that plan there and for obca_parking_plan_solve_goals (obca_lib.cu), which keeps
+// the plans on the device.
+// plan_check_args: the planner's argument checks, in the entries' order and with their messages (args: no required array is null).
+int plan_check_args(int B, bool args, int n_ob, double Ts, int sampleN);
+// Device outputs of the planner, in the layout of obca_plan_parking_warmstart_goals with the stride cap.
+struct PlanDevOut {
+  double *rx, *ry, *ryaw, *xWS, *uWS;
+  int *N, *status, *expansions;
+};
+// Plans B >= 1 start poses x0 (host, 3 per pose: x, y, yaw) towards their goals xF (host, 3 per pose) into `out` on the stream st of the
+// current device dev (k_plan_hmap, then k_plan), with arguments that passed plan_check_args and cap >= 2.  Returns once the stream is
+// synchronised, after the planner's device scratch is freed; plan_ms (may be null): device time of k_plan.
+int plan_warmstart_dev(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L,
+                       int sampleN, int max_expansions, int max_nodes, int cap, int dev, cudaStream_t st, const PlanDevOut& out,
+                       float* plan_ms);

@@ -6,6 +6,7 @@
 //   k_quad_solve<SDV>        quadcopter model (config 4): persistent CTA per problem, block-cooperative KKT sweep on FP64 tensor cores (DMMA)
 //   k_dualws<VM>             K2: one thread per (problem, stage, obstacle) micro interior-point solve.
 //   k_check                  K5: ParkingConstraints twin + strict audit, one CTA per problem.
+//   k_flow_list, k_flow_gather, k_flow_scatter   the index maps of obca_parking_plan_solve_goals (obca_flow.h): plans -> solve -> poses
 // There is NO CPU fallback: every compute entry point returns OBCA_ERR_NO_DEVICE without a CUDA device.
 // Host-pointer entries stage their arrays through one device buffer per device (DevCtx::stage), laid out, copied and scattered back
 // with the helpers of obca_devstage.h, which the GPU planners (obca_plan.cu, obca_plan3d.cu) use for their per-call buffers too.
@@ -20,10 +21,12 @@
 #include <vector>
 
 #include "../../include/obca.h"
+#include "../../include/obca_planner.h"
 #include "obca_check.cuh"
 #include "obca_devstage.h"
 #include "obca_dualws.cuh"
 #include "obca_eval.cuh"
+#include "obca_flow.h"
 #include "obca_host.h"
 #include "obca_phased.cuh"
 
@@ -136,6 +139,61 @@ __global__ void k_check(const __grid_constant__ ParkProblem P, int B, const int*
       }
     }
     __syncthreads();
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// plan -> solve -> check without leaving the device (obca_parking_plan_solve_goals): copies along the index maps of obca_flow.h
+// ---------------------------------------------------------------------------------------------------------
+// One CTA lists the poses obca_flow::listed takes, in pose order: list[q] = p, Nb[q] = its horizon; cnt[0] = the count, cnt[1] = the
+// largest listed horizon.  A pose planned OK to a horizon the solver does not take gets OBCA_PLAN_CAPACITY.
+constexpr int FLOW_LIST_THREADS = 1024;
+__global__ void __launch_bounds__(FLOW_LIST_THREADS) k_flow_list(int B, int Ncap, int* __restrict__ status, const int* __restrict__ N,
+                                                                 int* __restrict__ list, int* __restrict__ Nb, int* __restrict__ cnt) {
+  __shared__ int s_warp[FLOW_LIST_THREADS / 32];
+  __shared__ int s_base, s_max;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  if (threadIdx.x == 0) { s_base = 0; s_max = 0; }
+  __syncthreads();
+  for (int p0 = 0; p0 < B; p0 += blockDim.x) {
+    const int p = p0 + threadIdx.x;
+    bool on = false;
+    if (p < B) {
+      const int st = status[p], n = N[p];
+      on = obca_flow::listed(st, n, Ncap);
+      if (st == OBCA_PLAN_OK && !on) status[p] = OBCA_PLAN_CAPACITY;
+      if (on) atomicMax(&s_max, n);
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, on);
+    if (lane == 0) s_warp[warp] = __popc(m);
+    __syncthreads();
+    int off = s_base + __popc(m & ((1u << lane) - 1));
+    for (int w = 0; w < warp; ++w) off += s_warp[w];
+    if (on) { list[off] = p; Nb[off] = N[p]; }
+    __syncthreads();
+    if (threadIdx.x == 0)
+      for (int w = 0; w < nw; ++w) s_base += s_warp[w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) { cnt[0] = s_base; cnt[1] = s_max; }
+}
+
+// One thread per (slot q < Bs, stage k <= M): the planner's outputs and x0 / xF of pose list[q] to the solve's inputs at the horizon M.
+__global__ void k_flow_gather(int Bs, int M, int cap, const int* __restrict__ list, const int* __restrict__ Nb, const obca_flow::Gather g) {
+  const size_t total = (size_t)Bs * (M + 1);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int q = (int)(i / (M + 1)), k = (int)(i % (M + 1));
+    obca_flow::gather_stage(g, q, list[q], Nb[q], k, M, cap);
+  }
+}
+
+// One thread per (slot q < Bs, stage k <= M): the outputs of slot q (at the horizon M) to pose list[q] (at Ncap), its own horizon only.
+__global__ void k_flow_scatter(int Bs, int M, int Ncap, int V, int nOb, const int* __restrict__ list, const int* __restrict__ Nb,
+                               const obca_flow::Outs src, const obca_flow::Outs dst) {
+  const size_t total = (size_t)Bs * (M + 1);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int q = (int)(i / (M + 1)), k = (int)(i % (M + 1));
+    obca_flow::scatter_stage(src, dst, V, nOb, q, list[q], Nb[q], k, M, Ncap);
   }
 }
 
@@ -769,6 +827,16 @@ static int parking_solve_host(bool mixed, int B, int N, const int* Nb, int nOb, 
   return 0;
 }
 
+// ParkingConstraints over B problems on the device's stream (device pointers, laid out for P.N; Nb, sl, e, strict may be null).
+static int check_parking_dev(DevCtx& c, const ParkProblem& P, int B, const int* Nb, const double* x0, const double* xF, const double* x,
+                             const double* u, const double* l, const double* n, const double* ts, const double* sl, int sd, int* feasible,
+                             int* e, int* strict) {
+  const int grid = B < 4 * c.sms ? B : 4 * c.sms;
+  k_check<<<grid, 128, 0, c.st>>>(P, B, Nb, x0, xF, x, u, l, n, ts, sl, sd, feasible, e, strict);
+  CK(cudaGetLastError());
+  return 0;
+}
+
 // ParkingConstraints over a batch (host pointers).  Nb (host pointer, optional): per-problem horizons <= N, with every
 // per-problem array laid out for N.
 static int check_parking(int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b, const double* x0,
@@ -808,9 +876,8 @@ static int check_parking(int B, int N, const int* Nb, int nOb, const int* vOb, c
   lay.place(c->stage);
   cudaStream_t st = c->st;
   CK(lay.copy_in(st));
-  const int grid = B < 4 * c->sms ? B : 4 * c->sms;
-  k_check<<<grid, 128, 0, st>>>(P, B, Nb ? dNb : nullptr, d0, dF, dx, du, dl, dn, dt, sl ? ds : nullptr, sd, dfeas, de, dstrict);
-  CK(cudaGetLastError());
+  rc = check_parking_dev(*c, P, B, Nb ? dNb : nullptr, d0, dF, dx, du, dl, dn, dt, sl ? ds : nullptr, sd, dfeas, de, dstrict);
+  if (rc) return rc;
   CK(lay.copy_out(st));
   CK(cudaStreamSynchronize(st));
   return 0;
@@ -1093,6 +1160,148 @@ int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x,
   rc = check_sampling_times(B, Tsb);
   if (rc) return rc;
   return quad_check_host(B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst);
+}
+
+int obca_parking_plan_solve_goals(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts,
+                                  double L, int sampleN, int max_expansions, int max_nodes, int nOb, const int* vOb, const double* A,
+                                  const double* b, const double* ego, const double* XYbounds, int fixTime, int signed_dist,
+                                  const obca_opts* opts, int Ncap, double* xp, double* up, double* ts, double* lp, double* np, double* sl,
+                                  int* N, int* status, int* expansions, int* exitflag, int* iters, double* kkt_err, int* feasible,
+                                  int* strict, double* plan_seconds, double* solve_seconds) {
+  // the planner's checks, then the solver's, with the messages of the entries this one composes; nothing is written before they pass
+  int rc = plan_check_args(B, x0 && xF && ox && oy && vOb && A && b && ego && XYbounds && xp && up && ts && lp && np && N && status &&
+                                  exitflag && iters && kkt_err && feasible, n_ob, Ts, sampleN);
+  if (rc) return rc;
+  if (Ncap < 2) { set_err("Ncap < 2"); return OBCA_ERR_ARG; }
+  ParkProblem P;
+  if (const int e_ = fill_problem(P, Ncap, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
+  rc = check_park_horizon(Ncap);
+  if (rc) return rc;
+  DevCtx* c;
+  const int dev = opts ? opts->device : 0;
+  rc = get_ctx(dev, &c);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = 0.0;
+  if (solve_seconds) *solve_seconds = 0.0;
+  if (B == 0) return 0;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  cudaStream_t st = c->st;
+  const int V = P.V, cap = Ncap + 1;      // the planner's stride: stages 0..Ncap, so a longer plan comes back as OBCA_PLAN_CAPACITY
+  const size_t Bs = B;
+  // stage 1: plan into device buffers (N is copied in first: the planner leaves it alone where it finds no path)
+  std::vector<double> x03(3 * Bs), xF3(3 * Bs);
+  for (size_t p = 0; p < Bs; ++p)
+    for (int r = 0; r < 3; ++r) { x03[3 * p + r] = x0[4 * p + r]; xF3[3 * p + r] = xF[4 * p + r]; }
+  PlanDevOut po;
+  double *d0, *dF;
+  int *dlist, *dNb, *dcnt;
+  DevLayout pl;
+  pl.add(po.rx, cap * Bs);
+  pl.add(po.ry, cap * Bs);
+  pl.add(po.ryaw, cap * Bs);
+  pl.add(po.xWS, 4 * cap * Bs);
+  pl.add(po.uWS, 2 * cap * Bs);
+  pl.inout(po.N, N, Bs);
+  pl.out(po.status, status, Bs);
+  pl.out(po.expansions, expansions, Bs);
+  pl.in(d0, x0, 4 * Bs);
+  pl.in(dF, xF, 4 * Bs);
+  pl.add(dlist, Bs);
+  pl.add(dNb, Bs);
+  pl.add(dcnt, 2);
+  DevBuf dplan;
+  CK(alloc_layout(dplan, pl));
+  CK(pl.copy_in(st));
+  float plan_ms = 0.f;
+  rc = plan_warmstart_dev(B, x03.data(), xF3.data(), ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap, dev, st, po, &plan_ms);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = plan_ms * 1e-3;
+  // stage 2: list the poses to solve; their count and longest horizon size the solve (its occupancy follows the layout's horizon)
+  k_flow_list<<<1, FLOW_LIST_THREADS, 0, st>>>(B, Ncap, po.status, po.N, dlist, dNb, dcnt);
+  CK(cudaGetLastError());
+  int cnt[2] = {0, 0};
+  CK(to_host(cnt, dcnt, 2, st));
+  CK(cudaStreamSynchronize(st));
+  const int Bq = cnt[0], M = cnt[1];
+  if (Bq == 0) {
+    CK(pl.copy_out(st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  // stage 3: gather the listed poses into the inputs of the mixed solve at the horizon M; its outputs start as zeros
+  ParkProblem PM;
+  fill_problem(PM, M, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist);      // the shape passed above, with 2 <= M <= Ncap
+  const size_t Qs = Bq, MS = M + 1;
+  obca_flow::Gather g;
+  g.rx = po.rx; g.ry = po.ry; g.ryaw = po.ryaw; g.xWS = po.xWS; g.uWS = po.uWS; g.x0 = d0; g.xF = dF;
+  obca_flow::Outs so;
+  char* dout;
+  DevLayout outs;
+  outs.add(so.xp, 4 * MS * Qs);
+  outs.add(so.up, 2 * (size_t)M * Qs);
+  outs.add(so.ts, MS * Qs);
+  outs.add(so.lp, (size_t)V * MS * Qs);
+  outs.add(so.np, 4 * (size_t)nOb * MS * Qs);
+  outs.add(so.sl, (size_t)nOb * MS * Qs);
+  outs.add(so.kkt_err, Qs);
+  outs.add(so.exitflag, Qs);
+  outs.add(so.iters, Qs);
+  outs.add(so.feasible, Qs);
+  outs.add(so.strict, Qs);
+  DevLayout sl_;
+  sl_.add(g.mrx, MS * Qs);
+  sl_.add(g.mry, MS * Qs);
+  sl_.add(g.mryaw, MS * Qs);
+  sl_.add(g.mxWS, 4 * MS * Qs);
+  sl_.add(g.muWS, 2 * (size_t)M * Qs);
+  sl_.add(g.mx0, 4 * Qs);
+  sl_.add(g.mxF, 4 * Qs);
+  sl_.add(dout, outs.bytes);
+  DevBuf dsolve;
+  CK(alloc_layout(dsolve, sl_));
+  outs.place(dout);
+  CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
+  const size_t items = Qs * MS;
+  const int threads = 256, blocks = (int)((items + threads - 1) / threads);
+  k_flow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
+  CK(cudaGetLastError());
+  // stage 4: the mixed solve (DualMultWS inside); stage 5: ParkingConstraints on its outputs
+  obca_opts o2;
+  if (opts) o2 = *opts; else obca_default_opts(&o2);
+  rc = parking_solve_dev(Bq, M, dNb, nOb, vOb, A, b, g.mx0, g.mxF, Ts, L, ego, XYbounds, g.mrx, g.mry, g.mryaw, g.mxWS, g.muWS, nullptr,
+                         nullptr, fixTime, signed_dist, &o2, so.xp, so.up, so.ts, so.lp, so.np, so.sl, so.exitflag, so.iters, so.kkt_err,
+                         solve_seconds);
+  if (rc) return rc;
+  rc = check_parking_dev(*c, PM, Bq, dNb, g.mx0, g.mxF, so.xp, so.up, so.lp, so.np, so.ts, so.sl, signed_dist, so.feasible, nullptr,
+                         so.strict);
+  if (rc) return rc;
+  // stage 6: the solved poses' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
+  // write keeps the caller's value), then everything back in one pass
+  obca_flow::Outs d;
+  const size_t NS = Ncap + 1;
+  DevLayout ol;
+  ol.inout(d.xp, xp, 4 * NS * Bs);
+  ol.inout(d.up, up, 2 * (size_t)Ncap * Bs);
+  ol.inout(d.ts, ts, NS * Bs);
+  ol.inout(d.lp, lp, (size_t)V * NS * Bs);
+  ol.inout(d.np, np, 4 * (size_t)nOb * NS * Bs);
+  ol.inout(d.sl, sl, (size_t)nOb * NS * Bs);
+  ol.inout(d.kkt_err, kkt_err, Bs);
+  ol.inout(d.exitflag, exitflag, Bs);
+  ol.inout(d.iters, iters, Bs);
+  ol.inout(d.feasible, feasible, Bs);
+  ol.inout(d.strict, strict, Bs);
+  DevBuf dcaller;
+  CK(alloc_layout(dcaller, ol));
+  if (!sl) d.sl = nullptr;
+  if (!strict) d.strict = nullptr;
+  CK(ol.copy_in(st));
+  k_flow_scatter<<<blocks, threads, 0, st>>>(Bq, M, Ncap, V, nOb, dlist, dNb, so, d);
+  CK(cudaGetLastError());
+  CK(ol.copy_out(st));
+  CK(pl.copy_out(st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
 }
 
 int obca_last_profile(int device, unsigned long long* out8) {

@@ -94,45 +94,33 @@ int launch_hmaps(const HeurGrid& H, const std::vector<long>& gcell, double* dmap
 
 }  // namespace
 
-// Both warm-start entries: B start poses, goal p at xF + goal_stride * p (3: a goal per pose, 0: one goal for the batch).
-static int plan_warmstart(int B, const double* x0, const double* xF, size_t goal_stride, const double* ox, const double* oy, int n_ob,
-                          double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap, const obca_opts* opts, double* rx,
-                          double* ry, double* ryaw, double* xWS, double* uWS, int* N, int* status, int* expansions, double* plan_seconds) {
+int plan_check_args(int B, bool args, int n_ob, double Ts, int sampleN) {
   if (B < 0) { obca_set_last_error("B < 0"); return OBCA_ERR_ARG; }
-  if (!x0 || !xF || !ox || !oy || !rx || !ry || !ryaw || !xWS || !uWS || !N || !status) {
-    obca_set_last_error("null argument"); return OBCA_ERR_ARG;
-  }
+  if (!args) { obca_set_last_error("null argument"); return OBCA_ERR_ARG; }
   if (n_ob <= 0) { obca_set_last_error("n_ob <= 0: the planner needs obstacle points"); return OBCA_ERR_ARG; }
   if (!(Ts > 0)) { obca_set_last_error("Ts <= 0"); return OBCA_ERR_ARG; }
   if (sampleN < 1) { obca_set_last_error("sampleN < 1"); return OBCA_ERR_ARG; }
-  if (cap < 2) { obca_set_last_error("cap < 2"); return OBCA_ERR_ARG; }
   if (motion_nlist() != PLAN_NLIST) { obca_set_last_error("motion primitive length differs from the kernel's"); return OBCA_ERR_UNSUPPORTED; }
-  const int dev = opts ? opts->device : 0;
-  const int rc = check_device(dev);
-  if (rc) return rc;
-  if (plan_seconds) *plan_seconds = 0.0;
-  if (B == 0) return 0;
-  if (max_nodes <= 0) max_nodes = PLAN_DEFAULT_NODES;
+  return 0;
+}
 
-  std::vector<double> xFs(3 * (size_t)B);
-  for (int p = 0; p < B; ++p)
-    for (int r = 0; r < 3; ++r) xFs[3 * (size_t)p + r] = xF[goal_stride * p + r];
+int plan_warmstart_dev(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L,
+                       int sampleN, int max_expansions, int max_nodes, int cap, int dev, cudaStream_t st, const PlanDevOut& out,
+                       float* plan_ms) {
+  if (max_nodes <= 0) max_nodes = PLAN_DEFAULT_NODES;
   PlanSetup S;
-  plan_setup(S, B, xFs.data(), ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap);
+  plan_setup(S, B, xF, ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap);
   int sms = 0;
-  Stream st;
   Event e0, e1;
-  CK(cudaSetDevice(dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CK(cudaStreamCreateWithFlags(&st.h, cudaStreamNonBlocking));
   CK(cudaEventCreate(&e0.h));
   CK(cudaEventCreate(&e1.h));
   const int grid = B < sms * PLAN_CTAS_PER_SM ? B : sms * PLAN_CTAS_PER_SM;
   const size_t P = plan_path_max(cap, sampleN), nc = (size_t)S.ob.start.size(), ni = S.ob.ids.size();
   const size_t nh = S.C.hcells * (S.gcell.size() / 2);
-  // batch constants: obstacle points, cell grid (CSR), one heuristic map per distinct goal cell, counter
-  double *dox, *doy, *dpmap;
-  int *dstart, *dids, *dcounter;
+  // batch constants: obstacle points, cell grid (CSR), one heuristic map per distinct goal cell, counter; the poses and goals
+  double *dox, *doy, *dpmap, *dx0, *dxF;
+  int *dstart, *dids, *dcounter, *dhidx;
   DevLayout cl;
   cl.in(dox, S.ob.ox.data(), n_ob);
   cl.in(doy, S.ob.oy.data(), n_ob);
@@ -140,14 +128,17 @@ static int plan_warmstart(int B, const double* x0, const double* xF, size_t goal
   cl.in(dids, ni > 0 ? S.ob.ids.data() : nullptr, ni > 0 ? ni : 1);
   cl.add(dpmap, nh > 0 ? nh : 1);
   cl.add(dcounter, 1);
+  cl.in(dx0, x0, 3 * (size_t)B);
+  cl.in(dxF, xF, 3 * (size_t)B);
+  cl.in(dhidx, S.hidx.data(), B);
   DevBuf dconst, dhmap;
   CK(alloc_layout(dconst, cl));
-  CK(cl.copy_in(st.h));
-  CK(cudaMemsetAsync(dcounter, 0, sizeof(int), st.h));
-  const int hrc = launch_hmaps(S.H, S.gcell, dpmap, dev, st.h, dhmap, nullptr, nullptr);
+  CK(cl.copy_in(st));
+  CK(cudaMemsetAsync(dcounter, 0, sizeof(int), st));
+  const int hrc = launch_hmaps(S.H, S.gcell, dpmap, dev, st, dhmap, nullptr, nullptr);
   if (hrc) return hrc;
   PlanConst C = S.C;
-  C.grid.start = dstart; C.grid.ids = dids; C.grid.ox = dox; C.grid.oy = doy; C.pmap = dpmap;      // C.goals / C.hidx below
+  C.grid.start = dstart; C.grid.ids = dids; C.grid.ox = dox; C.grid.oy = doy; C.pmap = dpmap; C.goals = dxF; C.hidx = dhidx;
   // per resident CTA: cell table, node pool, heap, course and path buffers
   PlanScratch W0;
   DevLayout wl;
@@ -165,36 +156,58 @@ static int plan_warmstart(int B, const double* x0, const double* xF, size_t goal
   wl.add(W0.work, 9 * (P + 40) * grid);
   DevBuf dscr;
   CK(alloc_layout(dscr, wl));
-  CK(cudaMemsetAsync(W0.table, 0xff, C.table_size * grid * sizeof(int), st.h));      // -1: no node
-  // inputs / outputs: outputs are copied in first, so that the kernel leaves every entry it does not write as the caller had it
+  CK(cudaMemsetAsync(W0.table, 0xff, C.table_size * grid * sizeof(int), st));      // -1: no node
+  PlanIO io{dx0, out.rx, out.ry, out.ryaw, out.xWS, out.uWS, out.N, out.status, out.expansions};
+  CK(cudaEventRecord(e0.h, st));
+  k_plan<<<grid, PLAN_THREADS, 0, st>>>(B, C, io, W0, dcounter);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e1.h, st));
+  CK(cudaStreamSynchronize(st));      // the scratch is freed on return
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e0.h, e1.h));
+  if (plan_ms) *plan_ms = ms;
+  return 0;
+}
+
+// Both warm-start entries: B start poses, goal p at xF + goal_stride * p (3: a goal per pose, 0: one goal for the batch).  The outputs
+// are copied to the device first, so that the kernel leaves every entry it does not write as the caller had it.
+static int plan_warmstart(int B, const double* x0, const double* xF, size_t goal_stride, const double* ox, const double* oy, int n_ob,
+                          double Ts, double L, int sampleN, int max_expansions, int max_nodes, int cap, const obca_opts* opts, double* rx,
+                          double* ry, double* ryaw, double* xWS, double* uWS, int* N, int* status, int* expansions, double* plan_seconds) {
+  int rc = plan_check_args(B, x0 && xF && ox && oy && rx && ry && ryaw && xWS && uWS && N && status, n_ob, Ts, sampleN);
+  if (rc) return rc;
+  if (cap < 2) { obca_set_last_error("cap < 2"); return OBCA_ERR_ARG; }
+  const int dev = opts ? opts->device : 0;
+  rc = check_device(dev);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = 0.0;
+  if (B == 0) return 0;
+
+  std::vector<double> xFs(3 * (size_t)B);
+  for (int p = 0; p < B; ++p)
+    for (int r = 0; r < 3; ++r) xFs[3 * (size_t)p + r] = xF[goal_stride * p + r];
+  Stream st;
+  CK(cudaSetDevice(dev));
+  CK(cudaStreamCreateWithFlags(&st.h, cudaStreamNonBlocking));
   const size_t cb = (size_t)B * cap;
-  double *dx0, *dxF, *drx, *dry, *dryaw, *dxWS, *duWS;
-  int *dhidx, *dN, *dst, *dex;
+  PlanDevOut o;
   DevLayout il;
-  il.in(dx0, x0, 3 * (size_t)B);
-  il.in(dxF, xFs.data(), 3 * (size_t)B);
-  il.in(dhidx, S.hidx.data(), B);
-  il.inout(drx, rx, cb);
-  il.inout(dry, ry, cb);
-  il.inout(dryaw, ryaw, cb);
-  il.inout(dxWS, xWS, 4 * cb);
-  il.inout(duWS, uWS, 2 * cb);
-  il.inout(dN, N, B);
-  il.out(dst, status, B);
-  il.out(dex, expansions, B);
+  il.inout(o.rx, rx, cb);
+  il.inout(o.ry, ry, cb);
+  il.inout(o.ryaw, ryaw, cb);
+  il.inout(o.xWS, xWS, 4 * cb);
+  il.inout(o.uWS, uWS, 2 * cb);
+  il.inout(o.N, N, B);
+  il.out(o.status, status, B);
+  il.out(o.expansions, expansions, B);
   DevBuf dio;
   CK(alloc_layout(dio, il));
   CK(il.copy_in(st.h));
-  C.goals = dxF; C.hidx = dhidx;
-  PlanIO io{dx0, drx, dry, dryaw, dxWS, duWS, dN, dst, dex};
-  CK(cudaEventRecord(e0.h, st.h));
-  k_plan<<<grid, PLAN_THREADS, 0, st.h>>>(B, C, io, W0, dcounter);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(e1.h, st.h));
+  float ms = 0.f;
+  rc = plan_warmstart_dev(B, x0, xFs.data(), ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap, dev, st.h, o, &ms);
+  if (rc) return rc;
   CK(il.copy_out(st.h));
   CK(cudaStreamSynchronize(st.h));
-  float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, e0.h, e1.h));
   if (plan_seconds) *plan_seconds = ms * 1e-3;
   return 0;
 }

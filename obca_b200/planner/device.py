@@ -156,3 +156,100 @@ def plan_batch(x0s, xF, scenario="backwards", Ts=None, L=2.7, sampleN=3, cap=512
         out.append(dict(rx=o["rx"][i, :n + 1].copy(), ry=o["ry"][i, :n + 1].copy(), ryaw=o["ryaw"][i, :n + 1].copy(),
                         xWS=o["xWS"][i, :4 * (n + 1)].reshape(4, n + 1).T.copy(), uWS=o["uWS"][i, :2 * n].reshape(2, n).T.copy(), N=n, Ts=Ts))
     return out
+
+
+def plan_solve_goals_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=2.7, sampleN=3, Ncap=319, fixTime=0, signed_dist=1,
+                         max_nodes=0, max_expansions=0, opts=None, host_fallback=False):
+    """obca_parking_plan_solve_goals's outputs as arrays: plan every start pose x0s (B, 4: x, y, yaw, v) towards its goal xFs ((B, 4), or
+    (4,) for all), solve the poses that planned and check the results, in one call.  Per-pose arrays in the entry's layout for Ncap,
+    row-major views of the column-major blocks: xp (B, Ncap+1, 4), up (B, Ncap, 2), ts (B, Ncap+1), lp (B, Ncap+1, V),
+    np (B, Ncap+1, 4nOb), sl (B, Ncap+1, nOb); one value per pose: N, status, expansions, exitflag, iters, kkt_err, feasible, strict; and
+    plan_seconds, time (the solve's device seconds).  The buffers start as NaN (the integers as -1): entries the call does not write stay
+    so.  host_fallback: the poses whose search outgrew the device's scratch (POOL_FULL) are planned by the host twin (native.plan_cloud_raw,
+    the same decisions), and those that plan to 2 <= N <= Ncap are solved and checked by parking_solve_mixed / check_parking_mixed in one
+    more call each (their solve time is not in `time`), as plan_goals_raw(host_fallback=True) does for the planner alone."""
+    from .._lib import f64
+    from ..parking import _shared
+    x0s = f64(np.asarray(x0s, float).reshape(-1, 4)); B = x0s.shape[0]
+    xFs = f64(np.broadcast_to(np.asarray(xFs, float).reshape(-1, 4), (B, 4)))
+    vOb, V, A, b = _shared(nOb, vOb, A, b)
+    ox = f64(ox); oy = f64(oy); NS = Ncap + 1
+    nan = lambda *s: np.full(s, np.nan)
+    i32 = lambda: np.full(B, -1, np.int32)
+    o = dict(xp=nan(B, NS, 4), up=nan(B, Ncap, 2), ts=nan(B, NS), lp=nan(B, NS, V), np=nan(B, NS, 4 * nOb), sl=nan(B, NS, nOb), N=i32(),
+             status=i32(), expansions=i32(), exitflag=i32(), iters=i32(), kkt_err=nan(B), feasible=i32(), strict=i32())
+    secs = np.zeros(2)
+    opts = opts if opts is not None else _lib.default_opts()
+    p = _lib.ptr
+    f = _lib.lib().obca_parking_plan_solve_goals
+    f.restype = C.c_int
+    f.argtypes = ([C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 5
+                  + [C.c_int, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 16)
+    rc = f(B, p(x0s), p(xFs), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(nOb),
+           p(vOb), p(A), p(b), p(f64(np.asarray(ego).ravel())), p(f64(np.asarray(XYbounds).ravel())), int(fixTime), int(signed_dist),
+           C.cast(C.byref(opts), C.c_void_p), int(Ncap),
+           *[p(o[k]) for k in ("xp", "up", "ts", "lp", "np", "sl", "N", "status", "expansions", "exitflag", "iters", "kkt_err", "feasible",
+                               "strict")], p(secs[:1]), p(secs[1:]))
+    _lib.check(rc)
+    o["plan_seconds"], o["time"] = float(secs[0]), float(secs[1])
+    full = np.flatnonzero(o["status"] == POOL_FULL)
+    if host_fallback and full.size:
+        _solve_on_host_plans(o, full, x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, fixTime, signed_dist, opts)
+    return o
+
+
+def _solve_on_host_plans(o, full, x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, fixTime, signed_dist, opts):
+    """Plan the poses `full` with the host twin, then solve and check the ones it plans to 2 <= N <= Ncap; their entries of o (the layout
+    of plan_solve_goals_raw) get the results, the others the host twin's status (OBCA_PLAN_CAPACITY for a horizon outside [2, Ncap])."""
+    from .. import parking
+    h = native.plan_cloud_raw(x0s[full], xFs[full], ox, oy, Ts, L, sampleN)
+    st = h["status"].copy()
+    st[(st == 0) & ((h["N"] < 2) | (h["N"] > Ncap))] = 2
+    o["status"][full] = st; o["N"][full] = h["N"]; o["expansions"][full] = h["expansions"]
+    ok = np.flatnonzero(st == 0)
+    if ok.size == 0:
+        return
+    Ns = h["N"][ok]
+    rx = [h["rx"][i, :n + 1] for i, n in zip(ok, Ns)]; ry = [h["ry"][i, :n + 1] for i, n in zip(ok, Ns)]
+    ryaw = [h["ryaw"][i, :n + 1] for i, n in zip(ok, Ns)]
+    xWS = [h["xWS"][i, :4 * (n + 1)].reshape(4, n + 1).T for i, n in zip(ok, Ns)]
+    uWS = [h["uWS"][i, :2 * n].reshape(2, n).T for i, n in zip(ok, Ns)]
+    x0, xF = x0s[full[ok]], xFs[full[ok]]
+    r = parking.parking_solve_mixed(x0, xF, Ns, Ts, L, ego, XYbounds, nOb, vOb, A, b, rx, ry, ryaw, fixTime, xWS, uWS, signed_dist, opts=opts)
+    feas, _, strict = parking.check_parking_mixed(x0, xF, Ns, Ts, L, ego, XYbounds, nOb, vOb, A, b, r["xp"], r["up"], r["lp"], r["np"], r["ts"],
+                                                  fixTime, signed_dist, r["sl"], opts=opts)
+    for q, (i, n) in enumerate(zip(full[ok], Ns)):
+        for k, ext in (("xp", 1), ("up", 0), ("lp", 1), ("np", 1), ("sl", 1)):
+            o[k][i, :n + ext] = r[k][q].T
+        o["ts"][i, :n + 1] = r["ts"][q]
+    for k, v in (("exitflag", r["exitflag"]), ("iters", r["iters"]), ("kkt_err", r["kkt_err"]), ("feasible", feas), ("strict", strict)):
+        o[k][full[ok]] = v
+
+
+def plan_solve_goals(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=2.7, sampleN=3, Ncap=319, fixTime=0, signed_dist=1,
+                     max_nodes=0, max_expansions=0, opts=None, host_fallback=False):
+    """main.jl:215-269 for a batch in one call (obca_parking_plan_solve_goals): plan, solve and check every start pose x0s (B, 4) towards
+    its goal xFs ((B, 4), or (4,) for all).  Returns the keys of parking.parking_solve_mixed in the caller's pose order -- per-pose lists
+    in the Julia shapes (xp[i] 4 x (N[i]+1), up[i] 2 x N[i], ts[i], lp[i], np[i], sl[i]), None where the pose was not solved, and the
+    arrays exitflag, iters, kkt_err, N, time -- plus status (OBCA_PLAN_* of include/obca.h: 0 solved, 1 no path, 2 horizon over Ncap,
+    4 POOL_FULL: the search outgrew the device's scratch), expansions, feasible (ParkingConstraints' value), strict and plan_seconds.
+    host_fallback: plan, solve and check the POOL_FULL poses on the host twin's plans (see plan_solve_goals_raw)."""
+    o = plan_solve_goals_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, fixTime, signed_dist, max_nodes,
+                             max_expansions, opts, host_fallback)
+    ok = o["status"] == 0
+    cut = lambda a, ext: [a[i, :n + ext].T.copy() if ok[i] else None for i, n in enumerate(o["N"])]
+    out = dict(xp=cut(o["xp"], 1), up=cut(o["up"], 0), ts=[o["ts"][i, :n + 1].copy() if ok[i] else None for i, n in enumerate(o["N"])],
+               lp=cut(o["lp"], 1), np=cut(o["np"], 1), sl=cut(o["sl"], 1))
+    for k in ("exitflag", "iters", "feasible", "strict"):
+        out[k] = np.where(ok, o[k], 0).astype(np.int32)
+    out.update(kkt_err=np.where(ok, o["kkt_err"], np.nan), N=o["N"].copy(), status=o["status"].copy(), expansions=o["expansions"].copy(),
+               time=o["time"], plan_seconds=o["plan_seconds"])
+    return out
+
+
+def plan_solve_batch(x0s, xF, nOb, vOb, A, b, ego, XYbounds, scenario="backwards", Ts=None, L=2.7, sampleN=3, Ncap=319, **kw):
+    """plan_solve_goals with one goal xF (4,) for every pose among the demo cloud of `scenario`, as plan_batch relates to
+    plan_goals_batch: the sweeps of main.jl:165-168 planned, solved and checked in one call."""
+    ox, oy = native.obstacle_points(scenario)
+    Ts = Ts or (0.6 if scenario == "backwards" else 0.9) / 3 * sampleN
+    return plan_solve_goals(x0s, np.asarray(xF, float)[:4], ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, **kw)
