@@ -5,9 +5,11 @@ call (device.plan_quadcopter_batch); all three give the same plans --, solve all
 pairs -- each with the horizon N = path length - 1 and the sampling time Ts = round(0.25 * 80 / N, 2) the planner gave it -- in ONE
 GPU call (obca_quadcopter_solve_mixed), run the reference's constrSatisfaction on every result in one more call.  Pairs whose
 horizon exceeds the solver's limit (N + 1 <= 512; the planner gives N = 80..147 over the config-4 box) are counted and listed
-as skipped.
+as skipped.  Planner "flow" does all of it -- plan, warm start, solve, check -- in one call that keeps everything on the GPU
+(device.plan_solve_quadcopter, obca_quadcopter_plan_solve), with the pairs whose search outgrew the device's scratch planned on the host;
+it prints the same counts as "gpu".
 
-usage: python examples/sweep_quadcopter.py [K] [seed] [workers] [python|host|gpu]      (needs a CUDA device for the solves)
+usage: python examples/sweep_quadcopter.py [K] [seed] [workers] [python|host|gpu|flow]      (needs a CUDA device for the solves)
 """
 import os
 import sys
@@ -30,6 +32,8 @@ N_LIMIT = 511      # the quadcopter solver's longest horizon (N + 1 <= 512 stage
 def sweep(K=32, seed=2, signed_dist=1, workers=None, planner="python"):
     sc = scenarios.quadcopter_batch(K, seed=seed)          # config-4 start / goal pairs (mainQuadcopter.jl:48-51)
     t0 = time.time()
+    if planner == "flow":
+        return flow(sc, K, signed_dist, t0)
     if planner == "python":
         with ProcessPoolExecutor(workers) as ex:
             plans = list(ex.map(plan_quadcopter_warm_start, sc["x0"], sc["xF"], [sc["Ts80"]] * K))
@@ -38,7 +42,7 @@ def sweep(K=32, seed=2, signed_dist=1, workers=None, planner="python"):
     elif planner == "gpu":
         plans = device.plan_quadcopter_batch(sc["x0"], sc["xF"], sc["Ts80"])
     else:
-        raise ValueError(f"planner must be python, host or gpu, not {planner!r}")
+        raise ValueError(f"planner must be python, host, gpu or flow, not {planner!r}")
     t_plan = time.time() - t0
     N = np.array([p["N"] if p else -1 for p in plans])
     idx = [i for i in range(K) if 2 <= N[i] <= N_LIMIT]
@@ -55,6 +59,18 @@ def sweep(K=32, seed=2, signed_dist=1, workers=None, planner="python"):
     return out
 
 
+def flow(sc, K, signed_dist, t0):
+    o = device.plan_solve_quadcopter(sc["x0"], sc["xF"], sc["R"], sc["obs"], sc["Ts80"], signed_dist, Ncap=N_LIMIT, host_fallback=True)
+    t_all = time.time() - t0
+    N, ok = o["N"], o["status"] == 0
+    out = dict(K=K, planner="flow", planned=int((N >= 0).sum()), skipped=[(i, int(N[i])) for i in range(K) if N[i] > N_LIMIT],
+               t_plan=t_all, t_solve=o["time"], converged=int((o["exitflag"][ok] == 1).sum()), feasible=int(o["feasible"][ok].sum()),
+               N=N, Ts=o["Ts"])
+    if ok.any():
+        out.update(solved=int(ok.sum()), exitflag=o["exitflag"][ok])
+    return out
+
+
 if __name__ == "__main__":
     a = sys.argv
     try:
@@ -63,7 +79,8 @@ if __name__ == "__main__":
     except obca_b200.ObcaError as e:
         print("solve not run:", e); sys.exit(2)
     ok = o["N"][o["N"] >= 0]
-    print(f"{o['K']} start / goal pairs: {o['planned']} planned in {o['t_plan']:.1f} s ({o['planner']} planner), N = {ok.min()}..{ok.max()} "
+    how = "planned, solved and checked in one call" if o["planner"] == "flow" else "planned"
+    print(f"{o['K']} start / goal pairs: {o['planned']} {how} in {o['t_plan']:.1f} s ({o['planner']} planner), N = {ok.min()}..{ok.max()} "
           f"({len(set(ok.tolist()))} distinct), Ts = {np.nanmin(o['Ts']):.2f}..{np.nanmax(o['Ts']):.2f}")
     if o["skipped"]:
         print(f"skipped {len(o['skipped'])} pair(s) with N > {N_LIMIT} (pair, N): {o['skipped']}")

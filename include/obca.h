@@ -17,6 +17,8 @@
  *   obca_quadcopter_solve_mixed / obca_check_quadcopter_mixed: the same two for a batch whose problems have different
  *                                 horizons and sampling times (the 3-D A* warm starts of mainQuadcopter.jl:122-137 each
  *                                 come with their own N and Ts = round(Ts*80/N, 2))
+ *   obca_quadcopter_plan_solve: mainQuadcopter.jl:114-154 (plan -> warm start -> solve -> check) for a batch of start / goal
+ *                                 pairs in one call
  *
  * Conventions
  *   - every array is float64, COLUMN-MAJOR exactly as the Julia caller holds it; a batch of B problems is the B
@@ -301,6 +303,57 @@ int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, const double* 
                                          int n_ob, const double* lo, const double* hi, double reso, int max_nodes, int cap,
                                          const obca_opts* opts, double* rx, double* ry, double* rz, int* N, int* status, int* expansions,
                                          double* plan_seconds);
+
+/* The grid scale of the quadcopter flow: the 3-D A* plans on a grid 10x finer than the solve's units (mainQuadcopter.jl:114-119 scales
+ * the start and goal up, a_star_3d.plan_quadcopter_warm_start divides the path back down). */
+#define OBCA_QUAD_GRID_SCALE 10.0
+
+/* mainQuadcopter.jl:114-154 for a batch: plan every start / goal pair with the 3-D A* (obca_plan_quadcopter_warmstart_batch), build the
+ * warm start of every pair that planned (a_star_3d.plan_quadcopter_warm_start), solve those pairs (obca_quadcopter_solve_mixed) and run
+ * constrSatisfaction on the results (obca_check_quadcopter_mixed) in ONE call, with nothing leaving the device between the stages.  All
+ * on the library's stream of opts->device:
+ *   1. plan (k_plan3d) with the stride Ncap + 1 into device buffers, then free the planner's scratch;
+ *   2. list the pairs planned OK to a horizon 2 <= N[i] <= Ncap, in pair order; their count and longest horizon Nmax are the only values
+ *      read back before the solve, which is laid out for that Nmax, not for Ncap;
+ *   3. build those pairs' warm starts: xWS = the path / OBCA_QUAD_GRID_SCALE in rows 1-3 and zeros in rows 4-12, the sampling time
+ *      Tsb[i] = jround(Ts * 80 / N[i] * 100) / 100 (jround: round half away from zero) computed in IEEE double without fused
+ *      operations, and x0 / xF gathered into the inputs of the mixed solve;  4. solve;  5. check;
+ *   6. scatter the results to the caller's pair order and copy them back once.
+ * Inputs: x0, xF 12 x B in the solve's units, as for obca_quadcopter_solve_mixed; the planner's start and goal are OBCA_QUAD_GRID_SCALE
+ * times their rows 1-3, multiplied on the host.  The cloud ox, oy, oz (n_ob points), the bound corners lo, hi, the cell size reso and
+ * max_nodes are the planner's, in its units, as for obca_plan_quadcopter_warmstart_batch.  Ts: the nominal sampling time (0.25 in
+ * mainQuadcopter.jl).  R, ob, timeWS, signed_dist, opts: the solve's, as for obca_quadcopter_solve_mixed; opts == NULL: defaults with
+ * max_iter = 3000.  Ncap: 2 <= Ncap <= 511, the horizon the caller's arrays hold.
+ * Outputs, in the caller's pair order, in the layout of obca_quadcopter_solve_mixed with Nmax = Ncap: xp 12x(Ncap+1), up 4xNcap,
+ * ts Ncap+1, lp 30x(Ncap+1), slack 5x(Ncap+1) (may be NULL; written for signed_dist = 1 only); one value per pair: N (the planned
+ * horizon), Tsb (the pair's sampling time), status, expansions (may be NULL) as the planner writes them, exitflag, iters, kkt_err,
+ * feasible (the value constrSatisfaction returns) and worst (may be NULL; the largest violation it found).  status[i]:
+ *   OBCA_PLAN_OK (0)         planned and solved: every output of pair i over its own horizon N[i] is written, nothing past it;
+ *   OBCA_PLAN_NO_PATH (1)    no path: only status and N (as the planner leaves it) are written;
+ *   OBCA_PLAN_POOL_FULL (4)  the search outgrew its device scratch: the same (no host fallback here; obca_b200.planner.device plans such
+ *                            pairs on the host);
+ *   OBCA_PLAN_CAPACITY (2)   the path has more than Ncap + 1 points, or fewer than 3 (N[i] < 2): N[i] holds the horizon, nothing else.
+ * A pair that is not solved leaves every other output entry as the caller had it.  Pair i's warm start, solve, check and outputs are
+ * bit-identical to obca_quadcopter_solve_mixed followed by obca_check_quadcopter_mixed on the warm start
+ * a_star_3d.plan_quadcopter_warm_start builds from obca_plan_quadcopter_warmstart_batch's path.  plan_seconds (may be NULL): device time
+ * of k_plan3d; solve_seconds (may be NULL): as for obca_quadcopter_solve_mixed.  Device memory, freed before the call returns apart from
+ * the solve's workspace, which stays with the library as after any solve: the planner's buffers and the pairs' states,
+ * 24 x B x (Ncap + 1) + 212 x B bytes; while planning, the planner's scratch on top (about 4.0 GB on a 132-SM H100 for B >= 528, see
+ * obca_plan_quadcopter_warmstart_batch), freed before the solve allocates; then the solve's inputs and outputs for the Bs pairs it
+ * takes, about 8 x Bs x (Nmax + 1) x 64 bytes, its workspace (as obca_quadcopter_solve_mixed at Nmax), and at the end the caller's
+ * outputs, about 8 x B x (Ncap + 1) x 52 bytes, which are copied to the device first.
+ * One call solves one formulation: mainQuadcopter.jl solves QuadcopterDist and QuadcopterSignedDist on the same plan, which here plans
+ * twice (solving both from one plan is a possible extension).
+ * Return: 0, OBCA_ERR_ARG (the planner's: a null required array, max_nodes > 2^28, B < 0, n_ob < 0, reso <= 0, a non-finite coordinate,
+ * a map of more than 2^27 cells or a start / goal more than 2^30 cells from it; Ncap < 2; Ts not a finite number > 0, or so small that
+ * jround(Ts * 80 / Ncap * 100) < 1, which would give a pair a sampling time of 0), OBCA_ERR_UNSUPPORTED (Ncap > 511, the bound in
+ * obca_last_error()), all before any device work and with nothing written; OBCA_ERR_NO_DEVICE, OBCA_ERR_CUDA.  B = 0, or a batch in
+ * which no pair is solved, returns 0 without launching the solve (solve_seconds = 0). */
+int obca_quadcopter_plan_solve(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz, int n_ob,
+                               const double* lo, const double* hi, double reso, int max_nodes, double Ts, double R, const double* ob,
+                               double timeWS, int signed_dist, const obca_opts* opts, int Ncap, double* xp, double* up, double* ts,
+                               double* lp, double* slack, int* N, double* Tsb, int* status, int* expansions, int* exitflag, int* iters,
+                               double* kkt_err, int* feasible, double* worst, double* plan_seconds, double* solve_seconds);
 
 /* Device times of the last obca_parking_solve_batch[_dev] / obca_parking_solve_mixed on `device`: DualMultWS (0 when the caller passed lWS / nWS) and the
  * solve alone (= what solve_seconds reports; the reference's `time`, ParkingSignedDist.jl:297). */

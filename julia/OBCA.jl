@@ -179,3 +179,36 @@ function plan_solve_goals(x0s::AbstractMatrix, xFs::AbstractMatrix, ox::Abstract
             np = [cut(np, i, N[i] + 1) for i in 1:B], status = status, N = N, exitflag = flag, iters = iters, feasible = feasible,
             plan_time = ps[], solve_time = ss[])
 end
+
+# ---- plan -> warm start -> solve -> check for a batch of quadcopter pairs in one call (include/obca.h: obca_quadcopter_plan_solve) ---
+# mainQuadcopter.jl:114-154 for B start / goal pairs at once, nothing leaving the GPU between the stages.  x0s, xFs: B x 12 matrices
+# (row i = pair i's x0 / xF in the solve's units); ox, oy, oz, lo, hi, reso: the 3-D A*'s obstacle points and bounds on its 10x grid
+# (mainQuadcopter.jl:46-112); R, ob1..ob5 as for QuadcopterSignedDist.  Returns per-pair vectors in mainQuadcopter.jl's shapes (xp[i]
+# 12 x (N[i]+1), up[i] 4 x N[i], timeScale[i], lp[i] 30 x (N[i]+1)) with `nothing` where the pair was not solved, and status (0 solved,
+# 1 no path, 2 horizon outside [2, Ncap], 4 planner scratch full), N, Ts (each pair's sampling time), exitflag, iters, feasible.
+# Like every stub in this file it is not executed in this repository (no Julia in the build image); the tested twin is
+# obca_b200.planner.device.plan_solve_quadcopter (tests/test_gpu_quad_plan_solve.py).
+function plan_solve_quadcopter(x0s::AbstractMatrix, xFs::AbstractMatrix, ox::AbstractVector, oy::AbstractVector, oz::AbstractVector,
+                               lo::AbstractVector, hi::AbstractVector, R, ob1, ob2, ob3, ob4, ob5; Ts::Float64 = 0.25,
+                               reso::Float64 = 1.0, Ncap::Int = 511, signed_dist::Int = 1, max_nodes::Int = 0, timeWS::Float64 = 1.0)
+    B = size(x0s, 1); NS = Ncap + 1
+    ob = hcat(vec(_f64(ob1)), vec(_f64(ob2)), vec(_f64(ob3)), vec(_f64(ob4)), vec(_f64(ob5)))     # 6 x 5
+    xp = zeros(12, NS, B); up = zeros(4, Ncap, B); ts = zeros(NS, B); lp = zeros(30, NS, B); sl = zeros(5, NS, B)
+    N = fill(Cint(-1), B); Tsb = zeros(B); status = fill(Cint(-1), B); expansions = zeros(Cint, B); flag = zeros(Cint, B)
+    iters = zeros(Cint, B); kkt = zeros(B); feasible = zeros(Cint, B); worst = zeros(B); ps = Ref{Cdouble}(0.0); ss = Ref{Cdouble}(0.0)
+    rc = ccall((:obca_quadcopter_plan_solve, LIBOBCA), Cint,
+               (Cint, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint, Ptr{Cdouble}, Ptr{Cdouble}, Cdouble, Cint,
+                Cdouble, Cdouble, Ptr{Cdouble}, Cdouble, Cint, Ref{ObcaOpts}, Cint, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble},
+                Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cint}, Ptr{Cdouble}, Ptr{Cint}, Ptr{Cint}, Ptr{Cint}, Ptr{Cint}, Ptr{Cdouble},
+                Ptr{Cint}, Ptr{Cdouble}, Ref{Cdouble}, Ref{Cdouble}),
+               B, _f64(permutedims(x0s[:, 1:12])), _f64(permutedims(xFs[:, 1:12])), _f64(ox), _f64(oy), _f64(oz), length(ox),
+               _f64(lo), _f64(hi), reso, max_nodes, Ts, Float64(R), ob, timeWS, signed_dist,
+               (o = obca_default_opts(); o.max_iter = 3000; o), Ncap, xp, up, ts, lp, sl, N, Tsb, status, expansions, flag, iters,
+               kkt, feasible, worst, ps, ss)
+    rc == 0 || error("obca_quadcopter_plan_solve: ", rc, " ", unsafe_string(ccall((:obca_last_error, LIBOBCA), Cstring, ())))
+    ok = status .== 0
+    cut(a, i, n) = ok[i] ? a[:, 1:n, i] : nothing
+    return (xp = [cut(xp, i, N[i] + 1) for i in 1:B], up = [cut(up, i, N[i]) for i in 1:B],
+            timeScale = [ok[i] ? ts[1:N[i]+1, i] : nothing for i in 1:B], lp = [cut(lp, i, N[i] + 1) for i in 1:B],
+            status = status, N = N, Ts = Tsb, exitflag = flag, iters = iters, feasible = feasible, plan_time = ps[], solve_time = ss[])
+end

@@ -16,7 +16,8 @@ SYMBOLS = ["obca_version", "obca_device_count", "obca_last_error", "obca_default
            "obca_last_times", "obca_parking_solve_mixed", "obca_check_parking_mixed",
            "obca_quadcopter_solve_batch", "obca_check_quadcopter", "obca_quadcopter_solve_mixed",
            "obca_check_quadcopter_mixed", "obca_plan_parking_warmstart_batch", "obca_plan_quadcopter_warmstart_batch",
-           "obca_plan_parking_warmstart_goals", "obca_plan_parking_heuristic_maps", "obca_parking_plan_solve_goals"]
+           "obca_plan_parking_warmstart_goals", "obca_plan_parking_heuristic_maps", "obca_parking_plan_solve_goals",
+           "obca_quadcopter_plan_solve"]
 
 
 class ObcaOpts(C.Structure):

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <string.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -148,3 +149,24 @@ struct PlanDevOut {
 int plan_warmstart_dev(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L,
                        int sampleN, int max_expansions, int max_nodes, int cap, int dev, cudaStream_t st, const PlanDevOut& out,
                        float* plan_ms);
+
+// The GPU 3-D A* of obca_plan3d.cu, for obca_plan_quadcopter_warmstart_batch and for obca_quadcopter_plan_solve (obca_lib.cu), which keeps
+// the plans on the device.  The host set-up (obstacle bitmap, grid geometry, the pairs' cells) stays behind Plan3dSetup, so that only
+// obca_plan3d.cu, built without FMA contraction, compiles it.
+struct Plan3dSetup;
+struct Plan3dSetupFree {
+  void operator()(Plan3dSetup* s) const;
+};
+using Plan3dSetupPtr = std::unique_ptr<Plan3dSetup, Plan3dSetupFree>;
+// The planner's argument checks, in the entry's order and with its messages (args: no required array is null), then its host set-up
+// of B pairs (x0, xF: host, 3 per pair, in planner units) for paths of at most cap points.  Returns 0 or OBCA_ERR_ARG; touches no device.
+int plan3d_prepare(Plan3dSetupPtr& S, int B, bool args, const double* x0, const double* xF, const double* ox, const double* oy,
+                   const double* oz, int n_ob, const double* lo, const double* hi, double reso, int max_nodes, int cap);
+// Device outputs of the planner, in the layout of obca_plan_quadcopter_warmstart_batch with the stride cap; expansions may be null.
+struct Plan3dDevOut {
+  double *rx, *ry, *rz;
+  int *N, *status, *expansions;
+};
+// Plans the B >= 1 pairs of S into `out` on the stream st of the current device dev (k_plan3d).  Returns once the stream is
+// synchronised, after the planner's device scratch is freed; plan_ms (may be null): device time of k_plan3d.
+int plan3d_dev(const Plan3dSetup& S, int B, int dev, cudaStream_t st, const Plan3dDevOut& out, float* plan_ms);

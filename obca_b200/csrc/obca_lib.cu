@@ -7,6 +7,7 @@
 //   k_dualws<VM>             K2: one thread per (problem, stage, obstacle) micro interior-point solve.
 //   k_check                  K5: ParkingConstraints twin + strict audit, one CTA per problem.
 //   k_flow_list, k_flow_gather, k_flow_scatter   the index maps of obca_parking_plan_solve_goals (obca_flow.h): plans -> solve -> poses
+//   k_qflow_gather, k_qflow_scatter              the same for obca_quadcopter_plan_solve (obca_qflow.h), with k_flow_list
 // There is NO CPU fallback: every compute entry point returns OBCA_ERR_NO_DEVICE without a CUDA device.
 // Host-pointer entries stage their arrays through one device buffer per device (DevCtx::stage), laid out, copied and scattered back
 // with the helpers of obca_devstage.h, which the GPU planners (obca_plan.cu, obca_plan3d.cu) use for their per-call buffers too.
@@ -29,6 +30,7 @@
 #include "obca_flow.h"
 #include "obca_host.h"
 #include "obca_phased.cuh"
+#include "obca_qflow.h"
 
 using namespace obca;
 
@@ -194,6 +196,25 @@ __global__ void k_flow_scatter(int Bs, int M, int Ncap, int V, int nOb, const in
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int q = (int)(i / (M + 1)), k = (int)(i % (M + 1));
     obca_flow::scatter_stage(src, dst, V, nOb, q, list[q], Nb[q], k, M, Ncap);
+  }
+}
+
+// The same two copies for obca_quadcopter_plan_solve (obca_qflow.h); k_flow_list lists its pairs.  One thread per (slot q < Bs, stage
+// k <= M): pair list[q]'s path, x0 and xF to the warm start and inputs of the mixed solve at the horizon M, and its sampling time.
+__global__ void k_qflow_gather(int Bs, int M, int cap, const int* __restrict__ list, const int* __restrict__ Nb, const obca_qflow::Gather g) {
+  const size_t total = (size_t)Bs * (M + 1);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int q = (int)(i / (M + 1)), k = (int)(i % (M + 1));
+    obca_qflow::gather_stage(g, q, list[q], Nb[q], k, M, cap);
+  }
+}
+
+__global__ void k_qflow_scatter(int Bs, int M, int Ncap, const int* __restrict__ list, const int* __restrict__ Nb,
+                                const obca_qflow::Outs src, const obca_qflow::Outs dst) {
+  const size_t total = (size_t)Bs * (M + 1);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int q = (int)(i / (M + 1)), k = (int)(i % (M + 1));
+    obca_qflow::scatter_stage(src, dst, q, list[q], Nb[q], k, M, Ncap);
   }
 }
 
@@ -884,6 +905,27 @@ static int check_parking(int B, int N, const int* Nb, int nOb, const int* vOb, c
 }
 
 
+// The quadcopter solver's horizon bound, checked before any device work: a refused call launches nothing and writes no output.
+static int check_quad_horizon(int N) {
+  if (N <= QUAD_NMAX) return 0;
+  set_err("horizon too long for the quadcopter solver: N = " + std::to_string(N) + " > " + std::to_string(QUAD_NMAX) +
+          " (N + 1 <= " + std::to_string(QUAD_NMAX + 1) + " stages)");
+  return OBCA_ERR_UNSUPPORTED;
+}
+
+// The quadcopter solve of a batch on the device's stream (every pointer of bp a device pointer, laid out for P.N), between the events
+// ev0 and ev1 of the context, with the phase counters in c.prof; the caller copies the counters back and reads the time once the stream
+// is synchronised.
+static int quad_solve_dev(DevCtx& c, const QuadProblem& P, const IpmOpts& O, QBatchPtrs bp) {
+  bp.prof = c.prof;
+  CK(cudaMemsetAsync(c.prof, 0, 8 * sizeof(unsigned long long), c.st));
+  CK(cudaEventRecord(c.ev0, c.st));
+  const int rc = P.signed_dist ? launch_quad<true>(c, P, O, bp) : launch_quad<false>(c, P, O, bp);
+  if (rc) return rc;
+  CK(cudaEventRecord(c.ev1, c.st));
+  return 0;
+}
+
 // The quadcopter solve behind the uniform and the mixed entries (host pointers, staged through one device buffer).  Every
 // per-problem array is laid out for the horizon N.  mixed: Nb, Tsb (host pointers) hold per-problem horizons in [2, N] and sampling
 // times; problem b uses the first Nb[b] + 1 stages of its arrays and nothing past them is written.  Otherwise Nb and Tsb are null.
@@ -902,13 +944,10 @@ static int quad_solve_host(bool mixed, int B, int N, const int* Nb, const double
   }
   QuadProblem P;
   if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
-  if (N > QUAD_NMAX) {      // before any device work: nothing is launched and no output is written
-    set_err("horizon too long for the quadcopter solver: N = " + std::to_string(N) + " > " + std::to_string(QUAD_NMAX) +
-            " (N + 1 <= " + std::to_string(QUAD_NMAX + 1) + " stages)");
-    return OBCA_ERR_UNSUPPORTED;
-  }
+  int rc = check_quad_horizon(N);
+  if (rc) return rc;
   DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
+  rc = get_ctx(opts ? opts->device : 0, &c);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
   IpmOpts O = to_ipm(opts);
@@ -945,12 +984,9 @@ static int quad_solve_host(bool mixed, int B, int N, const int* Nb, const double
   QBatchPtrs bp;
   bp.x0 = d0; bp.xF = dF; bp.xWS = dW; bp.Nb = Nb ? dNb : nullptr; bp.Tsb = Nb ? dTs : nullptr;
   bp.timeWS = timeWS; bp.xp = dxp; bp.up = dup; bp.ts = dts; bp.lp = dlp; bp.slack = dsl;
-  bp.exitflag = dflag; bp.iters = diters; bp.kkt_err = derr; bp.B = B; bp.prof = c->prof;
-  CK(cudaMemsetAsync(c->prof, 0, 8 * sizeof(unsigned long long), st));
-  CK(cudaEventRecord(c->ev0, st));
-  rc = signed_dist ? launch_quad<true>(*c, P, O, bp) : launch_quad<false>(*c, P, O, bp);
+  bp.exitflag = dflag; bp.iters = diters; bp.kkt_err = derr; bp.B = B;
+  rc = quad_solve_dev(*c, P, O, bp);
   if (rc) return rc;
-  CK(cudaEventRecord(c->ev1, st));
   if (!Nb) CK(outs.copy_out(st));
   CK(lay.copy_out(st));
   CK(to_host(c->prof_host, c->prof, 8, st));
@@ -971,6 +1007,16 @@ static int quad_solve_host(bool mixed, int B, int N, const int* Nb, const double
     scatter_horizons(slack_out, outs.in_copy(dsl, h.data()), B, Nb, n_s, 5, 1);
     memcpy(kkt_err, outs.in_copy(derr, h.data()), Bs * sizeof(double));
   }
+  return 0;
+}
+
+// constrSatisfaction over B problems on the device's stream (device pointers, laid out for P.N; Nb and Tsb together, and worst, may be
+// null).
+static int quad_check_dev(DevCtx& c, const QuadProblem& P, int B, const int* Nb, const double* Tsb, const double* x0, const double* xF,
+                          const double* x, const double* u, const double* ts, const double* lam, int* feasible, double* worst) {
+  const int grid = B < 4 * c.sms ? B : 4 * c.sms;
+  k_quad_check<<<grid, 128, 0, c.st>>>(P, B, Nb, Tsb, x0, xF, x, u, ts, lam, feasible, worst);
+  CK(cudaGetLastError());
   return 0;
 }
 
@@ -1006,9 +1052,8 @@ static int quad_check_host(int B, int N, const int* Nb, const double* Tsb, const
   lay.place(c->stage);
   cudaStream_t st = c->st;
   CK(lay.copy_in(st));
-  const int grid = B < 4 * c->sms ? B : 4 * c->sms;
-  k_quad_check<<<grid, 128, 0, st>>>(P, B, Nb ? dNb : nullptr, Nb ? dTs : nullptr, d0, dF, dx, du, dt, dl, dfeas, dw);
-  CK(cudaGetLastError());
+  rc = quad_check_dev(*c, P, B, Nb ? dNb : nullptr, Nb ? dTs : nullptr, d0, dF, dx, du, dt, dl, dfeas, dw);
+  if (rc) return rc;
   CK(lay.copy_out(st));
   CK(cudaStreamSynchronize(st));
   return 0;
@@ -1301,6 +1346,163 @@ int obca_parking_plan_solve_goals(int B, const double* x0, const double* xF, con
   CK(ol.copy_out(st));
   CK(pl.copy_out(st));
   CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int obca_quadcopter_plan_solve(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz, int n_ob,
+                               const double* lo, const double* hi, double reso, int max_nodes, double Ts, double R, const double* ob,
+                               double timeWS, int signed_dist, const obca_opts* opts, int Ncap, double* xp, double* up, double* ts,
+                               double* lp, double* slack, int* N, double* Tsb, int* status, int* expansions, int* exitflag, int* iters,
+                               double* kkt_err, int* feasible, double* worst, double* plan_seconds, double* solve_seconds) {
+  // the planner's checks and set-up (start and goal on its grid, scaled here as mainQuadcopter.jl:114-119 does), then the solve's;
+  // nothing is written before they pass
+  // the planner's stride: stages 0..Ncap, so a longer path comes back as OBCA_PLAN_CAPACITY (an Ncap out of range is refused below)
+  const int cap = Ncap >= 2 && Ncap <= QUAD_NMAX ? Ncap + 1 : 3;
+  std::vector<double> s3(3 * (size_t)(B > 0 ? B : 1)), g3(s3.size());
+  if (x0 && xF)
+    for (int p = 0; p < B; ++p)
+      for (int r = 0; r < 3; ++r) {
+        s3[3 * (size_t)p + r] = OBCA_QUAD_GRID_SCALE * x0[12 * (size_t)p + r];
+        g3[3 * (size_t)p + r] = OBCA_QUAD_GRID_SCALE * xF[12 * (size_t)p + r];
+      }
+  Plan3dSetupPtr S;
+  int rc = plan3d_prepare(S, B, x0 && xF && ob && xp && up && ts && lp && N && Tsb && status && exitflag && iters && kkt_err && feasible,
+                          s3.data(), g3.data(), ox, oy, oz, n_ob, lo, hi, reso, max_nodes, cap);
+  if (rc) return rc;
+  if (Ncap < 2) { set_err("Ncap < 2"); return OBCA_ERR_ARG; }
+  rc = check_quad_horizon(Ncap);
+  if (rc) return rc;
+  if (!(std::isfinite(Ts) && Ts > 0)) { set_err("Ts must be a finite number > 0"); return OBCA_ERR_ARG; }
+  if (obca_qflow::ts_hundredths(Ts, Ncap) < 1) {
+    set_err("Ts = " + std::to_string(Ts) + " gives a pair planned to N = Ncap = " + std::to_string(Ncap) + " the sampling time 0");
+    return OBCA_ERR_ARG;
+  }
+  QuadProblem P;
+  if (fill_quad_problem(P, Ncap, std::nan(""), R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  DevCtx* c;
+  const int dev = opts ? opts->device : 0;
+  rc = get_ctx(dev, &c);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = 0.0;
+  if (solve_seconds) *solve_seconds = 0.0;
+  if (B == 0) return 0;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  cudaStream_t st = c->st;
+  const size_t Bs = B;
+  // stage 1: plan into device buffers (N and expansions are copied in first: the planner leaves them alone where it does not write them)
+  Plan3dDevOut po;
+  double *d0, *dF;
+  int *dlist, *dNb, *dcnt;
+  DevLayout pl;
+  pl.add(po.rx, cap * Bs);
+  pl.add(po.ry, cap * Bs);
+  pl.add(po.rz, cap * Bs);
+  pl.inout(po.N, N, Bs);
+  pl.out(po.status, status, Bs);
+  pl.inout(po.expansions, expansions, Bs);
+  pl.in(d0, x0, 12 * Bs);
+  pl.in(dF, xF, 12 * Bs);
+  pl.add(dlist, Bs);
+  pl.add(dNb, Bs);
+  pl.add(dcnt, 2);
+  DevBuf dplan;
+  CK(alloc_layout(dplan, pl));
+  CK(pl.copy_in(st));
+  if (!expansions) po.expansions = nullptr;
+  float plan_ms = 0.f;
+  rc = plan3d_dev(*S, B, dev, st, po, &plan_ms);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = plan_ms * 1e-3;
+  // stage 2: list the pairs to solve; their count and longest horizon size the solve (its occupancy follows the layout's horizon)
+  k_flow_list<<<1, FLOW_LIST_THREADS, 0, st>>>(B, Ncap, po.status, po.N, dlist, dNb, dcnt);
+  CK(cudaGetLastError());
+  int cnt[2] = {0, 0};
+  CK(to_host(cnt, dcnt, 2, st));
+  CK(cudaStreamSynchronize(st));
+  const int Bq = cnt[0], M = cnt[1];
+  if (Bq == 0) {
+    CK(pl.copy_out(st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  // stage 3: the listed pairs' warm starts, x0, xF and sampling times as the inputs of the mixed solve at the horizon M; its outputs
+  // start as zeros.  The check takes the Dist bounds whatever the formulation, as obca_check_quadcopter_mixed does.
+  QuadProblem PM, PC;
+  fill_quad_problem(PM, M, std::nan(""), R, ob, signed_dist);      // the shape passed above, with 2 <= M <= Ncap
+  fill_quad_problem(PC, M, std::nan(""), R, ob, 0);
+  const size_t Qs = Bq, MS = M + 1;
+  obca_qflow::Gather g;
+  g.rx = po.rx; g.ry = po.ry; g.rz = po.rz; g.x0 = d0; g.xF = dF; g.Ts = Ts;
+  obca_qflow::Outs so;
+  char* dout;
+  DevLayout outs;
+  outs.add(so.xp, 12 * MS * Qs);
+  outs.add(so.up, 4 * (size_t)M * Qs);
+  outs.add(so.ts, MS * Qs);
+  outs.add(so.lp, 30 * MS * Qs);
+  outs.add(so.slack, 5 * MS * Qs);
+  outs.add(so.kkt_err, Qs);
+  outs.add(so.worst, Qs);
+  outs.add(so.exitflag, Qs);
+  outs.add(so.iters, Qs);
+  outs.add(so.feasible, Qs);
+  DevLayout sl_;
+  sl_.add(g.mxWS, 12 * MS * Qs);
+  sl_.add(g.mx0, 12 * Qs);
+  sl_.add(g.mxF, 12 * Qs);
+  sl_.add(g.mTsb, Qs);
+  sl_.add(dout, outs.bytes);
+  DevBuf dsolve;
+  CK(alloc_layout(dsolve, sl_));
+  outs.place(dout);
+  so.Tsb = g.mTsb;
+  CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
+  const size_t items = Qs * MS;
+  const int threads = 256, blocks = (int)((items + threads - 1) / threads);
+  k_qflow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
+  CK(cudaGetLastError());
+  // stage 4: the mixed solve; stage 5: constrSatisfaction on its outputs
+  IpmOpts O = to_ipm(opts);
+  if (!opts) O.max_iter = 3000;                        // as obca_quadcopter_solve_mixed
+  QBatchPtrs bp;
+  bp.x0 = g.mx0; bp.xF = g.mxF; bp.xWS = g.mxWS; bp.Nb = dNb; bp.Tsb = g.mTsb;
+  bp.timeWS = timeWS; bp.xp = so.xp; bp.up = so.up; bp.ts = so.ts; bp.lp = so.lp; bp.slack = so.slack;
+  bp.exitflag = so.exitflag; bp.iters = so.iters; bp.kkt_err = so.kkt_err; bp.B = Bq;
+  rc = quad_solve_dev(*c, PM, O, bp);
+  if (rc) return rc;
+  CK(to_host(c->prof_host, c->prof, 8, st));
+  rc = quad_check_dev(*c, PC, Bq, dNb, g.mTsb, g.mx0, g.mxF, so.xp, so.up, so.ts, so.lp, so.feasible, so.worst);
+  if (rc) return rc;
+  // stage 6: the solved pairs' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
+  // write keeps the caller's value), then everything back in one pass
+  double* slack_out = signed_dist ? slack : nullptr;      // the Dist formulation has no slacks
+  obca_qflow::Outs d;
+  const size_t NS = Ncap + 1;
+  DevLayout ol;
+  ol.inout(d.xp, xp, 12 * NS * Bs);
+  ol.inout(d.up, up, 4 * (size_t)Ncap * Bs);
+  ol.inout(d.ts, ts, NS * Bs);
+  ol.inout(d.lp, lp, 30 * NS * Bs);
+  ol.inout(d.slack, slack_out, slack_out ? 5 * NS * Bs : 0);
+  ol.inout(d.kkt_err, kkt_err, Bs);
+  ol.inout(d.Tsb, Tsb, Bs);
+  ol.inout(d.worst, worst, worst ? Bs : 0);
+  ol.inout(d.exitflag, exitflag, Bs);
+  ol.inout(d.iters, iters, Bs);
+  ol.inout(d.feasible, feasible, Bs);
+  DevBuf dcaller;
+  CK(alloc_layout(dcaller, ol));
+  if (!slack_out) d.slack = nullptr;
+  if (!worst) d.worst = nullptr;
+  CK(ol.copy_in(st));
+  k_qflow_scatter<<<blocks, threads, 0, st>>>(Bq, M, Ncap, dlist, dNb, so, d);
+  CK(cudaGetLastError());
+  CK(ol.copy_out(st));
+  CK(pl.copy_out(st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+  if (solve_seconds) *solve_seconds = ms * 1e-3;
   return 0;
 }
 

@@ -64,33 +64,27 @@ __global__ void __launch_bounds__(P3_WARPS * 32) k_plan3d(int B, A3Const C, A3IO
 
 }  // namespace
 
-extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy,
-                                                    const double* oz, int n_ob, const double* lo, const double* hi, double reso,
-                                                    int max_nodes, int cap, const obca_opts* opts, double* rx, double* ry, double* rz,
-                                                    int* N, int* status, int* expansions, double* plan_seconds) {
-  if (!rx || !ry || !rz || !N || !status) { obca_set_last_error("null argument"); return OBCA_ERR_ARG; }
-  if (max_nodes > A3_MAX_NODES) { obca_set_last_error("max_nodes > 2^28"); return OBCA_ERR_ARG; }
-  A3Setup S;
-  {
-    std::string why;
-    if (astar3d_setup(S, why, B, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, cap)) { obca_set_last_error(why); return OBCA_ERR_ARG; }
-  }
-  const int dev = opts ? opts->device : 0;
-  const int rc = check_device(dev);
-  if (rc) return rc;
-  if (plan_seconds) *plan_seconds = 0.0;
-  if (B == 0) return 0;
-  if (max_nodes <= 0) max_nodes = P3_DEFAULT_NODES;
-  A3Const C = S.C;
-  C.max_nodes = max_nodes;
-  C.max_queue = max_nodes / 4 > 64 ? max_nodes / 4 : 64;
+struct Plan3dSetup : A3Setup {};
+void Plan3dSetupFree::operator()(Plan3dSetup* s) const { delete s; }
 
+int plan3d_prepare(Plan3dSetupPtr& S, int B, bool args, const double* x0, const double* xF, const double* ox, const double* oy,
+                   const double* oz, int n_ob, const double* lo, const double* hi, double reso, int max_nodes, int cap) {
+  if (!args) { obca_set_last_error("null argument"); return OBCA_ERR_ARG; }
+  if (max_nodes > A3_MAX_NODES) { obca_set_last_error("max_nodes > 2^28"); return OBCA_ERR_ARG; }
+  S.reset(new Plan3dSetup);
+  std::string why;
+  if (astar3d_setup(*S, why, B, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, cap)) { obca_set_last_error(why); return OBCA_ERR_ARG; }
+  if (max_nodes <= 0) max_nodes = P3_DEFAULT_NODES;
+  S->C.max_nodes = max_nodes;
+  S->C.max_queue = max_nodes / 4 > 64 ? max_nodes / 4 : 64;
+  return 0;
+}
+
+int plan3d_dev(const Plan3dSetup& S, int B, int dev, cudaStream_t st, const Plan3dDevOut& out, float* plan_ms) {
+  A3Const C = S.C;
   int sms = 0;
-  Stream st;
   Event e0, e1;
-  CK(cudaSetDevice(dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CK(cudaStreamCreateWithFlags(&st.h, cudaStreamNonBlocking));
   CK(cudaEventCreate(&e0.h));
   CK(cudaEventCreate(&e1.h));
   const int grid = (B + P3_WARPS - 1) / P3_WARPS < sms ? (B + P3_WARPS - 1) / P3_WARPS : sms;
@@ -106,8 +100,8 @@ extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, con
   cl.add(dcounter, 1);
   DevBuf dconst;
   CK(alloc_layout(dconst, cl));
-  CK(cl.copy_in(st.h));
-  CK(cudaMemsetAsync(dcounter, 0, sizeof(int), st.h));
+  CK(cl.copy_in(st));
+  CK(cudaMemsetAsync(dcounter, 0, sizeof(int), st));
   C.map = dmap;
   // per warp: cell table, node pool, queue
   const size_t table_stride = DevLayout::padded((size_t)(S.cells > 0 ? S.cells : 1) * sizeof(int)) / sizeof(int);
@@ -118,30 +112,53 @@ extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, con
   wl.add(W0.queue, (size_t)C.max_queue * nw);
   DevBuf dscr;
   CK(alloc_layout(dscr, wl));
-  CK(cudaMemsetAsync(W0.table, 0xff, table_stride * nw * sizeof(int), st.h));      // -1: no node
-  // outputs: copied in first, so that the kernel leaves every entry it does not write as the caller had it
-  const size_t cb = Bs * cap;
-  double *drx, *dry, *drz;
-  int *dN, *dst, *dex;
+  CK(cudaMemsetAsync(W0.table, 0xff, table_stride * nw * sizeof(int), st));      // -1: no node
+  const A3IO io{ds, dg, out.rx, out.ry, out.rz, out.N, out.status, out.expansions, nullptr, nullptr};
+  CK(cudaEventRecord(e0.h, st));
+  k_plan3d<<<grid, P3_WARPS * 32, 0, st>>>(B, C, io, W0, table_stride, dcounter);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e1.h, st));
+  CK(cudaStreamSynchronize(st));      // the scratch is freed on return
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e0.h, e1.h));
+  if (plan_ms) *plan_ms = ms;
+  return 0;
+}
+
+// The outputs are copied to the device first, so that the kernel leaves every entry it does not write as the caller had it.
+extern "C" int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, const double* xF, const double* ox, const double* oy,
+                                                    const double* oz, int n_ob, const double* lo, const double* hi, double reso,
+                                                    int max_nodes, int cap, const obca_opts* opts, double* rx, double* ry, double* rz,
+                                                    int* N, int* status, int* expansions, double* plan_seconds) {
+  Plan3dSetupPtr S;
+  int rc = plan3d_prepare(S, B, rx && ry && rz && N && status, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, max_nodes, cap);
+  if (rc) return rc;
+  const int dev = opts ? opts->device : 0;
+  rc = check_device(dev);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = 0.0;
+  if (B == 0) return 0;
+  Stream st;
+  CK(cudaSetDevice(dev));
+  CK(cudaStreamCreateWithFlags(&st.h, cudaStreamNonBlocking));
+  const size_t Bs = (size_t)B, cb = Bs * cap;
+  Plan3dDevOut o;
   DevLayout il;
-  il.inout(drx, rx, cb);
-  il.inout(dry, ry, cb);
-  il.inout(drz, rz, cb);
-  il.inout(dN, N, Bs);
-  il.out(dst, status, Bs);
-  il.inout(dex, expansions, Bs);
+  il.inout(o.rx, rx, cb);
+  il.inout(o.ry, ry, cb);
+  il.inout(o.rz, rz, cb);
+  il.inout(o.N, N, Bs);
+  il.out(o.status, status, Bs);
+  il.inout(o.expansions, expansions, Bs);
   DevBuf dio;
   CK(alloc_layout(dio, il));
   CK(il.copy_in(st.h));
-  const A3IO io{ds, dg, drx, dry, drz, dN, dst, expansions ? dex : nullptr, nullptr, nullptr};
-  CK(cudaEventRecord(e0.h, st.h));
-  k_plan3d<<<grid, P3_WARPS * 32, 0, st.h>>>(B, C, io, W0, table_stride, dcounter);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(e1.h, st.h));
+  if (!expansions) o.expansions = nullptr;
+  float ms = 0.f;
+  rc = plan3d_dev(*S, B, dev, st.h, o, &ms);
+  if (rc) return rc;
   CK(il.copy_out(st.h));
   CK(cudaStreamSynchronize(st.h));
-  float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, e0.h, e1.h));
   if (plan_seconds) *plan_seconds = ms * 1e-3;
   return 0;
 }

@@ -2,7 +2,9 @@
   - obca_plan_parking_warmstart_batch, Hybrid A*: B start poses towards one goal in one call (plan_raw, plan_batch);
   - obca_plan_parking_warmstart_goals, the same with a goal per pose among any point cloud (plan_goals_raw, plan_goals_batch);
   - obca_plan_quadcopter_warmstart_batch, the 3-D A* of the quadcopter flow: B start / goal pairs in one call (plan_quadcopter_raw,
-    plan_quadcopter_batch).
+    plan_quadcopter_batch);
+  - obca_parking_plan_solve_goals and obca_quadcopter_plan_solve, which plan, solve and check a batch in one call without leaving the
+    device (plan_solve_goals, plan_solve_quadcopter and their *_raw twins).
 Without a CUDA device the calls raise.  A search that outgrows the device's scratch comes back as POOL_FULL in `status` (the *_raw
 functions); the *_batch functions plan those problems with the host planner, which makes the same decisions."""
 from __future__ import annotations
@@ -253,3 +255,97 @@ def plan_solve_batch(x0s, xF, nOb, vOb, A, b, ego, XYbounds, scenario="backwards
     ox, oy = native.obstacle_points(scenario)
     Ts = Ts or (0.6 if scenario == "backwards" else 0.9) / 3 * sampleN
     return plan_solve_goals(x0s, np.asarray(xF, float)[:4], ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, **kw)
+
+
+def plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS=1.0, signed_dist=1, Ncap=511, max_nodes=0,
+                              opts=None, host_fallback=False):
+    """obca_quadcopter_plan_solve's outputs as arrays: plan every pair x0s[i] -> xFs[i] ((B, 12) in the solve's units; the planner takes
+    10 x rows 0-2) among the cloud (ox, oy, oz, lo, hi, reso in the planner's units), build the warm starts, solve the pairs that
+    planned and check the results, in one call.  Per-pair arrays in the entry's layout for Ncap, row-major views of the column-major
+    blocks: xp (B, Ncap+1, 12), up (B, Ncap, 4), ts (B, Ncap+1), lp (B, Ncap+1, 30), slack (B, Ncap+1, 5); one value per pair: N, Tsb,
+    status, expansions, exitflag, iters, kkt_err, feasible, worst; and plan_seconds, time (the solve's device seconds).  The buffers start
+    as NaN (the integers as -1): entries the call does not write stay so.  opts None: defaults with max_iter = 3000, as
+    quadcopter.quadcopter_solve_mixed.  host_fallback: the pairs whose search outgrew the device's scratch (POOL_FULL) are planned by the
+    host library (native.astar3d_raw, the same decisions), and those that plan to 2 <= N <= Ncap get their warm starts from
+    native.quadcopter_warm_start and are solved and checked by quadcopter_solve_mixed / check_quadcopter_mixed in one more call each
+    (their solve time is not in `time`)."""
+    from .._lib import f64
+    x0s = f64(np.asarray(x0s, float).reshape(-1, 12)); B = x0s.shape[0]
+    xFs = f64(np.broadcast_to(np.asarray(xFs, float).reshape(-1, 12), (B, 12)))
+    ox, oy, oz, lo, hi = (f64(np.asarray(a, float).ravel()) for a in (ox, oy, oz, lo, hi))
+    ob = f64(np.asarray(obs, float).reshape(5, 6))
+    NS = Ncap + 1
+    nan = lambda *s: np.full(s, np.nan)
+    i32 = lambda: np.full(B, -1, np.int32)
+    o = dict(xp=nan(B, NS, 12), up=nan(B, Ncap, 4), ts=nan(B, NS), lp=nan(B, NS, 30), slack=nan(B, NS, 5), N=i32(), Tsb=nan(B),
+             status=i32(), expansions=i32(), exitflag=i32(), iters=i32(), kkt_err=nan(B), feasible=i32(), worst=nan(B))
+    secs = np.zeros(2)
+    if opts is None:
+        opts = _lib.default_opts(); opts.max_iter = 3000
+    p = _lib.ptr
+    f = _lib.lib().obca_quadcopter_plan_solve
+    f.restype = C.c_int
+    f.argtypes = ([C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_double, C.c_double, C.c_void_p,
+                                                    C.c_double, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 16)
+    rc = f(B, p(x0s), p(xFs), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), float(Ts), float(R), p(ob),
+           float(timeWS), int(signed_dist), C.cast(C.byref(opts), C.c_void_p), int(Ncap),
+           *[p(o[k]) for k in ("xp", "up", "ts", "lp", "slack", "N", "Tsb", "status", "expansions", "exitflag", "iters", "kkt_err",
+                               "feasible", "worst")], p(secs[:1]), p(secs[1:]))
+    _lib.check(rc)
+    o["plan_seconds"], o["time"] = float(secs[0]), float(secs[1])
+    full = np.flatnonzero(o["status"] == POOL_FULL)
+    if host_fallback and full.size:
+        _solve_quadcopter_on_host_plans(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS, signed_dist, Ncap, opts)
+    return o
+
+
+def _solve_quadcopter_on_host_plans(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS, signed_dist, Ncap, opts):
+    """Plan the pairs `full` with the host library, then solve and check the ones it plans to 2 <= N <= Ncap; their entries of o (the
+    layout of plan_solve_quadcopter_raw) get the results, the others the host planner's status (OBCA_PLAN_CAPACITY for a horizon outside
+    [2, Ncap])."""
+    from .. import quadcopter
+    h = native.astar3d_raw(x0s[full, :3] * 10.0, xFs[full, :3] * 10.0, ox, oy, oz, lo, hi, reso, Ncap + 1)
+    st = h["status"].copy()
+    st[(st == 0) & (h["N"] < 2)] = 2
+    o["status"][full] = st; o["N"][full] = h["N"]; o["expansions"][full] = h["expansions"]
+    ok = np.flatnonzero(st == 0)
+    if ok.size == 0:
+        return
+    Ns = h["N"][ok]
+    ws = [native.quadcopter_warm_start(h["rx"][i, :n + 1].copy(), h["ry"][i, :n + 1].copy(), h["rz"][i, :n + 1].copy(), Ts)
+          for i, n in zip(ok, Ns)]
+    Tsb = np.array([w["Ts"] for w in ws])
+    x0, xF = x0s[full[ok]], xFs[full[ok]]
+    r = quadcopter.quadcopter_solve_mixed(x0, xF, Ns, Tsb, R, obs, [w["xWS"] for w in ws], timeWS, signed_dist, opts=opts)
+    feas, worst = quadcopter.check_quadcopter_mixed(r["xp"], r["up"], r["ts"], x0, xF, Ns, Tsb, r["lp"], obs, R, opts=opts)
+    for q, (i, n) in enumerate(zip(full[ok], Ns)):
+        for k, ext in (("xp", 1), ("up", 0), ("lp", 1)) + ((("slack", 1),) if signed_dist else ()):
+            o[k][i, :n + ext] = r[k][q].T
+        o["ts"][i, :n + 1] = r["ts"][q]
+    for k, v in (("Tsb", Tsb), ("exitflag", r["exitflag"]), ("iters", r["iters"]), ("kkt_err", r["kkt_err"]), ("feasible", feas),
+                 ("worst", worst)):
+        o[k][full[ok]] = v
+
+
+def plan_solve_quadcopter(x0s, xFs, R, obs, Ts=0.25, signed_dist=1, Ncap=511, max_nodes=0, opts=None, host_fallback=False):
+    """mainQuadcopter.jl:114-154 for a batch in one call (obca_quadcopter_plan_solve): plan every start / goal pair (x0s, xFs (B, 12))
+    among the environment of a_star_3d.quadcopter_environment() (reso = 1), build the warm starts, solve and check.  Returns the keys of
+    quadcopter.quadcopter_solve_mixed in the caller's pair order -- per-pair lists in the Julia shapes (xp[i] 12 x (N[i]+1), up[i]
+    4 x N[i], ts[i], lp[i] 30 x (N[i]+1), slack[i] 5 x (N[i]+1), the last for signed_dist = 1 only), None where the pair was not solved,
+    and the arrays exitflag, iters, kkt_err, N, Ts (the pairs' sampling times), time -- plus status (OBCA_PLAN_* of include/obca.h:
+    0 solved, 1 no path, 2 horizon outside [2, Ncap], 4 POOL_FULL: the search outgrew the device's scratch), expansions, feasible
+    (constrSatisfaction's value), worst and plan_seconds.  host_fallback: plan, solve and check the POOL_FULL pairs on the host library's
+    plans (see plan_solve_quadcopter_raw)."""
+    from .a_star_3d import quadcopter_environment
+    ox, oy, oz, lo, hi = quadcopter_environment()
+    o = plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, 1.0, Ts, R, obs, 1.0, signed_dist, Ncap, max_nodes, opts, host_fallback)
+    ok = o["status"] == 0
+    cut = lambda a, ext: [a[i, :n + ext].T.copy() if ok[i] else None for i, n in enumerate(o["N"])]
+    out = dict(xp=cut(o["xp"], 1), up=cut(o["up"], 0), ts=[o["ts"][i, :n + 1].copy() if ok[i] else None for i, n in enumerate(o["N"])],
+               lp=cut(o["lp"], 1), slack=cut(o["slack"], 1) if signed_dist else [None] * len(ok))
+    for k in ("exitflag", "iters", "feasible"):
+        out[k] = np.where(ok, o[k], 0).astype(np.int32)
+    out.update(kkt_err=np.where(ok, o["kkt_err"], np.nan), worst=np.where(ok, o["worst"], np.nan), N=o["N"].copy(),
+               Ts=np.where(ok, o["Tsb"], np.nan), status=o["status"].copy(), expansions=o["expansions"].copy(), time=o["time"],
+               plan_seconds=o["plan_seconds"])
+    return out
