@@ -7,9 +7,11 @@ GPU call (obca_quadcopter_solve_mixed), run the reference's constrSatisfaction o
 horizon exceeds the solver's limit (N + 1 <= 512; the planner gives N = 80..147 over the config-4 box) are counted and listed
 as skipped.  Planner "flow" does all of it -- plan, warm start, solve, check -- in one call that keeps everything on the GPU
 (device.plan_solve_quadcopter, obca_quadcopter_plan_solve), with the pairs whose search outgrew the device's scratch planned on the host;
-it prints the same counts as "gpu".
+it prints the same counts as "gpu".  Planner "both" plans once in one call and solves and checks with QuadcopterDist and then
+QuadcopterSignedDist in the same call (device.plan_solve_quadcopter_both, obca_quadcopter_plan_solve_both), as mainQuadcopter.jl:145-154
+does for one pair; it prints one line per formulation.
 
-usage: python examples/sweep_quadcopter.py [K] [seed] [workers] [python|host|gpu|flow]      (needs a CUDA device for the solves)
+usage: python examples/sweep_quadcopter.py [K] [seed] [workers] [python|host|gpu|flow|both]      (needs a CUDA device for the solves)
 """
 import os
 import sys
@@ -71,8 +73,30 @@ def flow(sc, K, signed_dist, t0):
     return out
 
 
+def both(K=32, seed=2):
+    """Every pair planned once on the GPU (POOL_FULL pairs on the host), then solved and checked with both formulations."""
+    sc = scenarios.quadcopter_batch(K, seed=seed)
+    o = device.plan_solve_quadcopter_both(sc["x0"], sc["xF"], sc["R"], sc["obs"], sc["Ts80"], Ncap=N_LIMIT, host_fallback=True)
+    ok = o["status"] == 0
+    return dict(K=K, planned=int(ok.sum()), N=np.where(ok, o["N"], -1), t_plan=o["plan_seconds"],
+                sets={f: dict(converged=int((o[f]["exitflag"][ok] == 1).sum()), feasible=int(o[f]["feasible"][ok].sum()),
+                              t_solve=o[f]["time"]) for f in ("dist", "sd")})
+
+
 if __name__ == "__main__":
     a = sys.argv
+    if len(a) > 4 and a[4] == "both":
+        try:
+            o = both(int(a[1]) if len(a) > 1 else 32, int(a[2]) if len(a) > 2 else 2)
+        except obca_b200.ObcaError as e:
+            print("solve not run:", e); sys.exit(2)
+        n = o["N"][o["N"] >= 0]
+        print(f"{o['K']} start / goal pairs: {o['planned']} planned once in {o['t_plan']:.2f} s GPU device time, N = {n.min()}..{n.max()}")
+        for f, name in (("dist", "QuadcopterDist"), ("sd", "QuadcopterSignedDist")):
+            s = o["sets"][f]
+            print(f"{name}: {o['planned']} planned, {s['converged']} converged, {s['feasible']} pass constrSatisfaction, "
+                  f"solve {s['t_solve'] * 1e3:.0f} ms device time")
+        sys.exit(0)
     try:
         o = sweep(int(a[1]) if len(a) > 1 else 32, int(a[2]) if len(a) > 2 else 2, 1, int(a[3]) if len(a) > 3 and int(a[3]) > 0 else None,
                   a[4] if len(a) > 4 else "python")

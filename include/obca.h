@@ -19,6 +19,8 @@
  *                                 come with their own N and Ts = round(Ts*80/N, 2))
  *   obca_quadcopter_plan_solve: mainQuadcopter.jl:114-154 (plan -> warm start -> solve -> check) for a batch of start / goal
  *                                 pairs in one call
+ *   obca_parking_plan_solve_both / obca_quadcopter_plan_solve_both: the same two flows planned once and solved with both
+ *                                 formulations, Distance then Signed Distance, as main.jl and mainQuadcopter.jl run them
  *
  * Conventions
  *   - every array is float64, COLUMN-MAJOR exactly as the Julia caller holds it; a batch of B problems is the B
@@ -342,8 +344,8 @@ int obca_plan_quadcopter_warmstart_batch(int B, const double* x0, const double* 
  * obca_plan_quadcopter_warmstart_batch), freed before the solve allocates; then the solve's inputs and outputs for the Bs pairs it
  * takes, about 8 x Bs x (Nmax + 1) x 64 bytes, its workspace (as obca_quadcopter_solve_mixed at Nmax), and at the end the caller's
  * outputs, about 8 x B x (Ncap + 1) x 52 bytes, which are copied to the device first.
- * One call solves one formulation: mainQuadcopter.jl solves QuadcopterDist and QuadcopterSignedDist on the same plan, which here plans
- * twice (solving both from one plan is a possible extension).
+ * One call solves one formulation: mainQuadcopter.jl solves QuadcopterDist and QuadcopterSignedDist on the same plan, which
+ * obca_quadcopter_plan_solve_both does from one plan.
  * Return: 0, OBCA_ERR_ARG (the planner's: a null required array, max_nodes > 2^28, B < 0, n_ob < 0, reso <= 0, a non-finite coordinate,
  * a map of more than 2^27 cells or a start / goal more than 2^30 cells from it; Ncap < 2; Ts not a finite number > 0, or so small that
  * jround(Ts * 80 / Ncap * 100) < 1, which would give a pair a sampling time of 0), OBCA_ERR_UNSUPPORTED (Ncap > 511, the bound in
@@ -354,6 +356,70 @@ int obca_quadcopter_plan_solve(int B, const double* x0, const double* xF, const 
                                double timeWS, int signed_dist, const obca_opts* opts, int Ncap, double* xp, double* up, double* ts,
                                double* lp, double* slack, int* N, double* Tsb, int* status, int* expansions, int* exitflag, int* iters,
                                double* kkt_err, int* feasible, double* worst, double* plan_seconds, double* solve_seconds);
+
+/* The outputs of one formulation of a flow call that solves both (obca_parking_plan_solve_both, obca_quadcopter_plan_solve_both):
+ * the arrays obca_parking_plan_solve_goals / obca_quadcopter_plan_solve take for their solve and check, with the same shapes, layout
+ * and nullability.  Parking: sl, strict and solve_seconds may be NULL, every other field is required.  Quadcopter: slack, worst and
+ * solve_seconds may be NULL, every other field is required; slack is written for the Signed Distance set only. */
+typedef struct obca_parking_flow_out {
+  double *xp, *up, *ts, *lp, *np, *sl;
+  int *exitflag, *iters;
+  double* kkt_err;
+  int *feasible, *strict;
+  double* solve_seconds;
+} obca_parking_flow_out;
+
+typedef struct obca_quadcopter_flow_out {
+  double *xp, *up, *ts, *lp, *slack;
+  int *exitflag, *iters;
+  double* kkt_err;
+  int* feasible;
+  double* worst;
+  double* solve_seconds;
+} obca_quadcopter_flow_out;
+
+/* main.jl:215-269 as the reference runs it: plan every start pose ONCE, then solve and check the poses that planned with ParkingDist
+ * (main.jl:258) and then with ParkingSignedDist (main.jl:269), in one call.  Inputs and shared outputs (N, status, expansions,
+ * plan_seconds) are those of obca_parking_plan_solve_goals without signed_dist, written once as it writes them.  dist and sd (both
+ * required) receive the outputs of the Distance and the Signed Distance formulation: each set is bit for bit what
+ * obca_parking_plan_solve_goals with signed_dist = 0 / 1 writes for the same inputs, including the entries it leaves as the caller had
+ * them (poses not solved, entries past a pose's own horizon).  Both solves take the same listed poses at the same layout horizon Nmax,
+ * and DualMultWS runs inside each, as in the reference.  The Distance solve runs first: after the call obca_last_times,
+ * obca_last_schedule and obca_last_profile report the Signed Distance solve.
+ * Device memory: the peak of obca_parking_plan_solve_goals at the same B, Ncap and shape.  The planner's buffers and the gathered
+ * solve inputs and outputs stay allocated across both solves; for each formulation the outputs are zeroed, solved, checked, scattered
+ * to the caller's layout (about 8 x B x (Ncap + 1) x (7 + V + 5 nOb) bytes, copied to the device first) and copied back, and that
+ * caller-layout staging is freed before the next formulation runs.
+ * Return: the refusals of obca_parking_plan_solve_goals, and OBCA_ERR_ARG for a null dist or sd, or a null required field of either
+ * (obca_last_error() names it, e.g. "null argument: sd.xp"), all before any device work and with nothing written; OBCA_ERR_NO_DEVICE;
+ * OBCA_ERR_CUDA, after which the dist set may already have been written.  B = 0, or a batch in which no pose is solved, returns 0
+ * without a solve, with both solve_seconds 0. */
+int obca_parking_plan_solve_both(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts,
+                                 double L, int sampleN, int max_expansions, int max_nodes, int nOb, const int* vOb, const double* A,
+                                 const double* b, const double* ego, const double* XYbounds, int fixTime, const obca_opts* opts,
+                                 int Ncap, int* N, int* status, int* expansions, double* plan_seconds, const obca_parking_flow_out* dist,
+                                 const obca_parking_flow_out* sd);
+
+/* mainQuadcopter.jl:114-154 as the reference runs it: plan every start / goal pair ONCE and build its warm start, then solve and check
+ * the pairs that planned with QuadcopterDist and constrSatisfaction (:145-147) and then with QuadcopterSignedDist and constrSatisfaction
+ * (:152-154), in one call.  Inputs and shared outputs (N, Tsb, status, expansions, plan_seconds) are those of obca_quadcopter_plan_solve
+ * without signed_dist, written once as it writes them.  dist and sd (both required) receive the outputs of the Distance and the Signed
+ * Distance formulation: each set is bit for bit what obca_quadcopter_plan_solve with signed_dist = 0 / 1 writes for the same inputs,
+ * including the entries it leaves as the caller had them (dist->slack is never written).  The Distance solve runs first: after the call
+ * obca_last_profile reports the Signed Distance solve.
+ * Device memory: the peak of obca_quadcopter_plan_solve at the same B and Ncap.  The planner's buffers, the pairs' states and the
+ * gathered solve inputs and outputs stay allocated across both solves; for each formulation the outputs are zeroed, solved, checked,
+ * scattered to the caller's layout (about 8 x B x (Ncap + 1) x 52 bytes, copied to the device first) and copied back, and that
+ * caller-layout staging is freed before the next formulation runs.
+ * Return: the refusals of obca_quadcopter_plan_solve, and OBCA_ERR_ARG for a null dist or sd, or a null required field of either
+ * (obca_last_error() names it, e.g. "null argument: dist.feasible"), all before any device work and with nothing written;
+ * OBCA_ERR_NO_DEVICE; OBCA_ERR_CUDA, after which the dist set may already have been written.  B = 0, or a batch in which no pair is
+ * solved, returns 0 without a solve, with both solve_seconds 0. */
+int obca_quadcopter_plan_solve_both(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz,
+                                    int n_ob, const double* lo, const double* hi, double reso, int max_nodes, double Ts, double R,
+                                    const double* ob, double timeWS, const obca_opts* opts, int Ncap, int* N, double* Tsb, int* status,
+                                    int* expansions, double* plan_seconds, const obca_quadcopter_flow_out* dist,
+                                    const obca_quadcopter_flow_out* sd);
 
 /* Device times of the last obca_parking_solve_batch[_dev] / obca_parking_solve_mixed on `device`: DualMultWS (0 when the caller passed lWS / nWS) and the
  * solve alone (= what solve_seconds reports; the reference's `time`, ParkingSignedDist.jl:297). */

@@ -212,3 +212,80 @@ function plan_solve_quadcopter(x0s::AbstractMatrix, xFs::AbstractMatrix, ox::Abs
             timeScale = [ok[i] ? ts[1:N[i]+1, i] : nothing for i in 1:B], lp = [cut(lp, i, N[i] + 1) for i in 1:B],
             status = status, N = N, Ts = Tsb, exitflag = flag, iters = iters, feasible = feasible, plan_time = ps[], solve_time = ss[])
 end
+
+# ---- one plan, both formulations (include/obca.h: obca_parking_plan_solve_both, obca_quadcopter_plan_solve_both) ----------------------
+# main.jl:215-269 and mainQuadcopter.jl:114-154 as the reference runs them: every problem planned once, then solved and checked with the
+# Distance and then the Signed Distance formulation in the same call.  Each formulation's outputs go through one struct of pointers
+# (obca_parking_flow_out / obca_quadcopter_flow_out), passed by Ref.  Like every stub in this file they are not executed in this
+# repository (no Julia in the build image); the tested twins are obca_b200.planner.device.plan_solve_goals_both and
+# plan_solve_quadcopter_both (tests/test_gpu_plan_solve_both.py).
+struct ParkingFlowOut
+    xp::Ptr{Cdouble}; up::Ptr{Cdouble}; ts::Ptr{Cdouble}; lp::Ptr{Cdouble}; np::Ptr{Cdouble}; sl::Ptr{Cdouble}
+    exitflag::Ptr{Cint}; iters::Ptr{Cint}; kkt_err::Ptr{Cdouble}; feasible::Ptr{Cint}; strict::Ptr{Cint}; solve_seconds::Ptr{Cdouble}
+end
+
+struct QuadcopterFlowOut
+    xp::Ptr{Cdouble}; up::Ptr{Cdouble}; ts::Ptr{Cdouble}; lp::Ptr{Cdouble}; slack::Ptr{Cdouble}
+    exitflag::Ptr{Cint}; iters::Ptr{Cint}; kkt_err::Ptr{Cdouble}; feasible::Ptr{Cint}; worst::Ptr{Cdouble}; solve_seconds::Ptr{Cdouble}
+end
+
+# Returns (status, N, plan_time, dist, sd): dist and sd hold the per-pose vectors and values plan_solve_goals returns for one formulation.
+function plan_solve_goals_both(x0s::AbstractMatrix, xFs::AbstractMatrix, ox::AbstractVector, oy::AbstractVector, Ts, L, nOb, vOb, A,
+                               b, ego, XYbounds; sampleN::Int = 3, Ncap::Int = 319, fixTime::Int = 0, max_nodes::Int = 0,
+                               max_expansions::Int = 0)
+    B = size(x0s, 1); V = Int(sum(vOb)); NS = Ncap + 1
+    mk() = (xp = zeros(4, NS, B), up = zeros(2, Ncap, B), ts = zeros(NS, B), lp = zeros(V, NS, B), np = zeros(4 * nOb, NS, B),
+            sl = zeros(nOb, NS, B), flag = zeros(Cint, B), iters = zeros(Cint, B), kkt = zeros(B), feasible = zeros(Cint, B),
+            strict = zeros(Cint, B), ss = zeros(1))
+    sets = (mk(), mk())
+    N = fill(Cint(-1), B); status = fill(Cint(-1), B); expansions = zeros(Cint, B); ps = Ref{Cdouble}(0.0)
+    rc = GC.@preserve sets begin
+        outs = [Ref(ParkingFlowOut(pointer(s.xp), pointer(s.up), pointer(s.ts), pointer(s.lp), pointer(s.np), pointer(s.sl), pointer(s.flag),
+                                   pointer(s.iters), pointer(s.kkt), pointer(s.feasible), pointer(s.strict), pointer(s.ss))) for s in sets]
+        ccall((:obca_parking_plan_solve_both, LIBOBCA), Cint,
+              (Cint, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint, Cdouble, Cdouble, Cint, Cint, Cint, Cint, Ptr{Cint},
+               Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint, Ref{ObcaOpts}, Cint, Ptr{Cint}, Ptr{Cint}, Ptr{Cint},
+               Ref{Cdouble}, Ref{ParkingFlowOut}, Ref{ParkingFlowOut}),
+              B, _f64(permutedims(x0s[:, 1:4])), _f64(permutedims(xFs[:, 1:4])), _f64(ox), _f64(oy), length(ox), Ts, L, sampleN,
+              max_expansions, max_nodes, nOb, Cint.(vec(vOb)), _f64(A), _f64(vec(b)), _f64(vec(ego)), _f64(vec(XYbounds)), fixTime,
+              obca_default_opts(), Ncap, N, status, expansions, ps, outs[1], outs[2])
+    end
+    rc == 0 || error("obca_parking_plan_solve_both: ", rc, " ", unsafe_string(ccall((:obca_last_error, LIBOBCA), Cstring, ())))
+    ok = status .== 0
+    cut(a, i, n) = ok[i] ? a[:, 1:n, i] : nothing
+    one(s) = (xp = [cut(s.xp, i, N[i] + 1) for i in 1:B], up = [cut(s.up, i, N[i]) for i in 1:B],
+              timeScale = [ok[i] ? s.ts[1:N[i]+1, i] : nothing for i in 1:B], lp = [cut(s.lp, i, N[i] + 1) for i in 1:B],
+              np = [cut(s.np, i, N[i] + 1) for i in 1:B], exitflag = s.flag, iters = s.iters, feasible = s.feasible, solve_time = s.ss[1])
+    return (status = status, N = N, plan_time = ps[], dist = one(sets[1]), sd = one(sets[2]))
+end
+
+# Returns (status, N, Ts, plan_time, dist, sd): dist and sd hold the per-pair vectors and values plan_solve_quadcopter returns for one
+# formulation.
+function plan_solve_quadcopter_both(x0s::AbstractMatrix, xFs::AbstractMatrix, ox::AbstractVector, oy::AbstractVector,
+                                    oz::AbstractVector, lo::AbstractVector, hi::AbstractVector, R, ob1, ob2, ob3, ob4, ob5;
+                                    Ts::Float64 = 0.25, reso::Float64 = 1.0, Ncap::Int = 511, max_nodes::Int = 0, timeWS::Float64 = 1.0)
+    B = size(x0s, 1); NS = Ncap + 1
+    ob = hcat(vec(_f64(ob1)), vec(_f64(ob2)), vec(_f64(ob3)), vec(_f64(ob4)), vec(_f64(ob5)))     # 6 x 5
+    mk() = (xp = zeros(12, NS, B), up = zeros(4, Ncap, B), ts = zeros(NS, B), lp = zeros(30, NS, B), sl = zeros(5, NS, B),
+            flag = zeros(Cint, B), iters = zeros(Cint, B), kkt = zeros(B), feasible = zeros(Cint, B), worst = zeros(B), ss = zeros(1))
+    sets = (mk(), mk())
+    N = fill(Cint(-1), B); Tsb = zeros(B); status = fill(Cint(-1), B); expansions = zeros(Cint, B); ps = Ref{Cdouble}(0.0)
+    rc = GC.@preserve sets begin
+        outs = [Ref(QuadcopterFlowOut(pointer(s.xp), pointer(s.up), pointer(s.ts), pointer(s.lp), pointer(s.sl), pointer(s.flag),
+                                      pointer(s.iters), pointer(s.kkt), pointer(s.feasible), pointer(s.worst), pointer(s.ss))) for s in sets]
+        ccall((:obca_quadcopter_plan_solve_both, LIBOBCA), Cint,
+              (Cint, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint, Ptr{Cdouble}, Ptr{Cdouble}, Cdouble,
+               Cint, Cdouble, Cdouble, Ptr{Cdouble}, Cdouble, Ref{ObcaOpts}, Cint, Ptr{Cint}, Ptr{Cdouble}, Ptr{Cint}, Ptr{Cint},
+               Ref{Cdouble}, Ref{QuadcopterFlowOut}, Ref{QuadcopterFlowOut}),
+              B, _f64(permutedims(x0s[:, 1:12])), _f64(permutedims(xFs[:, 1:12])), _f64(ox), _f64(oy), _f64(oz), length(ox),
+              _f64(lo), _f64(hi), reso, max_nodes, Ts, Float64(R), ob, timeWS, (o = obca_default_opts(); o.max_iter = 3000; o), Ncap,
+              N, Tsb, status, expansions, ps, outs[1], outs[2])
+    end
+    rc == 0 || error("obca_quadcopter_plan_solve_both: ", rc, " ", unsafe_string(ccall((:obca_last_error, LIBOBCA), Cstring, ())))
+    ok = status .== 0
+    cut(a, i, n) = ok[i] ? a[:, 1:n, i] : nothing
+    one(s) = (xp = [cut(s.xp, i, N[i] + 1) for i in 1:B], up = [cut(s.up, i, N[i]) for i in 1:B],
+              timeScale = [ok[i] ? s.ts[1:N[i]+1, i] : nothing for i in 1:B], lp = [cut(s.lp, i, N[i] + 1) for i in 1:B],
+              exitflag = s.flag, iters = s.iters, feasible = s.feasible, solve_time = s.ss[1])
+    return (status = status, N = N, Ts = Tsb, plan_time = ps[], dist = one(sets[1]), sd = one(sets[2]))
+end

@@ -17,7 +17,7 @@ SYMBOLS = ["obca_version", "obca_device_count", "obca_last_error", "obca_default
            "obca_quadcopter_solve_batch", "obca_check_quadcopter", "obca_quadcopter_solve_mixed",
            "obca_check_quadcopter_mixed", "obca_plan_parking_warmstart_batch", "obca_plan_quadcopter_warmstart_batch",
            "obca_plan_parking_warmstart_goals", "obca_plan_parking_heuristic_maps", "obca_parking_plan_solve_goals",
-           "obca_quadcopter_plan_solve"]
+           "obca_quadcopter_plan_solve", "obca_parking_plan_solve_both", "obca_quadcopter_plan_solve_both"]
 
 
 class ObcaOpts(C.Structure):
@@ -30,6 +30,18 @@ class ObcaOpts(C.Structure):
                 ("gamma_theta", C.c_double), ("gamma_phi", C.c_double), ("delta", C.c_double), ("s_theta", C.c_double),
                 ("s_phi", C.c_double), ("eta_phi", C.c_double), ("gamma_alpha", C.c_double),
                 ("max_backtrack", C.c_int), ("dc", C.c_double), ("max_kick", C.c_int), ("quad_dual_ws", C.c_int), ("device", C.c_int), ("retry", C.c_int), ("q4", C.c_int)]
+
+
+class ParkingFlowOut(C.Structure):
+    """obca_parking_flow_out: one formulation's output arrays (host pointers) of obca_parking_plan_solve_both."""
+    _fields_ = [(k, C.c_void_p) for k in ("xp", "up", "ts", "lp", "np", "sl", "exitflag", "iters", "kkt_err", "feasible", "strict",
+                                          "solve_seconds")]
+
+
+class QuadcopterFlowOut(C.Structure):
+    """obca_quadcopter_flow_out: one formulation's output arrays of obca_quadcopter_plan_solve_both."""
+    _fields_ = [(k, C.c_void_p) for k in ("xp", "up", "ts", "lp", "slack", "exitflag", "iters", "kkt_err", "feasible", "worst",
+                                          "solve_seconds")]
 
 
 class ObcaError(RuntimeError):

@@ -1059,6 +1059,360 @@ static int quad_check_host(int B, int N, const int* Nb, const double* Tsb, const
   return 0;
 }
 
+// ---- plan -> solve -> check without leaving the device, for one formulation or for both on one plan ------------------------------------
+
+// The first null required field of a flow output set (its name), or null when every required field is there.
+static const char* missing_field(const obca_parking_flow_out& o) {
+  return !o.xp ? "xp" : !o.up ? "up" : !o.ts ? "ts" : !o.lp ? "lp" : !o.np ? "np" : !o.exitflag ? "exitflag" : !o.iters ? "iters"
+       : !o.kkt_err ? "kkt_err" : !o.feasible ? "feasible" : nullptr;
+}
+static const char* missing_field(const obca_quadcopter_flow_out& o) {
+  return !o.xp ? "xp" : !o.up ? "up" : !o.ts ? "ts" : !o.lp ? "lp" : !o.exitflag ? "exitflag" : !o.iters ? "iters"
+       : !o.kkt_err ? "kkt_err" : !o.feasible ? "feasible" : nullptr;
+}
+
+// The null checks of the *_both entries on their two output sets, with the set and the field named in the message.
+template <class Out>
+static int check_both_sets(const Out* dist, const Out* sd) {
+  const Out* sets[2] = {dist, sd};
+  const char* names[2] = {"dist", "sd"};
+  for (int f = 0; f < 2; ++f) {
+    if (!sets[f]) { set_err(std::string("null argument: ") + names[f]); return OBCA_ERR_ARG; }
+    if (const char* m = missing_field(*sets[f])) { set_err(std::string("null argument: ") + names[f] + "." + m); return OBCA_ERR_ARG; }
+  }
+  return 0;
+}
+
+// One formulation of a flow call: its signed_dist and the caller's arrays it writes.
+template <class Out>
+struct FlowSet {
+  int signed_dist;
+  const Out* out;
+};
+
+template <class Out>
+static bool sets_complete(int nf, const FlowSet<Out>* sets) {
+  for (int f = 0; f < nf; ++f)
+    if (missing_field(*sets[f].out)) return false;
+  return true;
+}
+
+// obca_parking_plan_solve_goals (nf = 1) and obca_parking_plan_solve_both (nf = 2, Dist then SD): the stages the formulations share
+// (checks, plan, list, gather) run once, then each formulation is solved, checked and scattered into its own set in turn.
+static int parking_plan_solve(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts, double L,
+                              int sampleN, int max_expansions, int max_nodes, int nOb, const int* vOb, const double* A, const double* b,
+                              const double* ego, const double* XYbounds, int fixTime, const obca_opts* opts, int Ncap, int* N, int* status,
+                              int* expansions, double* plan_seconds, int nf, const FlowSet<obca_parking_flow_out>* sets) {
+  // the planner's checks, then the solver's, with the messages of the entries this one composes; nothing is written before they pass
+  int rc = plan_check_args(B, x0 && xF && ox && oy && vOb && A && b && ego && XYbounds && N && status && sets_complete(nf, sets), n_ob, Ts,
+                           sampleN);
+  if (rc) return rc;
+  if (Ncap < 2) { set_err("Ncap < 2"); return OBCA_ERR_ARG; }
+  ParkProblem P;
+  for (int f = 0; f < nf; ++f)
+    if (const int e_ = fill_problem(P, Ncap, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sets[f].signed_dist)) {
+      set_err(shape_error(e_)); return OBCA_ERR_ARG;
+    }
+  rc = check_park_horizon(Ncap);
+  if (rc) return rc;
+  DevCtx* c;
+  const int dev = opts ? opts->device : 0;
+  rc = get_ctx(dev, &c);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = 0.0;
+  for (int f = 0; f < nf; ++f)
+    if (sets[f].out->solve_seconds) *sets[f].out->solve_seconds = 0.0;
+  if (B == 0) return 0;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  cudaStream_t st = c->st;
+  const int V = P.V, cap = Ncap + 1;      // the planner's stride: stages 0..Ncap, so a longer plan comes back as OBCA_PLAN_CAPACITY
+  const size_t Bs = B;
+  // stage 1: plan into device buffers (N is copied in first: the planner leaves it alone where it finds no path)
+  std::vector<double> x03(3 * Bs), xF3(3 * Bs);
+  for (size_t p = 0; p < Bs; ++p)
+    for (int r = 0; r < 3; ++r) { x03[3 * p + r] = x0[4 * p + r]; xF3[3 * p + r] = xF[4 * p + r]; }
+  PlanDevOut po;
+  double *d0, *dF;
+  int *dlist, *dNb, *dcnt;
+  DevLayout pl;
+  pl.add(po.rx, cap * Bs);
+  pl.add(po.ry, cap * Bs);
+  pl.add(po.ryaw, cap * Bs);
+  pl.add(po.xWS, 4 * cap * Bs);
+  pl.add(po.uWS, 2 * cap * Bs);
+  pl.inout(po.N, N, Bs);
+  pl.out(po.status, status, Bs);
+  pl.out(po.expansions, expansions, Bs);
+  pl.in(d0, x0, 4 * Bs);
+  pl.in(dF, xF, 4 * Bs);
+  pl.add(dlist, Bs);
+  pl.add(dNb, Bs);
+  pl.add(dcnt, 2);
+  DevBuf dplan;
+  CK(alloc_layout(dplan, pl));
+  CK(pl.copy_in(st));
+  float plan_ms = 0.f;
+  rc = plan_warmstart_dev(B, x03.data(), xF3.data(), ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap, dev, st, po, &plan_ms);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = plan_ms * 1e-3;
+  // stage 2: list the poses to solve; their count and longest horizon size the solve (its occupancy follows the layout's horizon)
+  k_flow_list<<<1, FLOW_LIST_THREADS, 0, st>>>(B, Ncap, po.status, po.N, dlist, dNb, dcnt);
+  CK(cudaGetLastError());
+  int cnt[2] = {0, 0};
+  CK(to_host(cnt, dcnt, 2, st));
+  CK(cudaStreamSynchronize(st));
+  const int Bq = cnt[0], M = cnt[1];
+  if (Bq == 0) {
+    CK(pl.copy_out(st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  // stage 3: gather the listed poses into the inputs of the mixed solve at the horizon M, once for every formulation
+  const size_t Qs = Bq, MS = M + 1;
+  obca_flow::Gather g;
+  g.rx = po.rx; g.ry = po.ry; g.ryaw = po.ryaw; g.xWS = po.xWS; g.uWS = po.uWS; g.x0 = d0; g.xF = dF;
+  obca_flow::Outs so;
+  char* dout;
+  DevLayout outs;
+  outs.add(so.xp, 4 * MS * Qs);
+  outs.add(so.up, 2 * (size_t)M * Qs);
+  outs.add(so.ts, MS * Qs);
+  outs.add(so.lp, (size_t)V * MS * Qs);
+  outs.add(so.np, 4 * (size_t)nOb * MS * Qs);
+  outs.add(so.sl, (size_t)nOb * MS * Qs);
+  outs.add(so.kkt_err, Qs);
+  outs.add(so.exitflag, Qs);
+  outs.add(so.iters, Qs);
+  outs.add(so.feasible, Qs);
+  outs.add(so.strict, Qs);
+  DevLayout sl_;
+  sl_.add(g.mrx, MS * Qs);
+  sl_.add(g.mry, MS * Qs);
+  sl_.add(g.mryaw, MS * Qs);
+  sl_.add(g.mxWS, 4 * MS * Qs);
+  sl_.add(g.muWS, 2 * (size_t)M * Qs);
+  sl_.add(g.mx0, 4 * Qs);
+  sl_.add(g.mxF, 4 * Qs);
+  sl_.add(dout, outs.bytes);
+  DevBuf dsolve;
+  CK(alloc_layout(dsolve, sl_));
+  outs.place(dout);
+  const size_t items = Qs * MS;
+  const int threads = 256, blocks = (int)((items + threads - 1) / threads);
+  k_flow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
+  CK(cudaGetLastError());
+  obca_opts o2;
+  if (opts) o2 = *opts; else obca_default_opts(&o2);
+  for (int f = 0; f < nf; ++f) {
+    const int sd = sets[f].signed_dist;
+    const obca_parking_flow_out& u = *sets[f].out;
+    ParkProblem PM;
+    fill_problem(PM, M, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sd);      // the shape passed above, with 2 <= M <= Ncap
+    // stage 4: the mixed solve (DualMultWS inside) into outputs that start as zeros; stage 5: ParkingConstraints on its outputs
+    CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
+    rc = parking_solve_dev(Bq, M, dNb, nOb, vOb, A, b, g.mx0, g.mxF, Ts, L, ego, XYbounds, g.mrx, g.mry, g.mryaw, g.mxWS, g.muWS, nullptr,
+                           nullptr, fixTime, sd, &o2, so.xp, so.up, so.ts, so.lp, so.np, so.sl, so.exitflag, so.iters, so.kkt_err,
+                           u.solve_seconds);
+    if (rc) return rc;
+    rc = check_parking_dev(*c, PM, Bq, dNb, g.mx0, g.mxF, so.xp, so.up, so.lp, so.np, so.ts, so.sl, sd, so.feasible, nullptr, so.strict);
+    if (rc) return rc;
+    // stage 6: the solved poses' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
+    // write keeps the caller's value), then back in one pass; this staging is freed before the next formulation runs
+    obca_flow::Outs d;
+    const size_t NS = Ncap + 1;
+    DevLayout ol;
+    ol.inout(d.xp, u.xp, 4 * NS * Bs);
+    ol.inout(d.up, u.up, 2 * (size_t)Ncap * Bs);
+    ol.inout(d.ts, u.ts, NS * Bs);
+    ol.inout(d.lp, u.lp, (size_t)V * NS * Bs);
+    ol.inout(d.np, u.np, 4 * (size_t)nOb * NS * Bs);
+    ol.inout(d.sl, u.sl, (size_t)nOb * NS * Bs);
+    ol.inout(d.kkt_err, u.kkt_err, Bs);
+    ol.inout(d.exitflag, u.exitflag, Bs);
+    ol.inout(d.iters, u.iters, Bs);
+    ol.inout(d.feasible, u.feasible, Bs);
+    ol.inout(d.strict, u.strict, Bs);
+    DevBuf dcaller;
+    CK(alloc_layout(dcaller, ol));
+    if (!u.sl) d.sl = nullptr;
+    if (!u.strict) d.strict = nullptr;
+    CK(ol.copy_in(st));
+    k_flow_scatter<<<blocks, threads, 0, st>>>(Bq, M, Ncap, V, nOb, dlist, dNb, so, d);
+    CK(cudaGetLastError());
+    CK(ol.copy_out(st));
+    CK(cudaStreamSynchronize(st));
+  }
+  CK(pl.copy_out(st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// obca_quadcopter_plan_solve (nf = 1) and obca_quadcopter_plan_solve_both (nf = 2, Dist then SD): the stages the formulations share
+// (checks, plan, list, warm starts) run once, then each formulation is solved, checked and scattered into its own set in turn.
+static int quad_plan_solve(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz, int n_ob,
+                           const double* lo, const double* hi, double reso, int max_nodes, double Ts, double R, const double* ob,
+                           double timeWS, const obca_opts* opts, int Ncap, int* N, double* Tsb, int* status, int* expansions,
+                           double* plan_seconds, int nf, const FlowSet<obca_quadcopter_flow_out>* sets) {
+  // the planner's checks and set-up (start and goal on its grid, scaled here as mainQuadcopter.jl:114-119 does), then the solve's;
+  // nothing is written before they pass
+  // the planner's stride: stages 0..Ncap, so a longer path comes back as OBCA_PLAN_CAPACITY (an Ncap out of range is refused below)
+  const int cap = Ncap >= 2 && Ncap <= QUAD_NMAX ? Ncap + 1 : 3;
+  std::vector<double> s3(3 * (size_t)(B > 0 ? B : 1)), g3(s3.size());
+  if (x0 && xF)
+    for (int p = 0; p < B; ++p)
+      for (int r = 0; r < 3; ++r) {
+        s3[3 * (size_t)p + r] = OBCA_QUAD_GRID_SCALE * x0[12 * (size_t)p + r];
+        g3[3 * (size_t)p + r] = OBCA_QUAD_GRID_SCALE * xF[12 * (size_t)p + r];
+      }
+  Plan3dSetupPtr S;
+  int rc = plan3d_prepare(S, B, x0 && xF && ob && N && Tsb && status && sets_complete(nf, sets), s3.data(), g3.data(), ox, oy, oz, n_ob,
+                          lo, hi, reso, max_nodes, cap);
+  if (rc) return rc;
+  if (Ncap < 2) { set_err("Ncap < 2"); return OBCA_ERR_ARG; }
+  rc = check_quad_horizon(Ncap);
+  if (rc) return rc;
+  if (!(std::isfinite(Ts) && Ts > 0)) { set_err("Ts must be a finite number > 0"); return OBCA_ERR_ARG; }
+  if (obca_qflow::ts_hundredths(Ts, Ncap) < 1) {
+    set_err("Ts = " + std::to_string(Ts) + " gives a pair planned to N = Ncap = " + std::to_string(Ncap) + " the sampling time 0");
+    return OBCA_ERR_ARG;
+  }
+  QuadProblem P;
+  for (int f = 0; f < nf; ++f)
+    if (fill_quad_problem(P, Ncap, std::nan(""), R, ob, sets[f].signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  DevCtx* c;
+  const int dev = opts ? opts->device : 0;
+  rc = get_ctx(dev, &c);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = 0.0;
+  for (int f = 0; f < nf; ++f)
+    if (sets[f].out->solve_seconds) *sets[f].out->solve_seconds = 0.0;
+  if (B == 0) return 0;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  cudaStream_t st = c->st;
+  const size_t Bs = B;
+  // stage 1: plan into device buffers (N and expansions are copied in first: the planner leaves them alone where it does not write them)
+  Plan3dDevOut po;
+  double *d0, *dF;
+  int *dlist, *dNb, *dcnt;
+  DevLayout pl;
+  pl.add(po.rx, cap * Bs);
+  pl.add(po.ry, cap * Bs);
+  pl.add(po.rz, cap * Bs);
+  pl.inout(po.N, N, Bs);
+  pl.out(po.status, status, Bs);
+  pl.inout(po.expansions, expansions, Bs);
+  pl.in(d0, x0, 12 * Bs);
+  pl.in(dF, xF, 12 * Bs);
+  pl.add(dlist, Bs);
+  pl.add(dNb, Bs);
+  pl.add(dcnt, 2);
+  DevBuf dplan;
+  CK(alloc_layout(dplan, pl));
+  CK(pl.copy_in(st));
+  if (!expansions) po.expansions = nullptr;
+  float plan_ms = 0.f;
+  rc = plan3d_dev(*S, B, dev, st, po, &plan_ms);
+  if (rc) return rc;
+  if (plan_seconds) *plan_seconds = plan_ms * 1e-3;
+  // stage 2: list the pairs to solve; their count and longest horizon size the solve (its occupancy follows the layout's horizon)
+  k_flow_list<<<1, FLOW_LIST_THREADS, 0, st>>>(B, Ncap, po.status, po.N, dlist, dNb, dcnt);
+  CK(cudaGetLastError());
+  int cnt[2] = {0, 0};
+  CK(to_host(cnt, dcnt, 2, st));
+  CK(cudaStreamSynchronize(st));
+  const int Bq = cnt[0], M = cnt[1];
+  if (Bq == 0) {
+    CK(pl.copy_out(st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  // stage 3: the listed pairs' warm starts, x0, xF and sampling times as the inputs of the mixed solve at the horizon M, once for every
+  // formulation.  The check takes the Dist bounds whatever the formulation, as obca_check_quadcopter_mixed does.
+  QuadProblem PC;
+  fill_quad_problem(PC, M, std::nan(""), R, ob, 0);      // the shape passed above, with 2 <= M <= Ncap
+  const size_t Qs = Bq, MS = M + 1;
+  obca_qflow::Gather g;
+  g.rx = po.rx; g.ry = po.ry; g.rz = po.rz; g.x0 = d0; g.xF = dF; g.Ts = Ts;
+  obca_qflow::Outs so;
+  char* dout;
+  DevLayout outs;
+  outs.add(so.xp, 12 * MS * Qs);
+  outs.add(so.up, 4 * (size_t)M * Qs);
+  outs.add(so.ts, MS * Qs);
+  outs.add(so.lp, 30 * MS * Qs);
+  outs.add(so.slack, 5 * MS * Qs);
+  outs.add(so.kkt_err, Qs);
+  outs.add(so.worst, Qs);
+  outs.add(so.exitflag, Qs);
+  outs.add(so.iters, Qs);
+  outs.add(so.feasible, Qs);
+  DevLayout sl_;
+  sl_.add(g.mxWS, 12 * MS * Qs);
+  sl_.add(g.mx0, 12 * Qs);
+  sl_.add(g.mxF, 12 * Qs);
+  sl_.add(g.mTsb, Qs);
+  sl_.add(dout, outs.bytes);
+  DevBuf dsolve;
+  CK(alloc_layout(dsolve, sl_));
+  outs.place(dout);
+  so.Tsb = g.mTsb;
+  const size_t items = Qs * MS;
+  const int threads = 256, blocks = (int)((items + threads - 1) / threads);
+  k_qflow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
+  CK(cudaGetLastError());
+  IpmOpts O = to_ipm(opts);
+  if (!opts) O.max_iter = 3000;                        // as obca_quadcopter_solve_mixed
+  QBatchPtrs bp;
+  bp.x0 = g.mx0; bp.xF = g.mxF; bp.xWS = g.mxWS; bp.Nb = dNb; bp.Tsb = g.mTsb;
+  bp.timeWS = timeWS; bp.xp = so.xp; bp.up = so.up; bp.ts = so.ts; bp.lp = so.lp; bp.slack = so.slack;
+  bp.exitflag = so.exitflag; bp.iters = so.iters; bp.kkt_err = so.kkt_err; bp.B = Bq;
+  for (int f = 0; f < nf; ++f) {
+    const int sd = sets[f].signed_dist;
+    const obca_quadcopter_flow_out& u = *sets[f].out;
+    QuadProblem PM;
+    fill_quad_problem(PM, M, std::nan(""), R, ob, sd);
+    // stage 4: the mixed solve into outputs that start as zeros; stage 5: constrSatisfaction on its outputs
+    CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
+    rc = quad_solve_dev(*c, PM, O, bp);
+    if (rc) return rc;
+    CK(to_host(c->prof_host, c->prof, 8, st));
+    rc = quad_check_dev(*c, PC, Bq, dNb, g.mTsb, g.mx0, g.mxF, so.xp, so.up, so.ts, so.lp, so.feasible, so.worst);
+    if (rc) return rc;
+    // stage 6: the solved pairs' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
+    // write keeps the caller's value), then back in one pass; this staging is freed before the next formulation runs
+    double* slack_out = sd ? u.slack : nullptr;      // the Dist formulation has no slacks
+    obca_qflow::Outs d;
+    const size_t NS = Ncap + 1;
+    DevLayout ol;
+    ol.inout(d.xp, u.xp, 12 * NS * Bs);
+    ol.inout(d.up, u.up, 4 * (size_t)Ncap * Bs);
+    ol.inout(d.ts, u.ts, NS * Bs);
+    ol.inout(d.lp, u.lp, 30 * NS * Bs);
+    ol.inout(d.slack, slack_out, slack_out ? 5 * NS * Bs : 0);
+    ol.inout(d.kkt_err, u.kkt_err, Bs);
+    ol.inout(d.Tsb, Tsb, Bs);
+    ol.inout(d.worst, u.worst, u.worst ? Bs : 0);
+    ol.inout(d.exitflag, u.exitflag, Bs);
+    ol.inout(d.iters, u.iters, Bs);
+    ol.inout(d.feasible, u.feasible, Bs);
+    DevBuf dcaller;
+    CK(alloc_layout(dcaller, ol));
+    if (!slack_out) d.slack = nullptr;
+    if (!u.worst) d.worst = nullptr;
+    CK(ol.copy_in(st));
+    k_qflow_scatter<<<blocks, threads, 0, st>>>(Bq, M, Ncap, dlist, dNb, so, d);
+    CK(cudaGetLastError());
+    CK(ol.copy_out(st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+    if (u.solve_seconds) *u.solve_seconds = ms * 1e-3;
+  }
+  CK(pl.copy_out(st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
 extern "C" {
 
 #ifdef OBCA_QPROF   // development builds only: cycles of the quadcopter sweep's phases, summed over CTAs; resets the counters
@@ -1213,140 +1567,22 @@ int obca_parking_plan_solve_goals(int B, const double* x0, const double* xF, con
                                   const obca_opts* opts, int Ncap, double* xp, double* up, double* ts, double* lp, double* np, double* sl,
                                   int* N, int* status, int* expansions, int* exitflag, int* iters, double* kkt_err, int* feasible,
                                   int* strict, double* plan_seconds, double* solve_seconds) {
-  // the planner's checks, then the solver's, with the messages of the entries this one composes; nothing is written before they pass
-  int rc = plan_check_args(B, x0 && xF && ox && oy && vOb && A && b && ego && XYbounds && xp && up && ts && lp && np && N && status &&
-                                  exitflag && iters && kkt_err && feasible, n_ob, Ts, sampleN);
+  const obca_parking_flow_out out = {xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, feasible, strict, solve_seconds};
+  const FlowSet<obca_parking_flow_out> set = {signed_dist, &out};
+  return parking_plan_solve(B, x0, xF, ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, nOb, vOb, A, b, ego, XYbounds, fixTime,
+                            opts, Ncap, N, status, expansions, plan_seconds, 1, &set);
+}
+
+int obca_parking_plan_solve_both(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts,
+                                 double L, int sampleN, int max_expansions, int max_nodes, int nOb, const int* vOb, const double* A,
+                                 const double* b, const double* ego, const double* XYbounds, int fixTime, const obca_opts* opts,
+                                 int Ncap, int* N, int* status, int* expansions, double* plan_seconds, const obca_parking_flow_out* dist,
+                                 const obca_parking_flow_out* sd) {
+  const int rc = check_both_sets(dist, sd);
   if (rc) return rc;
-  if (Ncap < 2) { set_err("Ncap < 2"); return OBCA_ERR_ARG; }
-  ParkProblem P;
-  if (const int e_ = fill_problem(P, Ncap, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
-  rc = check_park_horizon(Ncap);
-  if (rc) return rc;
-  DevCtx* c;
-  const int dev = opts ? opts->device : 0;
-  rc = get_ctx(dev, &c);
-  if (rc) return rc;
-  if (plan_seconds) *plan_seconds = 0.0;
-  if (solve_seconds) *solve_seconds = 0.0;
-  if (B == 0) return 0;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  cudaStream_t st = c->st;
-  const int V = P.V, cap = Ncap + 1;      // the planner's stride: stages 0..Ncap, so a longer plan comes back as OBCA_PLAN_CAPACITY
-  const size_t Bs = B;
-  // stage 1: plan into device buffers (N is copied in first: the planner leaves it alone where it finds no path)
-  std::vector<double> x03(3 * Bs), xF3(3 * Bs);
-  for (size_t p = 0; p < Bs; ++p)
-    for (int r = 0; r < 3; ++r) { x03[3 * p + r] = x0[4 * p + r]; xF3[3 * p + r] = xF[4 * p + r]; }
-  PlanDevOut po;
-  double *d0, *dF;
-  int *dlist, *dNb, *dcnt;
-  DevLayout pl;
-  pl.add(po.rx, cap * Bs);
-  pl.add(po.ry, cap * Bs);
-  pl.add(po.ryaw, cap * Bs);
-  pl.add(po.xWS, 4 * cap * Bs);
-  pl.add(po.uWS, 2 * cap * Bs);
-  pl.inout(po.N, N, Bs);
-  pl.out(po.status, status, Bs);
-  pl.out(po.expansions, expansions, Bs);
-  pl.in(d0, x0, 4 * Bs);
-  pl.in(dF, xF, 4 * Bs);
-  pl.add(dlist, Bs);
-  pl.add(dNb, Bs);
-  pl.add(dcnt, 2);
-  DevBuf dplan;
-  CK(alloc_layout(dplan, pl));
-  CK(pl.copy_in(st));
-  float plan_ms = 0.f;
-  rc = plan_warmstart_dev(B, x03.data(), xF3.data(), ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, cap, dev, st, po, &plan_ms);
-  if (rc) return rc;
-  if (plan_seconds) *plan_seconds = plan_ms * 1e-3;
-  // stage 2: list the poses to solve; their count and longest horizon size the solve (its occupancy follows the layout's horizon)
-  k_flow_list<<<1, FLOW_LIST_THREADS, 0, st>>>(B, Ncap, po.status, po.N, dlist, dNb, dcnt);
-  CK(cudaGetLastError());
-  int cnt[2] = {0, 0};
-  CK(to_host(cnt, dcnt, 2, st));
-  CK(cudaStreamSynchronize(st));
-  const int Bq = cnt[0], M = cnt[1];
-  if (Bq == 0) {
-    CK(pl.copy_out(st));
-    CK(cudaStreamSynchronize(st));
-    return 0;
-  }
-  // stage 3: gather the listed poses into the inputs of the mixed solve at the horizon M; its outputs start as zeros
-  ParkProblem PM;
-  fill_problem(PM, M, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist);      // the shape passed above, with 2 <= M <= Ncap
-  const size_t Qs = Bq, MS = M + 1;
-  obca_flow::Gather g;
-  g.rx = po.rx; g.ry = po.ry; g.ryaw = po.ryaw; g.xWS = po.xWS; g.uWS = po.uWS; g.x0 = d0; g.xF = dF;
-  obca_flow::Outs so;
-  char* dout;
-  DevLayout outs;
-  outs.add(so.xp, 4 * MS * Qs);
-  outs.add(so.up, 2 * (size_t)M * Qs);
-  outs.add(so.ts, MS * Qs);
-  outs.add(so.lp, (size_t)V * MS * Qs);
-  outs.add(so.np, 4 * (size_t)nOb * MS * Qs);
-  outs.add(so.sl, (size_t)nOb * MS * Qs);
-  outs.add(so.kkt_err, Qs);
-  outs.add(so.exitflag, Qs);
-  outs.add(so.iters, Qs);
-  outs.add(so.feasible, Qs);
-  outs.add(so.strict, Qs);
-  DevLayout sl_;
-  sl_.add(g.mrx, MS * Qs);
-  sl_.add(g.mry, MS * Qs);
-  sl_.add(g.mryaw, MS * Qs);
-  sl_.add(g.mxWS, 4 * MS * Qs);
-  sl_.add(g.muWS, 2 * (size_t)M * Qs);
-  sl_.add(g.mx0, 4 * Qs);
-  sl_.add(g.mxF, 4 * Qs);
-  sl_.add(dout, outs.bytes);
-  DevBuf dsolve;
-  CK(alloc_layout(dsolve, sl_));
-  outs.place(dout);
-  CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
-  const size_t items = Qs * MS;
-  const int threads = 256, blocks = (int)((items + threads - 1) / threads);
-  k_flow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
-  CK(cudaGetLastError());
-  // stage 4: the mixed solve (DualMultWS inside); stage 5: ParkingConstraints on its outputs
-  obca_opts o2;
-  if (opts) o2 = *opts; else obca_default_opts(&o2);
-  rc = parking_solve_dev(Bq, M, dNb, nOb, vOb, A, b, g.mx0, g.mxF, Ts, L, ego, XYbounds, g.mrx, g.mry, g.mryaw, g.mxWS, g.muWS, nullptr,
-                         nullptr, fixTime, signed_dist, &o2, so.xp, so.up, so.ts, so.lp, so.np, so.sl, so.exitflag, so.iters, so.kkt_err,
-                         solve_seconds);
-  if (rc) return rc;
-  rc = check_parking_dev(*c, PM, Bq, dNb, g.mx0, g.mxF, so.xp, so.up, so.lp, so.np, so.ts, so.sl, signed_dist, so.feasible, nullptr,
-                         so.strict);
-  if (rc) return rc;
-  // stage 6: the solved poses' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
-  // write keeps the caller's value), then everything back in one pass
-  obca_flow::Outs d;
-  const size_t NS = Ncap + 1;
-  DevLayout ol;
-  ol.inout(d.xp, xp, 4 * NS * Bs);
-  ol.inout(d.up, up, 2 * (size_t)Ncap * Bs);
-  ol.inout(d.ts, ts, NS * Bs);
-  ol.inout(d.lp, lp, (size_t)V * NS * Bs);
-  ol.inout(d.np, np, 4 * (size_t)nOb * NS * Bs);
-  ol.inout(d.sl, sl, (size_t)nOb * NS * Bs);
-  ol.inout(d.kkt_err, kkt_err, Bs);
-  ol.inout(d.exitflag, exitflag, Bs);
-  ol.inout(d.iters, iters, Bs);
-  ol.inout(d.feasible, feasible, Bs);
-  ol.inout(d.strict, strict, Bs);
-  DevBuf dcaller;
-  CK(alloc_layout(dcaller, ol));
-  if (!sl) d.sl = nullptr;
-  if (!strict) d.strict = nullptr;
-  CK(ol.copy_in(st));
-  k_flow_scatter<<<blocks, threads, 0, st>>>(Bq, M, Ncap, V, nOb, dlist, dNb, so, d);
-  CK(cudaGetLastError());
-  CK(ol.copy_out(st));
-  CK(pl.copy_out(st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
+  const FlowSet<obca_parking_flow_out> sets[2] = {{0, dist}, {1, sd}};      // main.jl:258, then :269
+  return parking_plan_solve(B, x0, xF, ox, oy, n_ob, Ts, L, sampleN, max_expansions, max_nodes, nOb, vOb, A, b, ego, XYbounds, fixTime,
+                            opts, Ncap, N, status, expansions, plan_seconds, 2, sets);
 }
 
 int obca_quadcopter_plan_solve(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz, int n_ob,
@@ -1354,156 +1590,22 @@ int obca_quadcopter_plan_solve(int B, const double* x0, const double* xF, const 
                                double timeWS, int signed_dist, const obca_opts* opts, int Ncap, double* xp, double* up, double* ts,
                                double* lp, double* slack, int* N, double* Tsb, int* status, int* expansions, int* exitflag, int* iters,
                                double* kkt_err, int* feasible, double* worst, double* plan_seconds, double* solve_seconds) {
-  // the planner's checks and set-up (start and goal on its grid, scaled here as mainQuadcopter.jl:114-119 does), then the solve's;
-  // nothing is written before they pass
-  // the planner's stride: stages 0..Ncap, so a longer path comes back as OBCA_PLAN_CAPACITY (an Ncap out of range is refused below)
-  const int cap = Ncap >= 2 && Ncap <= QUAD_NMAX ? Ncap + 1 : 3;
-  std::vector<double> s3(3 * (size_t)(B > 0 ? B : 1)), g3(s3.size());
-  if (x0 && xF)
-    for (int p = 0; p < B; ++p)
-      for (int r = 0; r < 3; ++r) {
-        s3[3 * (size_t)p + r] = OBCA_QUAD_GRID_SCALE * x0[12 * (size_t)p + r];
-        g3[3 * (size_t)p + r] = OBCA_QUAD_GRID_SCALE * xF[12 * (size_t)p + r];
-      }
-  Plan3dSetupPtr S;
-  int rc = plan3d_prepare(S, B, x0 && xF && ob && xp && up && ts && lp && N && Tsb && status && exitflag && iters && kkt_err && feasible,
-                          s3.data(), g3.data(), ox, oy, oz, n_ob, lo, hi, reso, max_nodes, cap);
+  const obca_quadcopter_flow_out out = {xp, up, ts, lp, slack, exitflag, iters, kkt_err, feasible, worst, solve_seconds};
+  const FlowSet<obca_quadcopter_flow_out> set = {signed_dist, &out};
+  return quad_plan_solve(B, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, max_nodes, Ts, R, ob, timeWS, opts, Ncap, N, Tsb, status, expansions,
+                         plan_seconds, 1, &set);
+}
+
+int obca_quadcopter_plan_solve_both(int B, const double* x0, const double* xF, const double* ox, const double* oy, const double* oz,
+                                    int n_ob, const double* lo, const double* hi, double reso, int max_nodes, double Ts, double R,
+                                    const double* ob, double timeWS, const obca_opts* opts, int Ncap, int* N, double* Tsb, int* status,
+                                    int* expansions, double* plan_seconds, const obca_quadcopter_flow_out* dist,
+                                    const obca_quadcopter_flow_out* sd) {
+  const int rc = check_both_sets(dist, sd);
   if (rc) return rc;
-  if (Ncap < 2) { set_err("Ncap < 2"); return OBCA_ERR_ARG; }
-  rc = check_quad_horizon(Ncap);
-  if (rc) return rc;
-  if (!(std::isfinite(Ts) && Ts > 0)) { set_err("Ts must be a finite number > 0"); return OBCA_ERR_ARG; }
-  if (obca_qflow::ts_hundredths(Ts, Ncap) < 1) {
-    set_err("Ts = " + std::to_string(Ts) + " gives a pair planned to N = Ncap = " + std::to_string(Ncap) + " the sampling time 0");
-    return OBCA_ERR_ARG;
-  }
-  QuadProblem P;
-  if (fill_quad_problem(P, Ncap, std::nan(""), R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
-  DevCtx* c;
-  const int dev = opts ? opts->device : 0;
-  rc = get_ctx(dev, &c);
-  if (rc) return rc;
-  if (plan_seconds) *plan_seconds = 0.0;
-  if (solve_seconds) *solve_seconds = 0.0;
-  if (B == 0) return 0;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  cudaStream_t st = c->st;
-  const size_t Bs = B;
-  // stage 1: plan into device buffers (N and expansions are copied in first: the planner leaves them alone where it does not write them)
-  Plan3dDevOut po;
-  double *d0, *dF;
-  int *dlist, *dNb, *dcnt;
-  DevLayout pl;
-  pl.add(po.rx, cap * Bs);
-  pl.add(po.ry, cap * Bs);
-  pl.add(po.rz, cap * Bs);
-  pl.inout(po.N, N, Bs);
-  pl.out(po.status, status, Bs);
-  pl.inout(po.expansions, expansions, Bs);
-  pl.in(d0, x0, 12 * Bs);
-  pl.in(dF, xF, 12 * Bs);
-  pl.add(dlist, Bs);
-  pl.add(dNb, Bs);
-  pl.add(dcnt, 2);
-  DevBuf dplan;
-  CK(alloc_layout(dplan, pl));
-  CK(pl.copy_in(st));
-  if (!expansions) po.expansions = nullptr;
-  float plan_ms = 0.f;
-  rc = plan3d_dev(*S, B, dev, st, po, &plan_ms);
-  if (rc) return rc;
-  if (plan_seconds) *plan_seconds = plan_ms * 1e-3;
-  // stage 2: list the pairs to solve; their count and longest horizon size the solve (its occupancy follows the layout's horizon)
-  k_flow_list<<<1, FLOW_LIST_THREADS, 0, st>>>(B, Ncap, po.status, po.N, dlist, dNb, dcnt);
-  CK(cudaGetLastError());
-  int cnt[2] = {0, 0};
-  CK(to_host(cnt, dcnt, 2, st));
-  CK(cudaStreamSynchronize(st));
-  const int Bq = cnt[0], M = cnt[1];
-  if (Bq == 0) {
-    CK(pl.copy_out(st));
-    CK(cudaStreamSynchronize(st));
-    return 0;
-  }
-  // stage 3: the listed pairs' warm starts, x0, xF and sampling times as the inputs of the mixed solve at the horizon M; its outputs
-  // start as zeros.  The check takes the Dist bounds whatever the formulation, as obca_check_quadcopter_mixed does.
-  QuadProblem PM, PC;
-  fill_quad_problem(PM, M, std::nan(""), R, ob, signed_dist);      // the shape passed above, with 2 <= M <= Ncap
-  fill_quad_problem(PC, M, std::nan(""), R, ob, 0);
-  const size_t Qs = Bq, MS = M + 1;
-  obca_qflow::Gather g;
-  g.rx = po.rx; g.ry = po.ry; g.rz = po.rz; g.x0 = d0; g.xF = dF; g.Ts = Ts;
-  obca_qflow::Outs so;
-  char* dout;
-  DevLayout outs;
-  outs.add(so.xp, 12 * MS * Qs);
-  outs.add(so.up, 4 * (size_t)M * Qs);
-  outs.add(so.ts, MS * Qs);
-  outs.add(so.lp, 30 * MS * Qs);
-  outs.add(so.slack, 5 * MS * Qs);
-  outs.add(so.kkt_err, Qs);
-  outs.add(so.worst, Qs);
-  outs.add(so.exitflag, Qs);
-  outs.add(so.iters, Qs);
-  outs.add(so.feasible, Qs);
-  DevLayout sl_;
-  sl_.add(g.mxWS, 12 * MS * Qs);
-  sl_.add(g.mx0, 12 * Qs);
-  sl_.add(g.mxF, 12 * Qs);
-  sl_.add(g.mTsb, Qs);
-  sl_.add(dout, outs.bytes);
-  DevBuf dsolve;
-  CK(alloc_layout(dsolve, sl_));
-  outs.place(dout);
-  so.Tsb = g.mTsb;
-  CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
-  const size_t items = Qs * MS;
-  const int threads = 256, blocks = (int)((items + threads - 1) / threads);
-  k_qflow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
-  CK(cudaGetLastError());
-  // stage 4: the mixed solve; stage 5: constrSatisfaction on its outputs
-  IpmOpts O = to_ipm(opts);
-  if (!opts) O.max_iter = 3000;                        // as obca_quadcopter_solve_mixed
-  QBatchPtrs bp;
-  bp.x0 = g.mx0; bp.xF = g.mxF; bp.xWS = g.mxWS; bp.Nb = dNb; bp.Tsb = g.mTsb;
-  bp.timeWS = timeWS; bp.xp = so.xp; bp.up = so.up; bp.ts = so.ts; bp.lp = so.lp; bp.slack = so.slack;
-  bp.exitflag = so.exitflag; bp.iters = so.iters; bp.kkt_err = so.kkt_err; bp.B = Bq;
-  rc = quad_solve_dev(*c, PM, O, bp);
-  if (rc) return rc;
-  CK(to_host(c->prof_host, c->prof, 8, st));
-  rc = quad_check_dev(*c, PC, Bq, dNb, g.mTsb, g.mx0, g.mxF, so.xp, so.up, so.ts, so.lp, so.feasible, so.worst);
-  if (rc) return rc;
-  // stage 6: the solved pairs' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
-  // write keeps the caller's value), then everything back in one pass
-  double* slack_out = signed_dist ? slack : nullptr;      // the Dist formulation has no slacks
-  obca_qflow::Outs d;
-  const size_t NS = Ncap + 1;
-  DevLayout ol;
-  ol.inout(d.xp, xp, 12 * NS * Bs);
-  ol.inout(d.up, up, 4 * (size_t)Ncap * Bs);
-  ol.inout(d.ts, ts, NS * Bs);
-  ol.inout(d.lp, lp, 30 * NS * Bs);
-  ol.inout(d.slack, slack_out, slack_out ? 5 * NS * Bs : 0);
-  ol.inout(d.kkt_err, kkt_err, Bs);
-  ol.inout(d.Tsb, Tsb, Bs);
-  ol.inout(d.worst, worst, worst ? Bs : 0);
-  ol.inout(d.exitflag, exitflag, Bs);
-  ol.inout(d.iters, iters, Bs);
-  ol.inout(d.feasible, feasible, Bs);
-  DevBuf dcaller;
-  CK(alloc_layout(dcaller, ol));
-  if (!slack_out) d.slack = nullptr;
-  if (!worst) d.worst = nullptr;
-  CK(ol.copy_in(st));
-  k_qflow_scatter<<<blocks, threads, 0, st>>>(Bq, M, Ncap, dlist, dNb, so, d);
-  CK(cudaGetLastError());
-  CK(ol.copy_out(st));
-  CK(pl.copy_out(st));
-  CK(cudaStreamSynchronize(st));
-  float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-  if (solve_seconds) *solve_seconds = ms * 1e-3;
-  return 0;
+  const FlowSet<obca_quadcopter_flow_out> sets[2] = {{0, dist}, {1, sd}};      // mainQuadcopter.jl:145-147, then :152-154
+  return quad_plan_solve(B, x0, xF, ox, oy, oz, n_ob, lo, hi, reso, max_nodes, Ts, R, ob, timeWS, opts, Ncap, N, Tsb, status, expansions,
+                         plan_seconds, 2, sets);
 }
 
 int obca_last_profile(int device, unsigned long long* out8) {

@@ -4,7 +4,9 @@
   - obca_plan_quadcopter_warmstart_batch, the 3-D A* of the quadcopter flow: B start / goal pairs in one call (plan_quadcopter_raw,
     plan_quadcopter_batch);
   - obca_parking_plan_solve_goals and obca_quadcopter_plan_solve, which plan, solve and check a batch in one call without leaving the
-    device (plan_solve_goals, plan_solve_quadcopter and their *_raw twins).
+    device (plan_solve_goals, plan_solve_quadcopter and their *_raw twins);
+  - obca_parking_plan_solve_both and obca_quadcopter_plan_solve_both, the same with one plan solved and checked with both formulations
+    (plan_solve_goals_both, plan_solve_quadcopter_both and their *_raw twins).
 Without a CUDA device the calls raise.  A search that outgrows the device's scratch comes back as POOL_FULL in `status` (the *_raw
 functions); the *_batch functions plan those problems with the host planner, which makes the same decisions."""
 from __future__ import annotations
@@ -160,6 +162,29 @@ def plan_batch(x0s, xF, scenario="backwards", Ts=None, L=2.7, sampleN=3, cap=512
     return out
 
 
+_PK_SET = ("xp", "up", "ts", "lp", "np", "sl", "exitflag", "iters", "kkt_err", "feasible", "strict")
+_QC_SET = ("xp", "up", "ts", "lp", "slack", "exitflag", "iters", "kkt_err", "feasible", "worst")
+
+
+def _parking_flow_inputs(x0s, xFs, ox, oy, nOb, vOb, A, b):
+    """The flow entries' parking inputs as contiguous arrays: x0s (B, 4), xFs (B, 4), ox, oy and the obstacles (vOb, V, A, b)."""
+    from .._lib import f64
+    from ..parking import _shared
+    x0s = f64(np.asarray(x0s, float).reshape(-1, 4)); B = x0s.shape[0]
+    xFs = f64(np.broadcast_to(np.asarray(xFs, float).reshape(-1, 4), (B, 4)))
+    vOb, V, A, b = _shared(nOb, vOb, A, b)
+    return x0s, xFs, f64(ox), f64(oy), vOb, V, A, b
+
+
+def _parking_set(B, Ncap, V, nOb):
+    """One formulation's output arrays of the parking flow for B poses, NaN-filled (the integers -1)."""
+    NS = Ncap + 1
+    nan = lambda *s: np.full(s, np.nan)
+    i32 = lambda: np.full(B, -1, np.int32)
+    return dict(xp=nan(B, NS, 4), up=nan(B, Ncap, 2), ts=nan(B, NS), lp=nan(B, NS, V), np=nan(B, NS, 4 * nOb), sl=nan(B, NS, nOb),
+                exitflag=i32(), iters=i32(), kkt_err=nan(B), feasible=i32(), strict=i32())
+
+
 def plan_solve_goals_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=2.7, sampleN=3, Ncap=319, fixTime=0, signed_dist=1,
                          max_nodes=0, max_expansions=0, opts=None, host_fallback=False):
     """obca_parking_plan_solve_goals's outputs as arrays: plan every start pose x0s (B, 4: x, y, yaw, v) towards its goal xFs ((B, 4), or
@@ -171,15 +196,10 @@ def plan_solve_goals_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=
     the same decisions), and those that plan to 2 <= N <= Ncap are solved and checked by parking_solve_mixed / check_parking_mixed in one
     more call each (their solve time is not in `time`), as plan_goals_raw(host_fallback=True) does for the planner alone."""
     from .._lib import f64
-    from ..parking import _shared
-    x0s = f64(np.asarray(x0s, float).reshape(-1, 4)); B = x0s.shape[0]
-    xFs = f64(np.broadcast_to(np.asarray(xFs, float).reshape(-1, 4), (B, 4)))
-    vOb, V, A, b = _shared(nOb, vOb, A, b)
-    ox = f64(ox); oy = f64(oy); NS = Ncap + 1
-    nan = lambda *s: np.full(s, np.nan)
+    x0s, xFs, ox, oy, vOb, V, A, b = _parking_flow_inputs(x0s, xFs, ox, oy, nOb, vOb, A, b)
+    B = x0s.shape[0]
     i32 = lambda: np.full(B, -1, np.int32)
-    o = dict(xp=nan(B, NS, 4), up=nan(B, Ncap, 2), ts=nan(B, NS), lp=nan(B, NS, V), np=nan(B, NS, 4 * nOb), sl=nan(B, NS, nOb), N=i32(),
-             status=i32(), expansions=i32(), exitflag=i32(), iters=i32(), kkt_err=nan(B), feasible=i32(), strict=i32())
+    o = dict(_parking_set(B, Ncap, V, nOb), N=i32(), status=i32(), expansions=i32())
     secs = np.zeros(2)
     opts = opts if opts is not None else _lib.default_opts()
     p = _lib.ptr
@@ -196,19 +216,60 @@ def plan_solve_goals_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=
     o["plan_seconds"], o["time"] = float(secs[0]), float(secs[1])
     full = np.flatnonzero(o["status"] == POOL_FULL)
     if host_fallback and full.size:
-        _solve_on_host_plans(o, full, x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, fixTime, signed_dist, opts)
+        h, ok = _plan_on_host(o, full, x0s, xFs, ox, oy, Ts, L, sampleN, Ncap)
+        _solve_on_host_plans(o, full, h, ok, x0s, xFs, Ts, nOb, vOb, A, b, ego, XYbounds, L, fixTime, signed_dist, opts)
     return o
 
 
-def _solve_on_host_plans(o, full, x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, fixTime, signed_dist, opts):
-    """Plan the poses `full` with the host twin, then solve and check the ones it plans to 2 <= N <= Ncap; their entries of o (the layout
-    of plan_solve_goals_raw) get the results, the others the host twin's status (OBCA_PLAN_CAPACITY for a horizon outside [2, Ncap])."""
-    from .. import parking
+def plan_solve_goals_both_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=2.7, sampleN=3, Ncap=319, fixTime=0, max_nodes=0,
+                              max_expansions=0, opts=None, host_fallback=False):
+    """obca_parking_plan_solve_both's outputs as arrays: plan_solve_goals_raw's arguments without signed_dist; every pose is planned once,
+    then solved and checked with the Distance and then the Signed Distance formulation.  Returns the shared N, status, expansions and
+    plan_seconds, and under "dist" and "sd" the per-formulation keys of plan_solve_goals_raw (xp, up, ts, lp, np, sl, exitflag, iters,
+    kkt_err, feasible, strict, time), each what plan_solve_goals_raw with signed_dist = 0 / 1 returns for the same inputs.
+    host_fallback: the POOL_FULL poses are planned once by the host twin, then solved and checked with both formulations."""
+    from .._lib import f64
+    x0s, xFs, ox, oy, vOb, V, A, b = _parking_flow_inputs(x0s, xFs, ox, oy, nOb, vOb, A, b)
+    B = x0s.shape[0]
+    i32 = lambda: np.full(B, -1, np.int32)
+    o = dict(N=i32(), status=i32(), expansions=i32(), dist=_parking_set(B, Ncap, V, nOb), sd=_parking_set(B, Ncap, V, nOb))
+    secs = np.zeros(3)
+    sets = [_lib.ParkingFlowOut(*[o[f][k].ctypes.data for k in _PK_SET], secs[j + 1:j + 2].ctypes.data) for j, f in enumerate(("dist", "sd"))]
+    opts = opts if opts is not None else _lib.default_opts()
+    p = _lib.ptr
+    fn = _lib.lib().obca_parking_plan_solve_both
+    fn.restype = C.c_int
+    fn.argtypes = ([C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 5
+                   + [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 6)
+    rc = fn(B, p(x0s), p(xFs), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(nOb),
+            p(vOb), p(A), p(b), p(f64(np.asarray(ego).ravel())), p(f64(np.asarray(XYbounds).ravel())), int(fixTime),
+            C.cast(C.byref(opts), C.c_void_p), int(Ncap), p(o["N"]), p(o["status"]), p(o["expansions"]), p(secs[:1]),
+            *[C.cast(C.byref(s), C.c_void_p) for s in sets])
+    _lib.check(rc)
+    o["plan_seconds"] = float(secs[0])
+    o["dist"]["time"], o["sd"]["time"] = float(secs[1]), float(secs[2])
+    full = np.flatnonzero(o["status"] == POOL_FULL)
+    if host_fallback and full.size:
+        h, ok = _plan_on_host(o, full, x0s, xFs, ox, oy, Ts, L, sampleN, Ncap)
+        for sd, f in ((0, "dist"), (1, "sd")):
+            _solve_on_host_plans(o[f], full, h, ok, x0s, xFs, Ts, nOb, vOb, A, b, ego, XYbounds, L, fixTime, sd, opts)
+    return o
+
+
+def _plan_on_host(o, full, x0s, xFs, ox, oy, Ts, L, sampleN, Ncap):
+    """Plan the poses `full` with the host twin; their status, N and expansions in o get its outputs (OBCA_PLAN_CAPACITY for a horizon
+    outside [2, Ncap]).  Returns the host twin's outputs and the positions in `full` of the poses to solve."""
     h = native.plan_cloud_raw(x0s[full], xFs[full], ox, oy, Ts, L, sampleN)
     st = h["status"].copy()
     st[(st == 0) & ((h["N"] < 2) | (h["N"] > Ncap))] = 2
     o["status"][full] = st; o["N"][full] = h["N"]; o["expansions"][full] = h["expansions"]
-    ok = np.flatnonzero(st == 0)
+    return h, np.flatnonzero(st == 0)
+
+
+def _solve_on_host_plans(o, full, h, ok, x0s, xFs, Ts, nOb, vOb, A, b, ego, XYbounds, L, fixTime, signed_dist, opts):
+    """Solve and check the poses full[ok] on the host twin's plans h (_plan_on_host) with one formulation; their entries of o (one
+    formulation's arrays in the layout of plan_solve_goals_raw) get the results."""
+    from .. import parking
     if ok.size == 0:
         return
     Ns = h["N"][ok]
@@ -228,6 +289,17 @@ def _solve_on_host_plans(o, full, x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYb
         o[k][full[ok]] = v
 
 
+def _parking_lists(o, ok, N):
+    """One formulation's arrays of plan_solve_goals_raw as per-pose lists in the Julia shapes (None where ok[i] is False)."""
+    cut = lambda a, ext: [a[i, :n + ext].T.copy() if ok[i] else None for i, n in enumerate(N)]
+    out = dict(xp=cut(o["xp"], 1), up=cut(o["up"], 0), ts=[o["ts"][i, :n + 1].copy() if ok[i] else None for i, n in enumerate(N)],
+               lp=cut(o["lp"], 1), np=cut(o["np"], 1), sl=cut(o["sl"], 1))
+    for k in ("exitflag", "iters", "feasible", "strict"):
+        out[k] = np.where(ok, o[k], 0).astype(np.int32)
+    out.update(kkt_err=np.where(ok, o["kkt_err"], np.nan), time=o["time"])
+    return out
+
+
 def plan_solve_goals(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=2.7, sampleN=3, Ncap=319, fixTime=0, signed_dist=1,
                      max_nodes=0, max_expansions=0, opts=None, host_fallback=False):
     """main.jl:215-269 for a batch in one call (obca_parking_plan_solve_goals): plan, solve and check every start pose x0s (B, 4) towards
@@ -238,15 +310,22 @@ def plan_solve_goals(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=2.7,
     host_fallback: plan, solve and check the POOL_FULL poses on the host twin's plans (see plan_solve_goals_raw)."""
     o = plan_solve_goals_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, fixTime, signed_dist, max_nodes,
                              max_expansions, opts, host_fallback)
-    ok = o["status"] == 0
-    cut = lambda a, ext: [a[i, :n + ext].T.copy() if ok[i] else None for i, n in enumerate(o["N"])]
-    out = dict(xp=cut(o["xp"], 1), up=cut(o["up"], 0), ts=[o["ts"][i, :n + 1].copy() if ok[i] else None for i, n in enumerate(o["N"])],
-               lp=cut(o["lp"], 1), np=cut(o["np"], 1), sl=cut(o["sl"], 1))
-    for k in ("exitflag", "iters", "feasible", "strict"):
-        out[k] = np.where(ok, o[k], 0).astype(np.int32)
-    out.update(kkt_err=np.where(ok, o["kkt_err"], np.nan), N=o["N"].copy(), status=o["status"].copy(), expansions=o["expansions"].copy(),
-               time=o["time"], plan_seconds=o["plan_seconds"])
+    out = _parking_lists(o, o["status"] == 0, o["N"])
+    out.update(N=o["N"].copy(), status=o["status"].copy(), expansions=o["expansions"].copy(), plan_seconds=o["plan_seconds"])
     return out
+
+
+def plan_solve_goals_both(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=2.7, sampleN=3, Ncap=319, fixTime=0, max_nodes=0,
+                          max_expansions=0, opts=None, host_fallback=False):
+    """main.jl:215-269 as the reference runs it, for a batch in one call (obca_parking_plan_solve_both): every pose planned once, then
+    solved and checked with ParkingDist and ParkingSignedDist.  Returns the shared N, status, expansions and plan_seconds, and under
+    "dist" and "sd" the per-formulation keys of plan_solve_goals (per-pose lists in the Julia shapes, None where the pose was not solved,
+    and exitflag, iters, kkt_err, feasible, strict, time)."""
+    o = plan_solve_goals_both_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, fixTime, max_nodes, max_expansions,
+                                  opts, host_fallback)
+    ok = o["status"] == 0
+    return dict(N=o["N"].copy(), status=o["status"].copy(), expansions=o["expansions"].copy(), plan_seconds=o["plan_seconds"],
+                dist=_parking_lists(o["dist"], ok, o["N"]), sd=_parking_lists(o["sd"], ok, o["N"]))
 
 
 def plan_solve_batch(x0s, xF, nOb, vOb, A, b, ego, XYbounds, scenario="backwards", Ts=None, L=2.7, sampleN=3, Ncap=319, **kw):
@@ -255,6 +334,30 @@ def plan_solve_batch(x0s, xF, nOb, vOb, A, b, ego, XYbounds, scenario="backwards
     ox, oy = native.obstacle_points(scenario)
     Ts = Ts or (0.6 if scenario == "backwards" else 0.9) / 3 * sampleN
     return plan_solve_goals(x0s, np.asarray(xF, float)[:4], ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L, sampleN, Ncap, **kw)
+
+
+def _quadcopter_flow_inputs(x0s, xFs, ox, oy, oz, lo, hi, obs):
+    """The flow entries' quadcopter inputs as contiguous arrays: x0s, xFs (B, 12), the cloud and bounds, and ob (5, 6)."""
+    from .._lib import f64
+    x0s = f64(np.asarray(x0s, float).reshape(-1, 12)); B = x0s.shape[0]
+    xFs = f64(np.broadcast_to(np.asarray(xFs, float).reshape(-1, 12), (B, 12)))
+    ox, oy, oz, lo, hi = (f64(np.asarray(a, float).ravel()) for a in (ox, oy, oz, lo, hi))
+    return x0s, xFs, ox, oy, oz, lo, hi, f64(np.asarray(obs, float).reshape(5, 6))
+
+
+def _quadcopter_set(B, Ncap):
+    """One formulation's output arrays of the quadcopter flow for B pairs, NaN-filled (the integers -1)."""
+    NS = Ncap + 1
+    nan = lambda *s: np.full(s, np.nan)
+    i32 = lambda: np.full(B, -1, np.int32)
+    return dict(xp=nan(B, NS, 12), up=nan(B, Ncap, 4), ts=nan(B, NS), lp=nan(B, NS, 30), slack=nan(B, NS, 5), exitflag=i32(), iters=i32(),
+                kkt_err=nan(B), feasible=i32(), worst=nan(B))
+
+
+def _quadcopter_opts(opts):
+    if opts is None:
+        opts = _lib.default_opts(); opts.max_iter = 3000
+    return opts
 
 
 def plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS=1.0, signed_dist=1, Ncap=511, max_nodes=0,
@@ -269,19 +372,12 @@ def plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, ti
     host library (native.astar3d_raw, the same decisions), and those that plan to 2 <= N <= Ncap get their warm starts from
     native.quadcopter_warm_start and are solved and checked by quadcopter_solve_mixed / check_quadcopter_mixed in one more call each
     (their solve time is not in `time`)."""
-    from .._lib import f64
-    x0s = f64(np.asarray(x0s, float).reshape(-1, 12)); B = x0s.shape[0]
-    xFs = f64(np.broadcast_to(np.asarray(xFs, float).reshape(-1, 12), (B, 12)))
-    ox, oy, oz, lo, hi = (f64(np.asarray(a, float).ravel()) for a in (ox, oy, oz, lo, hi))
-    ob = f64(np.asarray(obs, float).reshape(5, 6))
-    NS = Ncap + 1
-    nan = lambda *s: np.full(s, np.nan)
+    x0s, xFs, ox, oy, oz, lo, hi, ob = _quadcopter_flow_inputs(x0s, xFs, ox, oy, oz, lo, hi, obs)
+    B = x0s.shape[0]
     i32 = lambda: np.full(B, -1, np.int32)
-    o = dict(xp=nan(B, NS, 12), up=nan(B, Ncap, 4), ts=nan(B, NS), lp=nan(B, NS, 30), slack=nan(B, NS, 5), N=i32(), Tsb=nan(B),
-             status=i32(), expansions=i32(), exitflag=i32(), iters=i32(), kkt_err=nan(B), feasible=i32(), worst=nan(B))
+    o = dict(_quadcopter_set(B, Ncap), N=i32(), Tsb=np.full(B, np.nan), status=i32(), expansions=i32())
     secs = np.zeros(2)
-    if opts is None:
-        opts = _lib.default_opts(); opts.max_iter = 3000
+    opts = _quadcopter_opts(opts)
     p = _lib.ptr
     f = _lib.lib().obca_quadcopter_plan_solve
     f.restype = C.c_int
@@ -295,25 +391,69 @@ def plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, ti
     o["plan_seconds"], o["time"] = float(secs[0]), float(secs[1])
     full = np.flatnonzero(o["status"] == POOL_FULL)
     if host_fallback and full.size:
-        _solve_quadcopter_on_host_plans(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS, signed_dist, Ncap, opts)
+        ws = _plan_quadcopter_on_host(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, Ncap)
+        _solve_quadcopter_on_host_plans(o, full, ws, x0s, xFs, R, obs, timeWS, signed_dist, opts)
     return o
 
 
-def _solve_quadcopter_on_host_plans(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS, signed_dist, Ncap, opts):
-    """Plan the pairs `full` with the host library, then solve and check the ones it plans to 2 <= N <= Ncap; their entries of o (the
-    layout of plan_solve_quadcopter_raw) get the results, the others the host planner's status (OBCA_PLAN_CAPACITY for a horizon outside
-    [2, Ncap])."""
-    from .. import quadcopter
+def plan_solve_quadcopter_both_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS=1.0, Ncap=511, max_nodes=0, opts=None,
+                                   host_fallback=False):
+    """obca_quadcopter_plan_solve_both's outputs as arrays: plan_solve_quadcopter_raw's arguments without signed_dist; every pair is
+    planned and warm-started once, then solved and checked with the Distance and then the Signed Distance formulation.  Returns the
+    shared N, Tsb, status, expansions and plan_seconds, and under "dist" and "sd" the per-formulation keys of plan_solve_quadcopter_raw
+    (xp, up, ts, lp, slack, exitflag, iters, kkt_err, feasible, worst, time), each what plan_solve_quadcopter_raw with signed_dist = 0 / 1
+    returns for the same inputs (the Dist set's slack is never written).  host_fallback: the POOL_FULL pairs are planned once by the host
+    library, then solved and checked with both formulations."""
+    x0s, xFs, ox, oy, oz, lo, hi, ob = _quadcopter_flow_inputs(x0s, xFs, ox, oy, oz, lo, hi, obs)
+    B = x0s.shape[0]
+    i32 = lambda: np.full(B, -1, np.int32)
+    o = dict(N=i32(), Tsb=np.full(B, np.nan), status=i32(), expansions=i32(), dist=_quadcopter_set(B, Ncap), sd=_quadcopter_set(B, Ncap))
+    secs = np.zeros(3)
+    sets = [_lib.QuadcopterFlowOut(*[o[f][k].ctypes.data for k in _QC_SET], secs[j + 1:j + 2].ctypes.data)
+            for j, f in enumerate(("dist", "sd"))]
+    opts = _quadcopter_opts(opts)
+    p = _lib.ptr
+    fn = _lib.lib().obca_quadcopter_plan_solve_both
+    fn.restype = C.c_int
+    fn.argtypes = ([C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_double, C.c_double, C.c_void_p,
+                                                     C.c_double, C.c_void_p, C.c_int] + [C.c_void_p] * 7)
+    rc = fn(B, p(x0s), p(xFs), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), float(Ts), float(R), p(ob),
+            float(timeWS), C.cast(C.byref(opts), C.c_void_p), int(Ncap), p(o["N"]), p(o["Tsb"]), p(o["status"]), p(o["expansions"]),
+            p(secs[:1]), *[C.cast(C.byref(s), C.c_void_p) for s in sets])
+    _lib.check(rc)
+    o["plan_seconds"] = float(secs[0])
+    o["dist"]["time"], o["sd"]["time"] = float(secs[1]), float(secs[2])
+    full = np.flatnonzero(o["status"] == POOL_FULL)
+    if host_fallback and full.size:
+        ws = _plan_quadcopter_on_host(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, Ncap)
+        for sd, f in ((0, "dist"), (1, "sd")):
+            _solve_quadcopter_on_host_plans(o[f], full, ws, x0s, xFs, R, obs, timeWS, sd, opts)
+    return o
+
+
+def _plan_quadcopter_on_host(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, Ncap):
+    """Plan the pairs `full` with the host library and build the warm starts of the ones it plans to 2 <= N <= Ncap; their status, N,
+    expansions and Tsb in o get its outputs (OBCA_PLAN_CAPACITY for a horizon outside [2, Ncap]).  Returns the positions in `full` of the
+    pairs to solve, their horizons and their warm starts (native.quadcopter_warm_start)."""
     h = native.astar3d_raw(x0s[full, :3] * 10.0, xFs[full, :3] * 10.0, ox, oy, oz, lo, hi, reso, Ncap + 1)
     st = h["status"].copy()
     st[(st == 0) & (h["N"] < 2)] = 2
     o["status"][full] = st; o["N"][full] = h["N"]; o["expansions"][full] = h["expansions"]
     ok = np.flatnonzero(st == 0)
-    if ok.size == 0:
-        return
     Ns = h["N"][ok]
     ws = [native.quadcopter_warm_start(h["rx"][i, :n + 1].copy(), h["ry"][i, :n + 1].copy(), h["rz"][i, :n + 1].copy(), Ts)
           for i, n in zip(ok, Ns)]
+    o["Tsb"][full[ok]] = [w["Ts"] for w in ws]
+    return ok, Ns, ws
+
+
+def _solve_quadcopter_on_host_plans(o, full, plans, x0s, xFs, R, obs, timeWS, signed_dist, opts):
+    """Solve and check the pairs of `plans` (_plan_quadcopter_on_host) with one formulation; their entries of o (one formulation's arrays
+    in the layout of plan_solve_quadcopter_raw) get the results."""
+    from .. import quadcopter
+    ok, Ns, ws = plans
+    if ok.size == 0:
+        return
     Tsb = np.array([w["Ts"] for w in ws])
     x0, xF = x0s[full[ok]], xFs[full[ok]]
     r = quadcopter.quadcopter_solve_mixed(x0, xF, Ns, Tsb, R, obs, [w["xWS"] for w in ws], timeWS, signed_dist, opts=opts)
@@ -322,9 +462,19 @@ def _solve_quadcopter_on_host_plans(o, full, x0s, xFs, ox, oy, oz, lo, hi, reso,
         for k, ext in (("xp", 1), ("up", 0), ("lp", 1)) + ((("slack", 1),) if signed_dist else ()):
             o[k][i, :n + ext] = r[k][q].T
         o["ts"][i, :n + 1] = r["ts"][q]
-    for k, v in (("Tsb", Tsb), ("exitflag", r["exitflag"]), ("iters", r["iters"]), ("kkt_err", r["kkt_err"]), ("feasible", feas),
-                 ("worst", worst)):
+    for k, v in (("exitflag", r["exitflag"]), ("iters", r["iters"]), ("kkt_err", r["kkt_err"]), ("feasible", feas), ("worst", worst)):
         o[k][full[ok]] = v
+
+
+def _quadcopter_lists(o, ok, N, signed_dist):
+    """One formulation's arrays of plan_solve_quadcopter_raw as per-pair lists in the Julia shapes (None where ok[i] is False)."""
+    cut = lambda a, ext: [a[i, :n + ext].T.copy() if ok[i] else None for i, n in enumerate(N)]
+    out = dict(xp=cut(o["xp"], 1), up=cut(o["up"], 0), ts=[o["ts"][i, :n + 1].copy() if ok[i] else None for i, n in enumerate(N)],
+               lp=cut(o["lp"], 1), slack=cut(o["slack"], 1) if signed_dist else [None] * len(ok))
+    for k in ("exitflag", "iters", "feasible"):
+        out[k] = np.where(ok, o[k], 0).astype(np.int32)
+    out.update(kkt_err=np.where(ok, o["kkt_err"], np.nan), worst=np.where(ok, o["worst"], np.nan), time=o["time"])
+    return out
 
 
 def plan_solve_quadcopter(x0s, xFs, R, obs, Ts=0.25, signed_dist=1, Ncap=511, max_nodes=0, opts=None, host_fallback=False):
@@ -340,12 +490,21 @@ def plan_solve_quadcopter(x0s, xFs, R, obs, Ts=0.25, signed_dist=1, Ncap=511, ma
     ox, oy, oz, lo, hi = quadcopter_environment()
     o = plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, 1.0, Ts, R, obs, 1.0, signed_dist, Ncap, max_nodes, opts, host_fallback)
     ok = o["status"] == 0
-    cut = lambda a, ext: [a[i, :n + ext].T.copy() if ok[i] else None for i, n in enumerate(o["N"])]
-    out = dict(xp=cut(o["xp"], 1), up=cut(o["up"], 0), ts=[o["ts"][i, :n + 1].copy() if ok[i] else None for i, n in enumerate(o["N"])],
-               lp=cut(o["lp"], 1), slack=cut(o["slack"], 1) if signed_dist else [None] * len(ok))
-    for k in ("exitflag", "iters", "feasible"):
-        out[k] = np.where(ok, o[k], 0).astype(np.int32)
-    out.update(kkt_err=np.where(ok, o["kkt_err"], np.nan), worst=np.where(ok, o["worst"], np.nan), N=o["N"].copy(),
-               Ts=np.where(ok, o["Tsb"], np.nan), status=o["status"].copy(), expansions=o["expansions"].copy(), time=o["time"],
+    out = _quadcopter_lists(o, ok, o["N"], signed_dist)
+    out.update(N=o["N"].copy(), Ts=np.where(ok, o["Tsb"], np.nan), status=o["status"].copy(), expansions=o["expansions"].copy(),
                plan_seconds=o["plan_seconds"])
     return out
+
+
+def plan_solve_quadcopter_both(x0s, xFs, R, obs, Ts=0.25, Ncap=511, max_nodes=0, opts=None, host_fallback=False):
+    """mainQuadcopter.jl:114-154 as the reference runs it, for a batch in one call (obca_quadcopter_plan_solve_both): every pair planned
+    and warm-started once, then solved and checked with QuadcopterDist and QuadcopterSignedDist.  Returns the shared N, Ts, status,
+    expansions and plan_seconds, and under "dist" and "sd" the per-formulation keys of plan_solve_quadcopter (per-pair lists in the Julia
+    shapes, None where the pair was not solved -- slack for "sd" only --, and exitflag, iters, kkt_err, feasible, worst, time)."""
+    from .a_star_3d import quadcopter_environment
+    ox, oy, oz, lo, hi = quadcopter_environment()
+    o = plan_solve_quadcopter_both_raw(x0s, xFs, ox, oy, oz, lo, hi, 1.0, Ts, R, obs, 1.0, Ncap, max_nodes, opts, host_fallback)
+    ok = o["status"] == 0
+    return dict(N=o["N"].copy(), Ts=np.where(ok, o["Tsb"], np.nan), status=o["status"].copy(), expansions=o["expansions"].copy(),
+                plan_seconds=o["plan_seconds"], dist=_quadcopter_lists(o["dist"], ok, o["N"], 0),
+                sd=_quadcopter_lists(o["sd"], ok, o["N"], 1))
