@@ -4,20 +4,58 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("OBCA_SO", os.path.join(HERE, "libobca.so"))   # OBCA_SO: development override
+HEADER = os.path.join(os.path.dirname(HERE), "include", "obca.h")
 
-SYMBOLS = ["obca_version", "obca_device_count", "obca_last_error", "obca_default_opts", "obca_parking_solve_batch",
-           "obca_parking_solve_batch_dev", "obca_dualmultws_batch", "obca_check_parking",
-           "obca_parking_eval_batch_dev", "obca_parking_eval_sizes", "obca_last_profile", "obca_last_schedule",
-           "obca_last_times", "obca_parking_solve_mixed", "obca_check_parking_mixed",
-           "obca_quadcopter_solve_batch", "obca_check_quadcopter", "obca_quadcopter_solve_mixed",
-           "obca_check_quadcopter_mixed", "obca_plan_parking_warmstart_batch", "obca_plan_quadcopter_warmstart_batch",
-           "obca_plan_parking_warmstart_goals", "obca_plan_parking_heuristic_maps", "obca_parking_plan_solve_goals",
-           "obca_quadcopter_plan_solve", "obca_parking_plan_solve_both", "obca_quadcopter_plan_solve_both"]
+
+class ObcaError(RuntimeError):
+    pass
+
+
+_ARG = {"int": C.c_int, "double": C.c_double, "long long": C.c_longlong}
+_RET = {"int": C.c_int, "double": C.c_double, "void": None, "const char *": C.c_char_p}
+
+
+def prototypes(header, error):
+    """{name: (restype, argtypes)} of every function `ret name(args);` the C header declares, in header order.  Every pointer
+    argument is c_void_p; int, double and long long arguments and int, double, void and const char* returns are typed as in C.
+    Any other type raises `error` naming the function: the binding never guesses a type."""
+    if not os.path.exists(header):
+        raise error(f"{header} not found: it declares the library's C-ABI")
+    with open(header) as f:
+        src = re.sub(r"/\*.*?\*/|//[^\n]*", " ", f.read(), flags=re.S)
+    src = re.sub(r"^[ \t]*#.*$", " ", src, flags=re.M)
+    src = " ".join(src.replace("*", " * ").split())      # one space between words and around every '*'
+    out = {}
+    for ret, name, args in re.findall(r"([\w *]+?) ?\b(\w+) ?\(([^()]*)\) ?;", src):
+        if ret.strip() not in _RET:
+            raise error(f"{header}: {name}: no ctypes type for the return type '{ret.strip()}'")
+        types = []
+        for a in ([] if args.strip() == "void" else args.split(",")):
+            a = a.strip()      # "const double * x0": the last word is the parameter's name
+            t = C.c_void_p if "*" in a else _ARG.get(a.rsplit(" ", 1)[0])
+            if t is None:
+                raise error(f"{header}: {name}: no ctypes type for the argument '{a}'")
+            types.append(t)
+        out[name] = (_RET[ret.strip()], types)
+    return out
+
+
+def declare(lib, protos):
+    """Type every function of `protos` (prototypes()) on the loaded library; a name it does not export raises."""
+    for name, (res, args) in protos.items():
+        f = getattr(lib, name)
+        f.restype, f.argtypes = res, args
+    return lib
+
+
+_PROTOTYPES = prototypes(HEADER, ObcaError)
+SYMBOLS = tuple(_PROTOTYPES)      # the functions include/obca.h declares
 
 
 class ObcaOpts(C.Structure):
@@ -44,10 +82,6 @@ class QuadcopterFlowOut(C.Structure):
                                           "solve_seconds")]
 
 
-class ObcaError(RuntimeError):
-    pass
-
-
 _lib = None
 
 
@@ -58,10 +92,7 @@ def lib():
         if not os.path.exists(SO_PATH):
             raise ObcaError(f"{SO_PATH} not found: run `python -c 'import __graft_entry__ as g; g.build()'` "
                             "(the OBCA hot path has no CPU fallback)")
-        _lib = C.CDLL(SO_PATH)
-        _lib.obca_last_error.restype = C.c_char_p
-        for s in SYMBOLS:
-            getattr(_lib, s)
+        _lib = declare(C.CDLL(SO_PATH), _PROTOTYPES)
     return _lib
 
 
@@ -71,6 +102,11 @@ def default_opts(device=0, retry=1) -> ObcaOpts:
     o.device = device
     o.retry = retry
     return o
+
+
+def opts_arg(opts):
+    """The opts argument of an entry: a reference to `opts`, or NULL for None, which selects the library's defaults."""
+    return None if opts is None else C.byref(opts)
 
 
 def check(rc):

@@ -17,7 +17,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import check, f64, lib, ptr
+from ._lib import opts_arg, check, f64, lib, ptr
 
 ego = None   # DualMultWS reads a global `ego` in the reference (DualMultWS.jl:39); set obca_b200.parking.ego
 
@@ -47,15 +47,13 @@ def parking_solve_batch(x0, xF, N, Ts, L, ego_, XYbounds, nOb, vOb, A, b, rx, ry
     if lWS is not None:
         lW = f64(np.transpose(np.asarray(lWS, dtype=np.float64).reshape(B, NS, V), (0, 2, 1)))
         nW = f64(np.transpose(np.asarray(nWS, dtype=np.float64).reshape(B, NS, 4 * nOb), (0, 2, 1)))
-    o = opts if opts is not None else _lib.default_opts()
     xp = np.zeros((B, NS, 4)); up = np.zeros((B, N, 2)); ts = np.zeros((B, NS))
     lp = np.zeros((B, NS, V)); npp = np.zeros((B, NS, 4 * nOb)); sl = np.zeros((B, NS, nOb))
     ef = np.zeros(B, np.int32); it = np.zeros(B, np.int32); err = np.zeros(B); sec = np.zeros(1)
     check(lib().obca_parking_solve_batch(
-        C.c_int(B), C.c_int(N), C.c_int(nOb), ptr(vOb), ptr(A), ptr(b), ptr(x0), ptr(xF), C.c_double(Ts),
-        C.c_double(L), ptr(f64(np.asarray(ego_).ravel())), ptr(f64(np.asarray(XYbounds).ravel())), ptr(rx), ptr(ry),
-        ptr(ryaw), ptr(xWS), ptr(uWS), ptr(lW), ptr(nW), C.c_int(int(fixTime)), C.c_int(int(signed_dist)), C.byref(o),
-        ptr(xp), ptr(up), ptr(ts), ptr(lp), ptr(npp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
+        B, N, nOb, ptr(vOb), ptr(A), ptr(b), ptr(x0), ptr(xF), float(Ts), float(L), ptr(f64(np.asarray(ego_).ravel())),
+        ptr(f64(np.asarray(XYbounds).ravel())), ptr(rx), ptr(ry), ptr(ryaw), ptr(xWS), ptr(uWS), ptr(lW), ptr(nW), int(fixTime),
+        int(signed_dist), opts_arg(opts), ptr(xp), ptr(up), ptr(ts), ptr(lp), ptr(npp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
     T = lambda a: np.transpose(a, (0, 2, 1))
     return dict(xp=T(xp), up=T(up), ts=ts, lp=T(lp), np=T(npp), sl=T(sl), exitflag=ef, iters=it, kkt_err=err,
                 time=float(sec[0]))
@@ -94,15 +92,13 @@ def parking_solve_mixed(x0, xF, Ns, Ts, L, ego_, XYbounds, nOb, vOb, A, b, rx, r
     if lWS is not None:
         lW = T(_pad_stages([np.asarray(w, float).reshape(-1, V)[:n + 1] for w, n in zip(lWS, Ns)], Nmax))
         nW = T(_pad_stages([np.asarray(w, float).reshape(-1, 4 * nOb)[:n + 1] for w, n in zip(nWS, Ns)], Nmax))
-    o = opts if opts is not None else _lib.default_opts()
     xp = np.zeros((B, NS, 4)); up = np.zeros((B, Nmax, 2)); ts = np.zeros((B, NS))
     lp = np.zeros((B, NS, V)); npp = np.zeros((B, NS, 4 * nOb)); sl = np.zeros((B, NS, nOb))
     ef = np.zeros(B, np.int32); it = np.zeros(B, np.int32); err = np.zeros(B); sec = np.zeros(1)
     check(lib().obca_parking_solve_mixed(
-        C.c_int(B), ptr(Ns), C.c_int(Nmax), C.c_int(nOb), ptr(vOb), ptr(A), ptr(b), ptr(x0), ptr(xF), C.c_double(Ts),
-        C.c_double(L), ptr(f64(np.asarray(ego_).ravel())), ptr(f64(np.asarray(XYbounds).ravel())), ptr(rx), ptr(ry),
-        ptr(ryaw), ptr(xW), ptr(uW), ptr(lW), ptr(nW), C.c_int(int(fixTime)), C.c_int(int(signed_dist)), C.byref(o),
-        ptr(xp), ptr(up), ptr(ts), ptr(lp), ptr(npp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
+        B, ptr(Ns), Nmax, nOb, ptr(vOb), ptr(A), ptr(b), ptr(x0), ptr(xF), float(Ts), float(L), ptr(f64(np.asarray(ego_).ravel())),
+        ptr(f64(np.asarray(XYbounds).ravel())), ptr(rx), ptr(ry), ptr(ryaw), ptr(xW), ptr(uW), ptr(lW), ptr(nW), int(fixTime),
+        int(signed_dist), opts_arg(opts), ptr(xp), ptr(up), ptr(ts), ptr(lp), ptr(npp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
     cut = lambda a, ext: [a[i, :n + ext].T.copy() for i, n in enumerate(Ns)]
     return dict(xp=cut(xp, 1), up=cut(up, 0), ts=[ts[i, :n + 1].copy() for i, n in enumerate(Ns)], lp=cut(lp, 1),
                 np=cut(npp, 1), sl=cut(sl, 1), exitflag=ef, iters=it, kkt_err=err, N=Ns.copy(), time=float(sec[0]))
@@ -130,10 +126,8 @@ def dualmultws_batch(N, nOb, vOb, A, b, rx, ry, ryaw, ego_, opts=None, want_d=Fa
     ry = f64(np.atleast_2d(ry)); ryaw = f64(np.atleast_2d(ryaw))
     vOb, V, A, b = _shared(nOb, vOb, A, b)
     lp = np.zeros((B, V, NS)); npp = np.zeros((B, 4 * nOb, NS)); d = np.zeros((B, nOb, NS))
-    o = opts if opts is not None else _lib.default_opts()
-    check(lib().obca_dualmultws_batch(C.c_int(B), C.c_int(N), C.c_int(nOb), ptr(vOb), ptr(A), ptr(b),
-                                      ptr(f64(np.asarray(ego_).ravel())), ptr(rx), ptr(ry), ptr(ryaw), C.byref(o),
-                                      ptr(lp), ptr(npp), ptr(d)))
+    check(lib().obca_dualmultws_batch(B, N, nOb, ptr(vOb), ptr(A), ptr(b), ptr(f64(np.asarray(ego_).ravel())), ptr(rx), ptr(ry),
+                                      ptr(ryaw), opts_arg(opts), ptr(lp), ptr(npp), ptr(d)))
     T = lambda a: np.transpose(a, (0, 2, 1)).copy()
     return (T(lp), T(npp), T(d)) if want_d else (T(lp), T(npp))
 
@@ -159,11 +153,9 @@ def check_parking_batch(x0, xF, N, Ts, L, ego_, XYbounds, nOb, vOb, A, b, x, u, 
     x0 = f64(np.broadcast_to(np.asarray(x0, float).reshape(-1, 4), (B, 4)))
     xF = f64(np.broadcast_to(np.asarray(xF, float).reshape(-1, 4), (B, 4)))
     feas = np.zeros(B, np.int32); e = np.zeros((B, 7), np.int32); strict = np.zeros(B, np.int32)
-    o = opts if opts is not None else _lib.default_opts()
-    check(lib().obca_check_parking(C.c_int(B), C.c_int(N), C.c_int(nOb), ptr(vOb), ptr(A), ptr(b), ptr(x0), ptr(xF),
-                                   C.c_double(Ts), C.c_double(L), ptr(f64(np.asarray(ego_).ravel())),
-                                   ptr(f64(np.asarray(XYbounds).ravel())), ptr(xx), ptr(uu), ptr(ll), ptr(nn), ptr(tt),
-                                   ptr(ss), C.c_int(int(fixTime)), C.c_int(int(sd)), C.byref(o), ptr(feas), ptr(e),
+    check(lib().obca_check_parking(B, N, nOb, ptr(vOb), ptr(A), ptr(b), ptr(x0), ptr(xF), float(Ts), float(L),
+                                   ptr(f64(np.asarray(ego_).ravel())), ptr(f64(np.asarray(XYbounds).ravel())), ptr(xx), ptr(uu),
+                                   ptr(ll), ptr(nn), ptr(tt), ptr(ss), int(fixTime), int(sd), opts_arg(opts), ptr(feas), ptr(e),
                                    ptr(strict)))
     return feas, e, strict
 
@@ -183,12 +175,10 @@ def check_parking_mixed(x0, xF, Ns, Ts, L, ego_, XYbounds, nOb, vOb, A, b, x, u,
     x0 = f64(np.broadcast_to(np.asarray(x0, float).reshape(-1, 4), (B, 4)))
     xF = f64(np.broadcast_to(np.asarray(xF, float).reshape(-1, 4), (B, 4)))
     feas = np.zeros(B, np.int32); e = np.zeros((B, 7), np.int32); strict = np.zeros(B, np.int32)
-    o = opts if opts is not None else _lib.default_opts()
-    check(lib().obca_check_parking_mixed(C.c_int(B), ptr(Ns), C.c_int(Nmax), C.c_int(nOb), ptr(vOb), ptr(A), ptr(b), ptr(x0),
-                                         ptr(xF), C.c_double(Ts), C.c_double(L), ptr(f64(np.asarray(ego_).ravel())),
-                                         ptr(f64(np.asarray(XYbounds).ravel())), ptr(xx), ptr(uu), ptr(ll), ptr(nn), ptr(tt),
-                                         ptr(ss), C.c_int(int(fixTime)), C.c_int(int(sd)), C.byref(o), ptr(feas), ptr(e),
-                                         ptr(strict)))
+    check(lib().obca_check_parking_mixed(B, ptr(Ns), Nmax, nOb, ptr(vOb), ptr(A), ptr(b), ptr(x0), ptr(xF), float(Ts), float(L),
+                                         ptr(f64(np.asarray(ego_).ravel())), ptr(f64(np.asarray(XYbounds).ravel())), ptr(xx),
+                                         ptr(uu), ptr(ll), ptr(nn), ptr(tt), ptr(ss), int(fixTime), int(sd), opts_arg(opts), ptr(feas),
+                                         ptr(e), ptr(strict)))
     return feas, e, strict
 
 
@@ -209,7 +199,7 @@ def eval_batch(x0, xF, N, Ts, L, ego_, XYbounds, nOb, vOb, A, b, rx, ry, ryaw, f
     xp = np.asarray(xp, float); B = xp.shape[0]; NS = N + 1
     vOb, V, A, b = _shared(nOb, vOb, A, b)
     nn = C.c_longlong(); mm = C.c_longlong()
-    check(lib().obca_parking_eval_sizes(C.c_int(N), C.c_int(nOb), ptr(vOb), C.c_int(int(signed_dist)), C.byref(nn), C.byref(mm)))
+    check(lib().obca_parking_eval_sizes(N, nOb, ptr(vOb), int(signed_dist), C.byref(nn), C.byref(mm)))
     n, m = nn.value, mm.value
     o = opts if opts is not None else _lib.default_opts()
     dev = torch.device("cuda", o.device)
@@ -227,10 +217,9 @@ def eval_batch(x0, xF, N, Ts, L, ego_, XYbounds, nOb, vOb, A, b, rx, ry, ryaw, f
     P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
     torch.cuda.synchronize(dev)      # the library launches on its own stream: torch's copies / fills must have landed first
     check(lib().obca_parking_eval_batch_dev(
-        C.c_int(B), C.c_int(N), C.c_int(nOb), ptr(vOb), ptr(A), ptr(b), P(bx0), P(bxF), C.c_double(Ts), C.c_double(L),
-        ptr(f64(np.asarray(ego_).ravel())), ptr(f64(np.asarray(XYbounds).ravel())), P(brx), P(bry), P(bryaw), P(dxp), P(dup), P(dts),
-        P(dlp), P(dnp), P(dsl), P(dy), C.c_int(int(fixTime)), C.c_int(int(signed_dist)), C.byref(o), P(c), P(g), P(fk),
-        C.c_int(int(reps)), ptr(ms)))
+        B, N, nOb, ptr(vOb), ptr(A), ptr(b), P(bx0), P(bxF), float(Ts), float(L), ptr(f64(np.asarray(ego_).ravel())),
+        ptr(f64(np.asarray(XYbounds).ravel())), P(brx), P(bry), P(bryaw), P(dxp), P(dup), P(dts), P(dlp), P(dnp), P(dsl), P(dy),
+        int(fixTime), int(signed_dist), C.byref(o), P(c), P(g), P(fk), int(reps), ptr(ms)))
     return c.cpu().numpy(), g.cpu().numpy(), fk.sum(1).cpu().numpy(), float(ms[0])
 
 

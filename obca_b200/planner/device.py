@@ -27,14 +27,10 @@ def _plan_call(entry, x0s, xF, ox, oy, Ts, L, sampleN, cap, max_nodes, max_expan
     o = dict(rx=np.full((B, cap), np.nan), ry=np.full((B, cap), np.nan), ryaw=np.full((B, cap), np.nan), xWS=np.full((B, 4 * cap), np.nan),
              uWS=np.full((B, 2 * cap), np.nan), N=np.full(B, -1, np.int32), status=np.full(B, -1, np.int32), expansions=np.zeros(B, np.int32))
     secs = C.c_double(0.0)
-    opts = opts if opts is not None else _lib.default_opts()
     p = _lib.ptr
-    f = getattr(_lib.lib(), entry)
-    f.restype = C.c_int
-    f.argtypes = [C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 10
-    rc = f(B, p(x0s), p(xF), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(cap),
-           C.cast(C.byref(opts), C.c_void_p), *[p(o[k]) for k in ("rx", "ry", "ryaw", "xWS", "uWS", "N", "status", "expansions")],
-           C.cast(C.byref(secs), C.c_void_p))
+    rc = getattr(_lib.lib(), entry)(B, p(x0s), p(xF), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions),
+                                    int(max_nodes), int(cap), _lib.opts_arg(opts),
+                                    *[p(o[k]) for k in ("rx", "ry", "ryaw", "xWS", "uWS", "N", "status", "expansions")], C.byref(secs))
     _lib.check(rc)
     o["seconds"] = secs.value
     return o
@@ -80,14 +76,11 @@ def heuristic_maps(goals, ox, oy, opts=None):
     g = np.ascontiguousarray(np.asarray(goals, float).reshape(len(goals), -1)[:, :2]); G = g.shape[0]
     ox = np.ascontiguousarray(ox, float); oy = np.ascontiguousarray(oy, float)
     mn = np.zeros(2, np.int64); w = np.zeros(2, np.int32); secs = C.c_double(0.0)
-    opts = opts if opts is not None else _lib.default_opts()
     p = _lib.ptr
     f = _lib.lib().obca_plan_parking_heuristic_maps
-    f.restype = C.c_int
-    f.argtypes = [C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 4 + [C.c_longlong, C.c_void_p]
-    f(G, p(g), p(ox), p(oy), int(ox.size), C.cast(C.byref(opts), C.c_void_p), p(mn), p(w), None, 0, None)      # reads the size
+    f(G, p(g), p(ox), p(oy), int(ox.size), _lib.opts_arg(opts), p(mn), p(w), None, 0, None)      # reads the size
     m = np.zeros(G * int(w[0]) * int(w[1]))
-    rc = f(G, p(g), p(ox), p(oy), int(ox.size), C.cast(C.byref(opts), C.c_void_p), p(mn), p(w), p(m), m.size, C.cast(C.byref(secs), C.c_void_p))
+    rc = f(G, p(g), p(ox), p(oy), int(ox.size), _lib.opts_arg(opts), p(mn), p(w), p(m), m.size, C.byref(secs))
     _lib.check(rc)
     return m.reshape(G, int(w[0]), int(w[1])), (int(mn[0]), int(mn[1])), secs.value
 
@@ -102,13 +95,10 @@ def plan_quadcopter_raw(starts, goals, ox, oy, oz, lo, hi, reso, cap=1024, max_n
     o = dict(rx=np.full((B, cap), np.nan), ry=np.full((B, cap), np.nan), rz=np.full((B, cap), np.nan), N=np.full(B, -1, np.int32),
              status=np.full(B, -1, np.int32), expansions=np.full(B, -1, np.int32))
     secs = C.c_double(0.0)
-    opts = opts if opts is not None else _lib.default_opts()
     p = _lib.ptr
-    fn = _lib.lib().obca_plan_quadcopter_warmstart_batch
-    fn.restype = C.c_int
-    fn.argtypes = [C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_int] + [C.c_void_p] * 8
-    rc = fn(B, p(s), p(g), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), int(cap), C.cast(C.byref(opts), C.c_void_p),
-            *[p(o[k]) for k in ("rx", "ry", "rz", "N", "status", "expansions")], C.cast(C.byref(secs), C.c_void_p))
+    rc = _lib.lib().obca_plan_quadcopter_warmstart_batch(B, p(s), p(g), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso),
+                                                         int(max_nodes), int(cap), _lib.opts_arg(opts),
+                                                         *[p(o[k]) for k in ("rx", "ry", "rz", "N", "status", "expansions")], C.byref(secs))
     _lib.check(rc)
     o["seconds"] = secs.value
     return o
@@ -201,17 +191,13 @@ def plan_solve_goals_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbounds, L=
     i32 = lambda: np.full(B, -1, np.int32)
     o = dict(_parking_set(B, Ncap, V, nOb), N=i32(), status=i32(), expansions=i32())
     secs = np.zeros(2)
-    opts = opts if opts is not None else _lib.default_opts()
     p = _lib.ptr
-    f = _lib.lib().obca_parking_plan_solve_goals
-    f.restype = C.c_int
-    f.argtypes = ([C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 5
-                  + [C.c_int, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 16)
-    rc = f(B, p(x0s), p(xFs), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(nOb),
-           p(vOb), p(A), p(b), p(f64(np.asarray(ego).ravel())), p(f64(np.asarray(XYbounds).ravel())), int(fixTime), int(signed_dist),
-           C.cast(C.byref(opts), C.c_void_p), int(Ncap),
-           *[p(o[k]) for k in ("xp", "up", "ts", "lp", "np", "sl", "N", "status", "expansions", "exitflag", "iters", "kkt_err", "feasible",
-                               "strict")], p(secs[:1]), p(secs[1:]))
+    rc = _lib.lib().obca_parking_plan_solve_goals(
+        B, p(x0s), p(xFs), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(nOb),
+        p(vOb), p(A), p(b), p(f64(np.asarray(ego).ravel())), p(f64(np.asarray(XYbounds).ravel())), int(fixTime), int(signed_dist),
+        _lib.opts_arg(opts), int(Ncap),
+        *[p(o[k]) for k in ("xp", "up", "ts", "lp", "np", "sl", "N", "status", "expansions", "exitflag", "iters", "kkt_err", "feasible",
+                            "strict")], p(secs[:1]), p(secs[1:]))
     _lib.check(rc)
     o["plan_seconds"], o["time"] = float(secs[0]), float(secs[1])
     full = np.flatnonzero(o["status"] == POOL_FULL)
@@ -235,16 +221,11 @@ def plan_solve_goals_both_raw(x0s, xFs, ox, oy, Ts, nOb, vOb, A, b, ego, XYbound
     o = dict(N=i32(), status=i32(), expansions=i32(), dist=_parking_set(B, Ncap, V, nOb), sd=_parking_set(B, Ncap, V, nOb))
     secs = np.zeros(3)
     sets = [_lib.ParkingFlowOut(*[o[f][k].ctypes.data for k in _PK_SET], secs[j + 1:j + 2].ctypes.data) for j, f in enumerate(("dist", "sd"))]
-    opts = opts if opts is not None else _lib.default_opts()
     p = _lib.ptr
-    fn = _lib.lib().obca_parking_plan_solve_both
-    fn.restype = C.c_int
-    fn.argtypes = ([C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 5
-                   + [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 6)
-    rc = fn(B, p(x0s), p(xFs), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(nOb),
-            p(vOb), p(A), p(b), p(f64(np.asarray(ego).ravel())), p(f64(np.asarray(XYbounds).ravel())), int(fixTime),
-            C.cast(C.byref(opts), C.c_void_p), int(Ncap), p(o["N"]), p(o["status"]), p(o["expansions"]), p(secs[:1]),
-            *[C.cast(C.byref(s), C.c_void_p) for s in sets])
+    rc = _lib.lib().obca_parking_plan_solve_both(
+        B, p(x0s), p(xFs), p(ox), p(oy), int(ox.size), float(Ts), float(L), int(sampleN), int(max_expansions), int(max_nodes), int(nOb),
+        p(vOb), p(A), p(b), p(f64(np.asarray(ego).ravel())), p(f64(np.asarray(XYbounds).ravel())), int(fixTime), _lib.opts_arg(opts),
+        int(Ncap), p(o["N"]), p(o["status"]), p(o["expansions"]), p(secs[:1]), *[C.byref(s) for s in sets])
     _lib.check(rc)
     o["plan_seconds"] = float(secs[0])
     o["dist"]["time"], o["sd"]["time"] = float(secs[1]), float(secs[2])
@@ -354,12 +335,6 @@ def _quadcopter_set(B, Ncap):
                 kkt_err=nan(B), feasible=i32(), worst=nan(B))
 
 
-def _quadcopter_opts(opts):
-    if opts is None:
-        opts = _lib.default_opts(); opts.max_iter = 3000
-    return opts
-
-
 def plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, timeWS=1.0, signed_dist=1, Ncap=511, max_nodes=0,
                               opts=None, host_fallback=False):
     """obca_quadcopter_plan_solve's outputs as arrays: plan every pair x0s[i] -> xFs[i] ((B, 12) in the solve's units; the planner takes
@@ -377,16 +352,12 @@ def plan_solve_quadcopter_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, obs, ti
     i32 = lambda: np.full(B, -1, np.int32)
     o = dict(_quadcopter_set(B, Ncap), N=i32(), Tsb=np.full(B, np.nan), status=i32(), expansions=i32())
     secs = np.zeros(2)
-    opts = _quadcopter_opts(opts)
     p = _lib.ptr
-    f = _lib.lib().obca_quadcopter_plan_solve
-    f.restype = C.c_int
-    f.argtypes = ([C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_double, C.c_double, C.c_void_p,
-                                                    C.c_double, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 16)
-    rc = f(B, p(x0s), p(xFs), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), float(Ts), float(R), p(ob),
-           float(timeWS), int(signed_dist), C.cast(C.byref(opts), C.c_void_p), int(Ncap),
-           *[p(o[k]) for k in ("xp", "up", "ts", "lp", "slack", "N", "Tsb", "status", "expansions", "exitflag", "iters", "kkt_err",
-                               "feasible", "worst")], p(secs[:1]), p(secs[1:]))
+    rc = _lib.lib().obca_quadcopter_plan_solve(
+        B, p(x0s), p(xFs), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), float(Ts), float(R), p(ob),
+        float(timeWS), int(signed_dist), _lib.opts_arg(opts), int(Ncap),
+        *[p(o[k]) for k in ("xp", "up", "ts", "lp", "slack", "N", "Tsb", "status", "expansions", "exitflag", "iters", "kkt_err",
+                            "feasible", "worst")], p(secs[:1]), p(secs[1:]))
     _lib.check(rc)
     o["plan_seconds"], o["time"] = float(secs[0]), float(secs[1])
     full = np.flatnonzero(o["status"] == POOL_FULL)
@@ -411,15 +382,11 @@ def plan_solve_quadcopter_both_raw(x0s, xFs, ox, oy, oz, lo, hi, reso, Ts, R, ob
     secs = np.zeros(3)
     sets = [_lib.QuadcopterFlowOut(*[o[f][k].ctypes.data for k in _QC_SET], secs[j + 1:j + 2].ctypes.data)
             for j, f in enumerate(("dist", "sd"))]
-    opts = _quadcopter_opts(opts)
     p = _lib.ptr
-    fn = _lib.lib().obca_quadcopter_plan_solve_both
-    fn.restype = C.c_int
-    fn.argtypes = ([C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_double, C.c_double, C.c_void_p,
-                                                     C.c_double, C.c_void_p, C.c_int] + [C.c_void_p] * 7)
-    rc = fn(B, p(x0s), p(xFs), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), float(Ts), float(R), p(ob),
-            float(timeWS), C.cast(C.byref(opts), C.c_void_p), int(Ncap), p(o["N"]), p(o["Tsb"]), p(o["status"]), p(o["expansions"]),
-            p(secs[:1]), *[C.cast(C.byref(s), C.c_void_p) for s in sets])
+    rc = _lib.lib().obca_quadcopter_plan_solve_both(
+        B, p(x0s), p(xFs), p(ox), p(oy), p(oz), int(ox.size), p(lo), p(hi), float(reso), int(max_nodes), float(Ts), float(R), p(ob),
+        float(timeWS), _lib.opts_arg(opts), int(Ncap), p(o["N"]), p(o["Tsb"]), p(o["status"]), p(o["expansions"]), p(secs[:1]),
+        *[C.byref(s) for s in sets])
     _lib.check(rc)
     o["plan_seconds"] = float(secs[0])
     o["dist"]["time"], o["sd"]["time"] = float(secs[1]), float(secs[2])

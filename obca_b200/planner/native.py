@@ -8,8 +8,11 @@ import os
 
 import numpy as np
 
+from .._lib import declare, prototypes
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(HERE, "libobca_planner.so")
+HEADER = os.path.join(os.path.dirname(os.path.dirname(HERE)), "include", "obca_planner.h")
 _lib = None
 
 
@@ -22,26 +25,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(SO_PATH):
             raise PlannerError(f"{SO_PATH} not found: run `python -c 'import __graft_entry__ as g; g.build()'`")
-        L = C.CDLL(SO_PATH)
-        d, i, p = C.c_double, C.c_int, C.c_void_p
-        L.obca_planner_version.restype = i
-        L.obca_hybrid_astar.restype = i
-        L.obca_hybrid_astar.argtypes = [d] * 6 + [p, p, i, d, d, i, i, p, p, p, p]
-        L.obca_scenario_obstacle_points.restype = i
-        L.obca_scenario_obstacle_points.argtypes = [i, i, p, p, p]
-        L.obca_plan_warmstart.restype = i
-        L.obca_plan_warmstart.argtypes = [p, p, i, d, d, i, i, p, p, p, p, p, p]
-        L.obca_plan_warmstart_batch.restype = i
-        L.obca_plan_warmstart_batch.argtypes = [i, p, p, i, d, d, i, i, i] + [p] * 7
-        L.obca_plan_warmstart_cloud_batch.restype = i
-        L.obca_plan_warmstart_cloud_batch.argtypes = [i, p, p, p, p, i, d, d, i, i, i] + [p] * 8
-        L.obca_reeds_shepp_length.restype = d
-        L.obca_reeds_shepp_length.argtypes = [d] * 7
-        L.obca_astar3d_batch.restype = i
-        L.obca_astar3d_batch.argtypes = [i] + [p] * 5 + [i, p, p, d, i, i] + [p] * 6
-        L.obca_astar3d_obstacle_map.restype = i
-        L.obca_astar3d_obstacle_map.argtypes = [p] * 3 + [i, p, p, d, p, p, p, C.c_longlong]
-        _lib = L
+        _lib = declare(C.CDLL(SO_PATH), prototypes(HEADER, PlannerError))
     return _lib
 
 

@@ -8,29 +8,25 @@ All computation happens in libobca.so on the GPU (obca_quadcopter_solve_batch / 
 twins for a batch whose problems have their own horizon and sampling time)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from . import _lib
-from ._lib import check, f64, lib, ptr
+from ._lib import opts_arg, check, f64, lib, ptr
 from .parking import _pad_stages
 
 
 def quadcopter_solve_batch(x0, xF, N, Ts, R, obs, xWS, timeWS=1.0, signed_dist=1, opts=None):
     """x0, xF (B,12); obs (5,6) = ob1..ob5; xWS (B,12,N+1).  Returns dict with Julia-shaped stacks:
-    xp (B,12,N+1), up (B,4,N), ts (B,N+1), lp (B,30,N+1), slack (B,5,N+1), exitflag, iters, kkt_err, time."""
+    xp (B,12,N+1), up (B,4,N), ts (B,N+1), lp (B,30,N+1), slack (B,5,N+1), exitflag, iters, kkt_err, time.  opts None: the library's
+    defaults with max_iter = 3000 (the reference leaves Ipopt's default max_iter)."""
     x0 = f64(np.atleast_2d(x0)); B = x0.shape[0]; NS = N + 1
     xF = f64(np.broadcast_to(np.asarray(xF, float).reshape(-1, 12), (B, 12)))
     ob = f64(np.asarray(obs, float).reshape(5, 6))                       # rows = obstacles == 6 x 5 column-major
     xw = f64(np.transpose(np.asarray(xWS, float).reshape(B, 12, -1)[:, :, :NS], (0, 2, 1)))
     xp = np.zeros((B, NS, 12)); up = np.zeros((B, N, 4)); ts = np.zeros((B, NS)); lp = np.zeros((B, NS, 30)); sl = np.zeros((B, NS, 5))
     ef = np.zeros(B, np.int32); it = np.zeros(B, np.int32); err = np.zeros(B); sec = np.zeros(1)
-    if opts is None:
-        opts = _lib.default_opts(); opts.max_iter = 3000                 # the reference leaves Ipopt's default max_iter
-    check(lib().obca_quadcopter_solve_batch(C.c_int(B), C.c_int(N), ptr(x0), ptr(xF), C.c_double(Ts), C.c_double(R), ptr(ob), ptr(xw),
-                                            C.c_double(float(timeWS)), C.c_int(int(signed_dist)), C.byref(opts), ptr(xp), ptr(up), ptr(ts),
-                                            ptr(lp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
+    check(lib().obca_quadcopter_solve_batch(B, N, ptr(x0), ptr(xF), float(Ts), float(R), ptr(ob), ptr(xw), float(timeWS), int(signed_dist),
+                                            opts_arg(opts), ptr(xp), ptr(up), ptr(ts), ptr(lp), ptr(sl), ptr(ef), ptr(it), ptr(err),
+                                            ptr(sec)))
     T = lambda a: np.transpose(a, (0, 2, 1))
     return dict(xp=T(xp), up=T(up), ts=ts, lp=T(lp), slack=T(sl), exitflag=ef, iters=it, kkt_err=err, time=float(sec[0]))
 
@@ -56,11 +52,9 @@ def quadcopter_solve_mixed(x0, xF, Ns, Ts, R, obs, xWS, timeWS=1.0, signed_dist=
     xw = f64(_pad_stages([np.asarray(w, float).reshape(12, -1)[:, :n + 1].T for w, n in zip(xWS, Ns)], Nmax))
     xp = np.zeros((B, NS, 12)); up = np.zeros((B, Nmax, 4)); ts = np.zeros((B, NS)); lp = np.zeros((B, NS, 30)); sl = np.zeros((B, NS, 5))
     ef = np.zeros(B, np.int32); it = np.zeros(B, np.int32); err = np.zeros(B); sec = np.zeros(1)
-    if opts is None:
-        opts = _lib.default_opts(); opts.max_iter = 3000                 # as quadcopter_solve_batch
-    check(lib().obca_quadcopter_solve_mixed(C.c_int(B), ptr(Ns), C.c_int(Nmax), ptr(x0), ptr(xF), ptr(Tsb), C.c_double(R), ptr(ob), ptr(xw),
-                                            C.c_double(float(timeWS)), C.c_int(int(signed_dist)), C.byref(opts), ptr(xp), ptr(up), ptr(ts),
-                                            ptr(lp), ptr(sl), ptr(ef), ptr(it), ptr(err), ptr(sec)))
+    check(lib().obca_quadcopter_solve_mixed(B, ptr(Ns), Nmax, ptr(x0), ptr(xF), ptr(Tsb), float(R), ptr(ob), ptr(xw), float(timeWS),
+                                            int(signed_dist), opts_arg(opts), ptr(xp), ptr(up), ptr(ts), ptr(lp), ptr(sl), ptr(ef), ptr(it),
+                                            ptr(err), ptr(sec)))
     cut = lambda a, ext: [a[i, :n + ext].T.copy() for i, n in enumerate(Ns)]
     return dict(xp=cut(xp, 1), up=cut(up, 0), ts=[ts[i, :n + 1].copy() for i, n in enumerate(Ns)], lp=cut(lp, 1), slack=cut(sl, 1),
                 exitflag=ef, iters=it, kkt_err=err, N=Ns.copy(), Ts=Tsb.copy(), time=float(sec[0]))
@@ -91,9 +85,8 @@ def check_quadcopter_batch(x, u, timeScale, x0, xF, Ts, lam, obs, R, opts=None):
     tt = f64(np.asarray(timeScale, float).reshape(B, N + 1))
     ob = f64(np.asarray(obs, float).reshape(5, 6))
     feas = np.zeros(B, np.int32); worst = np.zeros(B)
-    o = opts if opts is not None else _lib.default_opts()
-    check(lib().obca_check_quadcopter(C.c_int(B), C.c_int(N), ptr(xx), ptr(uu), ptr(tt), ptr(x0), ptr(xF), C.c_double(Ts), ptr(ll), ptr(ob),
-                                      C.c_double(R), C.byref(o), ptr(feas), ptr(worst)))
+    check(lib().obca_check_quadcopter(B, N, ptr(xx), ptr(uu), ptr(tt), ptr(x0), ptr(xF), float(Ts), ptr(ll), ptr(ob), float(R),
+                                      opts_arg(opts), ptr(feas), ptr(worst)))
     return feas, worst
 
 
@@ -110,9 +103,8 @@ def check_quadcopter_mixed(x, u, timeScale, x0, xF, Ns, Ts, lam, obs, R, opts=No
     x0 = f64(np.broadcast_to(np.asarray(x0, float).reshape(-1, 12), (B, 12))); xF = f64(np.broadcast_to(np.asarray(xF, float).reshape(-1, 12), (B, 12)))
     ob = f64(np.asarray(obs, float).reshape(5, 6))
     feas = np.zeros(B, np.int32); worst = np.zeros(B)
-    o = opts if opts is not None else _lib.default_opts()
-    check(lib().obca_check_quadcopter_mixed(C.c_int(B), ptr(Ns), C.c_int(Nmax), ptr(xx), ptr(uu), ptr(tt), ptr(x0), ptr(xF), ptr(Tsb),
-                                            ptr(ll), ptr(ob), C.c_double(R), C.byref(o), ptr(feas), ptr(worst)))
+    check(lib().obca_check_quadcopter_mixed(B, ptr(Ns), Nmax, ptr(xx), ptr(uu), ptr(tt), ptr(x0), ptr(xF), ptr(Tsb), ptr(ll), ptr(ob),
+                                            float(R), opts_arg(opts), ptr(feas), ptr(worst)))
     return feas, worst
 
 

@@ -28,27 +28,17 @@ def arg_index(fn, param):
     return names.index(param)
 
 
-class _Nulling:
-    """A function of libobca.so called with NULL for some of its parameters."""
-
-    def __init__(self, fn, pos):
-        object.__setattr__(self, "_fn", fn)
-        object.__setattr__(self, "_pos", pos)
-
-    def __setattr__(self, key, value):      # argtypes / restype set by a wrapper go to the real function
-        setattr(self._fn, key, value)
-
-    def __call__(self, *args):
-        return self._fn(*[None if i in self._pos else a for i, a in enumerate(args)])
-
-
 class _Lib:
+    """libobca.so with its function fn called with NULL for some of its parameters."""
+
     def __init__(self, real, fn, params):
         self._real, self._fn, self._pos = real, fn, {arg_index(fn, p) for p in params}
 
     def __getattr__(self, name):
         f = getattr(self._real, name)
-        return _Nulling(f, self._pos) if name == self._fn else f
+        if name != self._fn:
+            return f
+        return lambda *args: f(*[None if i in self._pos else a for i, a in enumerate(args)])
 
 
 def with_null(monkeypatch, lib, fn, params, call):

@@ -152,11 +152,9 @@ def test_cloud_entry_argument_errors():
 def _goals_call(lib, B=1, x0=True, xF=True, ob=True, n_ob=None, Ts=0.6, sampleN=3, cap=16):
     a = np.zeros(64); i = np.zeros(8, np.int32)
     p = lambda v: v.ctypes.data_as(C.c_void_p)
-    f = lib.obca_plan_parking_warmstart_goals
-    f.restype = C.c_int
-    f.argtypes = [C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 10
-    return f(B, p(a) if x0 else None, p(a) if xF else None, p(a) if ob else None, p(a), 4 if n_ob is None else n_ob, Ts, 2.7, sampleN, 0, 0,
-             cap, None, p(a), p(a), p(a), p(a), p(a), p(i), p(i), None, None)
+    return lib.obca_plan_parking_warmstart_goals(B, p(a) if x0 else None, p(a) if xF else None, p(a) if ob else None, p(a),
+                                                 4 if n_ob is None else n_ob, Ts, 2.7, sampleN, 0, 0, cap, None, p(a), p(a), p(a), p(a), p(a),
+                                                 p(i), p(i), None, None)
 
 
 def test_goals_cabi_argument_errors_and_no_device():

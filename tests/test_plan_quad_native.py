@@ -209,11 +209,8 @@ def test_emulated_device_search_mixed_batch_equals_host_library():
 def _call(lib, B=1, s=True, ob=True, n_ob=1, reso=1.0, cap=8, max_nodes=0, out=True):
     a = np.zeros(64); i = np.zeros(8, np.int32)
     p = lambda v: v.ctypes.data_as(C.c_void_p)
-    f = lib.obca_plan_quadcopter_warmstart_batch
-    f.restype = C.c_int
-    f.argtypes = [C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_int] + [C.c_void_p] * 8
-    return f(B, p(a) if s else None, p(a), p(a) if ob else None, p(a), p(a), n_ob, p(a), p(a), reso, max_nodes, cap, None,
-             p(a) if out else None, p(a), p(a), p(i), p(i), None, None)
+    return lib.obca_plan_quadcopter_warmstart_batch(B, p(a) if s else None, p(a), p(a) if ob else None, p(a), p(a), n_ob, p(a), p(a), reso,
+                                                    max_nodes, cap, None, p(a) if out else None, p(a), p(a), p(i), p(i), None, None)
 
 
 def test_cabi_argument_errors_and_no_device():
