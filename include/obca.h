@@ -32,6 +32,26 @@
  *     every compute entry point returns OBCA_ERR_NO_DEVICE.
  *   - `*_dev` variants take DEVICE pointers (cudaMalloc'ed by the caller on opts->device) and enqueue on the
  *     library's stream of that device; they return after the stream has been synchronised.
+ *
+ * Device-pointer entries on the caller's stream
+ *   obca_parking_solve_mixed_dev, obca_dualmultws_batch_dev, obca_check_parking_dev, obca_check_parking_mixed_dev,
+ *   obca_quadcopter_solve_batch_dev, obca_quadcopter_solve_mixed_dev, obca_check_quadcopter_dev, obca_check_quadcopter_mixed_dev
+ *   take the arguments of their host-pointer twin (the name without _dev), in its order and with its shapes, layout and nullability,
+ *   and one more, `stream`.  Every per-problem array (inputs and outputs, Nb and Tsb included) is a device pointer on opts->device;
+ *   the scene data (vOb, A, b, ego, XYbounds, ob), opts and solve_seconds stay host pointers.
+ *   - stream: a cudaStream_t of opts->device; NULL is that device's default stream.  On entry the library records an event on
+ *     `stream` and its own stream waits for it, so work enqueued on `stream` before the call has finished before any input is read.
+ *     The entry returns once the library's stream has finished: the outputs are then ready for any stream.  No entry synchronises
+ *     the device or waits for work on any other stream.  (obca_parking_solve_batch_dev predates this and takes no stream: it runs
+ *     on the library's stream only.)
+ *   - Each writes bit for bit what its twin writes for the same inputs and options: every output over each problem's own horizon,
+ *     exitflag (the quadcopter's 2 included), iters, kkt_err, feasible, e, strict, worst, DualMultWS's lp, np and d; and
+ *     obca_last_times / obca_last_profile / obca_last_schedule report the call as they report the twin's.
+ *   - The mixed entries write nothing past a problem's own horizon in the caller's arrays.
+ *   - Refusals: the twin's checks with its messages and codes -- a null argument, a shape error, a horizon bound (OBCA_ERR_UNSUPPORTED)
+ *     -- on the host, before any device work.  Nb and Tsb are in device memory: they are checked on the device (one small kernel and
+ *     an 8-byte readback) after the wait and before anything is written; a bad entry returns OBCA_ERR_ARG with the twin's message
+ *     (e.g. "Nb[37] = 1 outside [2, Nmax = 80]") and no output touched.  Without a CUDA device: OBCA_ERR_NO_DEVICE.
  */
 #ifndef OBCA_H
 #define OBCA_H
@@ -126,11 +146,25 @@ int obca_parking_solve_mixed(int B, const int* Nb, int Nmax, int nOb, const int*
                              double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                              double* solve_seconds);
 
+/* obca_parking_solve_mixed on device pointers (Nb included), on the caller's stream: see "Device-pointer entries" above. */
+int obca_parking_solve_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
+                                 const double* x0, const double* xF, double Ts, double L, const double* ego,
+                                 const double* XYbounds, const double* rx, const double* ry, const double* ryaw,
+                                 const double* xWS, const double* uWS, const double* lWS, const double* nWS,
+                                 int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
+                                 double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
+                                 double* solve_seconds, void* stream);
+
 /* Batched DualMultWS (DualMultWS.jl:29; `ego` is a global there, :39).  lp (N+1)xV, np (N+1)x4nOb per problem
  * (already transposed like :81-84); d (N+1)xnOb optional (optimal objective = ego/obstacle distance). */
 int obca_dualmultws_batch(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* ego,
                           const double* rx, const double* ry, const double* ryaw, const obca_opts* opts, double* lp,
                           double* np, double* d);
+
+/* obca_dualmultws_batch on device pointers (rx, ry, ryaw, lp, np, d), on the caller's stream. */
+int obca_dualmultws_batch_dev(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* ego,
+                              const double* rx, const double* ry, const double* ryaw, const obca_opts* opts, double* lp,
+                              double* np, double* d, void* stream);
 
 /* Batched ParkingConstraints (ParkingConstraints.jl:29-149), restated verbatim including its quirks
  * (SURVEY.md A.4-Q3).  x 4x(N+1), u 2xN, l Vx(N+1), n 4nOb x(N+1), timeScale (N+1).
@@ -149,6 +183,18 @@ int obca_check_parking_mixed(int B, const int* Nb, int Nmax, int nOb, const int*
                              const double* XYbounds, const double* x, const double* u, const double* l, const double* n,
                              const double* timeScale, const double* sl, int fixTime, int sd, const obca_opts* opts,
                              int* feasible, int* e, int* strict);
+
+/* obca_check_parking and obca_check_parking_mixed on device pointers (Nb, x0 ... sl, feasible, e, strict), on the caller's stream. */
+int obca_check_parking_dev(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* x0,
+                           const double* xF, double Ts, double L, const double* ego, const double* XYbounds,
+                           const double* x, const double* u, const double* l, const double* n, const double* timeScale,
+                           const double* sl, int fixTime, int sd, const obca_opts* opts, int* feasible, int* e,
+                           int* strict, void* stream);
+int obca_check_parking_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
+                                 const double* x0, const double* xF, double Ts, double L, const double* ego,
+                                 const double* XYbounds, const double* x, const double* u, const double* l, const double* n,
+                                 const double* timeScale, const double* sl, int fixTime, int sd, const obca_opts* opts,
+                                 int* feasible, int* e, int* strict, void* stream);
 
 /* Batched QuadcopterSignedDist (signed_dist=1, QuadcopterNavigation/QuadcopterSignedDist.jl:25-300, called from
  * mainQuadcopter.jl:152) / QuadcopterDist (signed_dist=0, QuadcopterDist.jl:25-282, mainQuadcopter.jl:145).
@@ -192,6 +238,23 @@ int obca_quadcopter_solve_mixed(int B, const int* Nb, int Nmax, const double* x0
 int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x, const double* u, const double* timeScale,
                                 const double* x0, const double* xF, const double* Tsb, const double* lambda,
                                 const double* ob, double R, const obca_opts* opts, int* feasible, double* worst);
+
+/* The quadcopter solves and checkers on device pointers (Nb, Tsb, x0, xF, xWS and every output but solve_seconds; the checkers' x ... lambda,
+ * feasible and worst), on the caller's stream. */
+int obca_quadcopter_solve_batch_dev(int B, int N, const double* x0, const double* xF, double Ts, double R, const double* ob,
+                                    const double* xWS, double timeWS, int signed_dist, const obca_opts* opts, double* xp,
+                                    double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters,
+                                    double* kkt_err, double* solve_seconds, void* stream);
+int obca_quadcopter_solve_mixed_dev(int B, const int* Nb, int Nmax, const double* x0, const double* xF, const double* Tsb,
+                                    double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
+                                    const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
+                                    int* exitflag, int* iters, double* kkt_err, double* solve_seconds, void* stream);
+int obca_check_quadcopter_dev(int B, int N, const double* x, const double* u, const double* timeScale, const double* x0,
+                              const double* xF, double Ts, const double* lambda, const double* ob, double R,
+                              const obca_opts* opts, int* feasible, double* worst, void* stream);
+int obca_check_quadcopter_mixed_dev(int B, const int* Nb, int Nmax, const double* x, const double* u, const double* timeScale,
+                                    const double* x0, const double* xF, const double* Tsb, const double* lambda,
+                                    const double* ob, double R, const obca_opts* opts, int* feasible, double* worst, void* stream);
 
 /* Hybrid A* warm starts on the GPU: B start poses x0 and a goal per pose xF (both 3 x B column-major: x, y, yaw) among the obstacle
  * points (ox[i], oy[i]), i < n_ob, in ONE call -- main.jl:215-248 for each pose, as obca_plan_warmstart_cloud_batch of

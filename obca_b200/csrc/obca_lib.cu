@@ -8,6 +8,7 @@
 //   k_check                  K5: ParkingConstraints twin + strict audit, one CTA per problem.
 //   k_flow_list, k_flow_gather, k_flow_scatter   the index maps of obca_parking_plan_solve_goals (obca_flow.h): plans -> solve -> poses
 //   k_qflow_gather, k_qflow_scatter              the same for obca_quadcopter_plan_solve (obca_qflow.h), with k_flow_list
+//   k_check_batch_args       the device-pointer mixed entries' check of the per-problem horizons and sampling times in device memory
 // There is NO CPU fallback: every compute entry point returns OBCA_ERR_NO_DEVICE without a CUDA device.
 // Host-pointer entries stage their arrays through one device buffer per device (DevCtx::stage), laid out, copied and scattered back
 // with the helpers of obca_devstage.h, which the GPU planners (obca_plan.cu, obca_plan3d.cu) use for their per-call buffers too.
@@ -313,6 +314,19 @@ __global__ void k_quad_check(const __grid_constant__ QuadProblem P, int B, const
   }
 }
 
+// The device-pointer entries' check of a device-resident batch (obca_*_mixed_dev): the first problem i whose horizon Nb[i] lies
+// outside [2, Nmax], or (Tsb not null) whose sampling time Tsb[i] is not a finite number > 0, as the key (order << 32) | Nb[i] in
+// *first_bad, which starts at ~0.  order = i for a bad horizon and B + i for a bad sampling time: a bad horizon anywhere in the batch
+// comes first, as the host-pointer entries check all horizons before any sampling time.
+__global__ void k_check_batch_args(int B, const int* __restrict__ Nb, int Nmax, const double* __restrict__ Tsb,
+                                   unsigned long long* __restrict__ first_bad) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)B; i += (size_t)gridDim.x * blockDim.x) {
+    const int n = Nb[i];
+    if (n < 2 || n > Nmax) atomicMin(first_bad, (unsigned long long)i << 32 | (unsigned)n);
+    if (Tsb && !(isfinite(Tsb[i]) && Tsb[i] > 0.0)) atomicMin(first_bad, (unsigned long long)(B + i) << 32);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
@@ -324,6 +338,8 @@ struct DevCtx {
   bool init = false;
   cudaStream_t st = nullptr;
   cudaEvent_t ev0 = nullptr, evm = nullptr, ev1 = nullptr;
+  cudaEvent_t evs = nullptr;                        // device-pointer entries: recorded on the caller's stream, waited for on st
+  unsigned long long* bad = nullptr;                // k_check_batch_args: the first bad problem of a device-resident batch
   int sms = 0;
   double* W = nullptr; size_t Wbytes = 0;
   int* counter = nullptr;
@@ -362,6 +378,8 @@ static int get_ctx(int dev, DevCtx** out) {
     cudaDeviceProp pr;
     CK(cudaGetDeviceProperties(&pr, dev));
     c.sms = pr.multiProcessorCount;
+    CK(cudaEventCreateWithFlags(&c.evs, cudaEventDisableTiming));
+    CK(cudaMalloc(&c.bad, sizeof(unsigned long long)));
     CK(cudaMalloc(&c.counter, sizeof(int)));
     CK(cudaMalloc(&c.prof, 8 * sizeof(unsigned long long)));
     CK(cudaMalloc(&c.ncnt, 6 * sizeof(int)));
@@ -738,14 +756,22 @@ static int parking_solve_dev(int B, int N, const int* Nb, int nOb, const int* vO
   return solve_dev_impl(*c, P, O, bp, solve_seconds);
 }
 
+// The refusal of problem q's horizon n outside [2, Nmax] and of its sampling time t (not finite and > 0), for host- and device-resident
+// batches alike.
+static int bad_horizon(int q, int n, int Nmax) {
+  set_err("Nb[" + std::to_string(q) + "] = " + std::to_string(n) + " outside [2, Nmax = " + std::to_string(Nmax) + "]");
+  return OBCA_ERR_ARG;
+}
+static int bad_sampling_time(int q, double t) {
+  set_err("Tsb[" + std::to_string(q) + "] = " + std::to_string(t) + " is not a finite sampling time > 0");
+  return OBCA_ERR_ARG;
+}
+
 // per-problem horizons: Nb[b] in [2, Nmax]
 static int check_horizons(int B, const int* Nb, int Nmax) {
   if (!Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
   for (int q = 0; q < B; ++q)
-    if (Nb[q] < 2 || Nb[q] > Nmax) {
-      set_err("Nb[" + std::to_string(q) + "] = " + std::to_string(Nb[q]) + " outside [2, Nmax = " + std::to_string(Nmax) + "]");
-      return OBCA_ERR_ARG;
-    }
+    if (Nb[q] < 2 || Nb[q] > Nmax) return bad_horizon(q, Nb[q], Nmax);
   return 0;
 }
 
@@ -753,10 +779,7 @@ static int check_horizons(int B, const int* Nb, int Nmax) {
 static int check_sampling_times(int B, const double* Tsb) {
   if (!Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
   for (int q = 0; q < B; ++q)
-    if (!(std::isfinite(Tsb[q]) && Tsb[q] > 0.0)) {
-      set_err("Tsb[" + std::to_string(q) + "] = " + std::to_string(Tsb[q]) + " is not a finite sampling time > 0");
-      return OBCA_ERR_ARG;
-    }
+    if (!(std::isfinite(Tsb[q]) && Tsb[q] > 0.0)) return bad_sampling_time(q, Tsb[q]);
   return 0;
 }
 
@@ -1056,6 +1079,127 @@ static int quad_check_host(int B, int N, const int* Nb, const double* Tsb, const
   if (rc) return rc;
   CK(lay.copy_out(st));
   CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// ---- device-pointer entries, ordered after the work the caller enqueued on its stream -------------------------------------------------
+
+// The library's stream waits for what the caller enqueued on `stream` (a cudaStream_t of the context's device; null: its default stream)
+// before the call: nothing the library enqueues after this reads an input before the caller's producers have finished.
+static int wait_caller_stream(DevCtx& c, void* stream) {
+  CK(cudaEventRecord(c.evs, (cudaStream_t)stream));
+  CK(cudaStreamWaitEvent(c.st, c.evs, 0));
+  return 0;
+}
+
+// check_horizons and (Tsb not null) check_sampling_times for device-resident Nb and Tsb, with their messages: k_check_batch_args on the
+// library's stream, then one 8-byte readback decides (a refused sampling time reads its value back for the message).  Runs before any
+// output is written.
+static int check_batch_args_dev(DevCtx& c, int B, const int* Nb, int Nmax, const double* Tsb) {
+  CK(cudaMemsetAsync(c.bad, 0xff, sizeof(unsigned long long), c.st));
+  const int threads = 256, need = (int)(((size_t)B + threads - 1) / threads), blocks = need < 4 * c.sms ? need : 4 * c.sms;
+  k_check_batch_args<<<blocks, threads, 0, c.st>>>(B, Nb, Nmax, Tsb, c.bad);
+  CK(cudaGetLastError());
+  unsigned long long bad = 0;
+  CK(to_host(&bad, c.bad, 1, c.st));
+  CK(cudaStreamSynchronize(c.st));
+  if (bad == ~0ull) return 0;
+  const long long order = (long long)(bad >> 32);
+  if (order < B) return bad_horizon((int)order, (int)(unsigned)bad, Nmax);
+  const int q = (int)(order - B);
+  double t = 0.0;
+  CK(to_host(&t, Tsb + q, 1, c.st));
+  CK(cudaStreamSynchronize(c.st));
+  return bad_sampling_time(q, t);
+}
+
+// obca_check_parking_dev (Nb null) and obca_check_parking_mixed_dev: the refusals of obca_check_parking[_mixed] in their order, then
+// ParkingConstraints on the caller's device arrays.
+static int check_parking_entry_dev(bool mixed, int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b,
+                                   const double* x0, const double* xF, double Ts, double L, const double* ego, const double* XYbounds,
+                                   const double* x, const double* u, const double* l, const double* n, const double* timeScale,
+                                   const double* sl, int fixTime, int sd, const obca_opts* opts, int* feasible, int* e, int* strict,
+                                   void* stream) {
+  if (mixed && !Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
+  if (B <= 0 || !vOb || !A || !b || !x0 || !xF || !ego || !XYbounds || !x || !u || !l || !n || !timeScale || !feasible) {
+    set_err("null argument"); return OBCA_ERR_ARG;
+  }
+  ParkProblem P;
+  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sd)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
+  DevCtx* c;
+  int rc = get_ctx(opts ? opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  rc = wait_caller_stream(*c, stream);
+  if (rc) return rc;
+  rc = mixed ? check_batch_args_dev(*c, B, Nb, N, nullptr) : 0;
+  if (rc) return rc;
+  rc = check_parking_dev(*c, P, B, Nb, x0, xF, x, u, l, n, timeScale, sl, sd, feasible, e, strict);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(c->st));
+  return 0;
+}
+
+// obca_quadcopter_solve_batch_dev (Nb, Tsb null) and obca_quadcopter_solve_mixed_dev: the refusals of quad_solve_host in its order,
+// then the solve on the caller's device arrays, reported as quad_solve_host reports it.
+static int quad_solve_entry_dev(bool mixed, int B, int N, const int* Nb, const double* Tsb, const double* x0, const double* xF, double Ts,
+                                double R, const double* ob, const double* xWS, double timeWS, int signed_dist, const obca_opts* opts,
+                                double* xp, double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters, double* kkt_err,
+                                double* solve_seconds, void* stream) {
+  if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
+    set_err("null argument"); return OBCA_ERR_ARG;
+  }
+  if (mixed && !Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
+  if (mixed && !Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
+  QuadProblem P;
+  if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  int rc = check_quad_horizon(N);
+  if (rc) return rc;
+  DevCtx* c;
+  rc = get_ctx(opts ? opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  rc = wait_caller_stream(*c, stream);
+  if (rc) return rc;
+  rc = mixed ? check_batch_args_dev(*c, B, Nb, N, Tsb) : 0;
+  if (rc) return rc;
+  IpmOpts O = to_ipm(opts);
+  if (!opts) O.max_iter = 3000;                        // as quad_solve_host
+  QBatchPtrs bp;
+  bp.x0 = x0; bp.xF = xF; bp.xWS = xWS; bp.Nb = mixed ? Nb : nullptr; bp.Tsb = mixed ? Tsb : nullptr;
+  bp.timeWS = timeWS; bp.xp = xp; bp.up = up; bp.ts = ts; bp.lp = lp; bp.slack = signed_dist ? slack : nullptr;
+  bp.exitflag = exitflag; bp.iters = iters; bp.kkt_err = kkt_err; bp.B = B;
+  rc = quad_solve_dev(*c, P, O, bp);
+  if (rc) return rc;
+  CK(to_host(c->prof_host, c->prof, 8, c->st));
+  CK(cudaStreamSynchronize(c->st));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+  if (solve_seconds) *solve_seconds = ms * 1e-3;
+  return 0;
+}
+
+// obca_check_quadcopter_dev (Nb, Tsb null) and obca_check_quadcopter_mixed_dev: the refusals of obca_check_quadcopter[_mixed] in their
+// order, then constrSatisfaction on the caller's device arrays.
+static int quad_check_entry_dev(bool mixed, int B, int N, const int* Nb, const double* Tsb, const double* x, const double* u,
+                                const double* timeScale, const double* x0, const double* xF, double Ts, const double* lambda,
+                                const double* ob, double R, const obca_opts* opts, int* feasible, double* worst, void* stream) {
+  if (mixed && !Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
+  if (mixed && !Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
+  if (B <= 0 || !x || !u || !timeScale || !x0 || !xF || !lambda || !ob || !feasible) { set_err("null argument"); return OBCA_ERR_ARG; }
+  QuadProblem P;
+  if (fill_quad_problem(P, N, Ts, R, ob, 0)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  DevCtx* c;
+  int rc = get_ctx(opts ? opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  rc = wait_caller_stream(*c, stream);
+  if (rc) return rc;
+  rc = mixed ? check_batch_args_dev(*c, B, Nb, N, Tsb) : 0;
+  if (rc) return rc;
+  rc = quad_check_dev(*c, P, B, Nb, Tsb, x0, xF, x, u, timeScale, lambda, feasible, worst);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(c->st));
   return 0;
 }
 
@@ -1559,6 +1703,100 @@ int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x,
   rc = check_sampling_times(B, Tsb);
   if (rc) return rc;
   return quad_check_host(B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst);
+}
+
+int obca_parking_solve_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
+                                 const double* x0, const double* xF, double Ts, double L, const double* ego,
+                                 const double* XYbounds, const double* rx, const double* ry, const double* ryaw,
+                                 const double* xWS, const double* uWS, const double* lWS, const double* nWS,
+                                 int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
+                                 double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
+                                 double* solve_seconds, void* stream) {
+  // the refusals of obca_parking_solve_mixed in its order (the horizons' values are checked on the device below)
+  if (B <= 0 || !vOb || !A || !b || !ego || !XYbounds || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up ||
+      !ts || !lp || !np || !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
+  if (!Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
+  ParkProblem P;
+  if (const int e_ = fill_problem(P, Nmax, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
+  int rc = check_park_horizon(Nmax);
+  if (rc) return rc;
+  DevCtx* c;
+  rc = get_ctx(opts ? opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  rc = wait_caller_stream(*c, stream);
+  if (rc) return rc;
+  rc = check_batch_args_dev(*c, B, Nb, Nmax, nullptr);
+  if (rc) return rc;
+  // the kernels write each problem's outputs over its own horizon only: the caller's arrays need no scatter
+  return parking_solve_dev(B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS, fixTime,
+                           signed_dist, opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds);
+}
+
+int obca_dualmultws_batch_dev(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* ego,
+                              const double* rx, const double* ry, const double* ryaw, const obca_opts* opts, double* lp,
+                              double* np, double* dd, void* stream) {
+  if (B <= 0 || !vOb || !A || !b || !ego || !rx || !ry || !ryaw || !lp || !np) { set_err("null argument"); return OBCA_ERR_ARG; }
+  ParkProblem P;
+  double xy[4] = {0, 1, 0, 1};
+  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, 1.0, 1.0, ego, xy, 0, 1)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
+  DevCtx* c;
+  int rc = get_ctx(opts ? opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  rc = wait_caller_stream(*c, stream);
+  if (rc) return rc;
+  rc = run_dualws(*c, P, B, nullptr, rx, ry, ryaw, lp, np, dd);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(c->st));
+  return 0;
+}
+
+int obca_check_parking_dev(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* x0,
+                           const double* xF, double Ts, double L, const double* ego, const double* XYbounds,
+                           const double* x, const double* u, const double* l, const double* n, const double* timeScale,
+                           const double* sl, int fixTime, int sd, const obca_opts* opts, int* feasible, int* e,
+                           int* strict, void* stream) {
+  return check_parking_entry_dev(false, B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime,
+                                 sd, opts, feasible, e, strict, stream);
+}
+
+int obca_check_parking_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
+                                 const double* x0, const double* xF, double Ts, double L, const double* ego,
+                                 const double* XYbounds, const double* x, const double* u, const double* l, const double* n,
+                                 const double* timeScale, const double* sl, int fixTime, int sd, const obca_opts* opts,
+                                 int* feasible, int* e, int* strict, void* stream) {
+  return check_parking_entry_dev(true, B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime,
+                                 sd, opts, feasible, e, strict, stream);
+}
+
+int obca_quadcopter_solve_batch_dev(int B, int N, const double* x0, const double* xF, double Ts, double R, const double* ob,
+                                    const double* xWS, double timeWS, int signed_dist, const obca_opts* opts, double* xp,
+                                    double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters,
+                                    double* kkt_err, double* solve_seconds, void* stream) {
+  return quad_solve_entry_dev(false, B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
+                              exitflag, iters, kkt_err, solve_seconds, stream);
+}
+
+int obca_quadcopter_solve_mixed_dev(int B, const int* Nb, int Nmax, const double* x0, const double* xF, const double* Tsb,
+                                    double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
+                                    const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
+                                    int* exitflag, int* iters, double* kkt_err, double* solve_seconds, void* stream) {
+  return quad_solve_entry_dev(true, B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
+                              exitflag, iters, kkt_err, solve_seconds, stream);
+}
+
+int obca_check_quadcopter_dev(int B, int N, const double* x, const double* u, const double* timeScale, const double* x0,
+                              const double* xF, double Ts, const double* lambda, const double* ob, double R,
+                              const obca_opts* opts, int* feasible, double* worst, void* stream) {
+  return quad_check_entry_dev(false, B, N, nullptr, nullptr, x, u, timeScale, x0, xF, Ts, lambda, ob, R, opts, feasible, worst, stream);
+}
+
+int obca_check_quadcopter_mixed_dev(int B, const int* Nb, int Nmax, const double* x, const double* u, const double* timeScale,
+                                    const double* x0, const double* xF, const double* Tsb, const double* lambda,
+                                    const double* ob, double R, const obca_opts* opts, int* feasible, double* worst, void* stream) {
+  return quad_check_entry_dev(true, B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst,
+                              stream);
 }
 
 int obca_parking_plan_solve_goals(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts,
