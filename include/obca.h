@@ -169,7 +169,10 @@ int obca_dualmultws_batch_dev(int B, int N, int nOb, const int* vOb, const doubl
 /* Batched ParkingConstraints (ParkingConstraints.jl:29-149), restated verbatim including its quirks
  * (SURVEY.md A.4-Q3).  x 4x(N+1), u 2xN, l Vx(N+1), n 4nOb x(N+1), timeScale (N+1).
  * feasible[B] = the reference's return value (0/1); e[7*B] = its seven pass flags; strict[B] (optional) = a
- * checker without the quirks: every dynamics row, every obstacle, box bounds, slack-aware distance row. */
+ * checker without the quirks: every dynamics row, every obstacle, box bounds, slack-aware distance row.  e[0] checks
+ * |timeScale - 1| with fixTime = 1 too, as the reference does (:47); strict exempts fixed time from it.
+ * Non-finite inputs: the reference's maximum() propagates NaN, so a group (e flag) that reads a NaN fails, and strict is 0
+ * whenever an entry it reads is NaN.  An infinite entry fails its group, directly or through the NaN it produces. */
 int obca_check_parking(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* x0,
                        const double* xF, double Ts, double L, const double* ego, const double* XYbounds,
                        const double* x, const double* u, const double* l, const double* n, const double* timeScale,
@@ -212,7 +215,11 @@ int obca_quadcopter_solve_batch(int B, int N, const double* x0, const double* xF
 
 /* Batched constrSatisfaction (QuadcopterNavigation/constrSatisfaction.jl:25-204, called from mainQuadcopter.jl:147,154),
  * restated verbatim (tolerance 1e-3, rows for i = 1..N, Dist-variant box on x10, one-sided norm row, quirk Q5).
- * feasible[B] = the reference's Bool; worst[B] (optional) = largest violation found. */
+ * feasible[B] = the reference's Bool; worst[B] (optional) = the largest contribution of the reference's groups: the start and
+ * end state (max |.|), per stage the u and x box groups (1.0 when violated), the 13 dynamics rows with the timeScale difference
+ * (max |.|), the 5 norm rows (max), the 5 distance rows (-min), and lambda (-min over the whole matrix); a zero (possibly -0.0) when none is positive.
+ * feasible = worst <= 1e-3.  Non-finite inputs: a test of the reference whose group holds a NaN never fails, so such a group
+ * contributes nothing (a NaN anywhere in lambda turns the lambda group off), while the other groups still decide. */
 int obca_check_quadcopter(int B, int N, const double* x, const double* u, const double* timeScale, const double* x0,
                           const double* xF, double Ts, const double* lambda, const double* ob, double R,
                           const obca_opts* opts, int* feasible, double* worst);

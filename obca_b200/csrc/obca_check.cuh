@@ -9,6 +9,7 @@
 // check_stage_strict(): the same audit without the quirks (all dynamics rows, all obstacles, box bounds,
 // |pp - 1| for the signed-distance variant, slack-aware distance row).
 // Arrays are in the reference's shapes: x 4x(N+1), u 2xN, l Vx(N+1), n 4nOb x(N+1), ts (N+1), column-major.
+// Every max is dmax_nan: a NaN fails its group, as it does through the reference's maximum().
 #pragma once
 #include "obca_common.cuh"
 
@@ -30,9 +31,9 @@ OBCA_HD void chk_init(ChkPart& c) {
 }
 OBCA_HD void chk_merge(ChkPart& a, const ChkPart& b) {
 #pragma unroll
-  for (int i = 0; i < 5; ++i) a.c0[i] = dmax(a.c0[i], b.c0[i]);
-  a.c1 = dmax(a.c1, b.c1); a.c2 = dmax(a.c2, b.c2); a.c3 = dmax(a.c3, b.c3); a.c4 = dmax(a.c4, b.c4);
-  a.c5 = dmax(a.c5, b.c5); a.c6 = dmax(a.c6, b.c6); a.sbox = dmax(a.sbox, b.sbox);
+  for (int i = 0; i < 5; ++i) a.c0[i] = dmax_nan(a.c0[i], b.c0[i]);
+  a.c1 = dmax_nan(a.c1, b.c1); a.c2 = dmax_nan(a.c2, b.c2); a.c3 = dmax_nan(a.c3, b.c3); a.c4 = dmax_nan(a.c4, b.c4);
+  a.c5 = dmax_nan(a.c5, b.c5); a.c6 = dmax_nan(a.c6, b.c6); a.sbox = dmax_nan(a.sbox, b.sbox);
 }
 
 OBCA_HD void chk_dyn(const ParkProblem& P, const double* xk, const double* uk, double tsk, double* f) {
@@ -60,7 +61,7 @@ OBCA_HD void check_stage(const ParkProblem& P, int N, int k, const double* x0, c
     chk_dyn(P, xk, uk, ts[k], f);
     const double* xn = x + 4 * (k + 1);
     if (P.fix_time || strict) {
-      c.c3 = dmax(dmax(dabs(xn[0] - f[0]), dabs(xn[1] - f[1])), dmax(dabs(xn[2] - f[2]), dabs(xn[3] - f[3])));
+      c.c3 = dmax_nan(dmax_nan(dabs(xn[0] - f[0]), dabs(xn[1] - f[1])), dmax_nan(dabs(xn[2] - f[2]), dabs(xn[3] - f[3])));
     } else {
       c.c3 = dabs(xn[3] - f[3]);                       // ParkingConstraints.jl:76-79 (last assignment wins)
     }
@@ -69,11 +70,11 @@ OBCA_HD void check_stage(const ParkProblem& P, int N, int k, const double* x0, c
     c.c5 = dabs(uk[0] - up1);                          // :88/:92, scaled by the caller
     if (strict) c.c5 /= (P.fix_time ? P.Ts : ts[k] * P.Ts);
   }
-  c.c0[2] = P.fix_time ? 0.0 : dabs(ts[k] - 1.0);
-  for (int r = 0; r < P.V; ++r) c.c0[3] = dmax(c.c0[3], -l[(size_t)P.V * k + r]);
-  for (int r = 0; r < 4 * P.nOb; ++r) c.c0[4] = dmax(c.c0[4], -n[(size_t)4 * P.nOb * k + r]);
-  if (k == 0) c.c1 = dmax(dmax(dabs(xk[0] - x0[0]), dabs(xk[1] - x0[1])), dmax(dabs(xk[2] - x0[2]), dabs(xk[3] - x0[3])));
-  if (k == N) c.c2 = dmax(dmax(dabs(xk[0] - xF[0]), dabs(xk[1] - xF[1])), dmax(dabs(xk[2] - xF[2]), dabs(xk[3] - xF[3])));
+  c.c0[2] = P.fix_time && strict ? 0.0 : dabs(ts[k] - 1.0);   // :47 checks timeScale with fixed time too; the strict audit does not
+  for (int r = 0; r < P.V; ++r) c.c0[3] = dmax_nan(c.c0[3], -l[(size_t)P.V * k + r]);
+  for (int r = 0; r < 4 * P.nOb; ++r) c.c0[4] = dmax_nan(c.c0[4], -n[(size_t)4 * P.nOb * k + r]);
+  if (k == 0) c.c1 = dmax_nan(dmax_nan(dabs(xk[0] - x0[0]), dabs(xk[1] - x0[1])), dmax_nan(dabs(xk[2] - x0[2]), dabs(xk[3] - x0[3])));
+  if (k == N) c.c2 = dmax_nan(dmax_nan(dabs(xk[0] - xF[0]), dabs(xk[1] - xF[1])), dmax_nan(dabs(xk[2] - xF[2]), dabs(xk[3] - xF[3])));
   double sn_, cs_;
   sincos(xk[2], &sn_, &cs_);
   const int j0 = strict ? 0 : P.nOb - 1;
@@ -92,17 +93,17 @@ OBCA_HD void check_stage(const ParkProblem& P, int N, int k, const double* x0, c
                   (xk[1] + sn_ * P.off) * p2 - bl;
     if (strict && sd && sl) dist += sl[(size_t)P.nOb * k + j];
     const double c64 = -dist + P.dmin;                                                    // :127-128
-    c.c6 = dmax(c.c6, dmax(dmax(c61, c62), dmax(c63, c64)));
+    c.c6 = dmax_nan(c.c6, dmax_nan(dmax_nan(c61, c62), dmax_nan(c63, c64)));
   }
   if (strict && k >= 1 && k <= N - 1) {
-    c.sbox = dmax(dmax(P.xyb[0] - xk[0], xk[0] - P.xyb[1]), dmax(P.xyb[2] - xk[1], xk[1] - P.xyb[3]));
-    c.sbox = dmax(c.sbox, dmax(-1.0 - xk[3], xk[3] - 2.0));
+    c.sbox = dmax_nan(dmax_nan(P.xyb[0] - xk[0], xk[0] - P.xyb[1]), dmax_nan(P.xyb[2] - xk[1], xk[1] - P.xyb[3]));
+    c.sbox = dmax_nan(c.sbox, dmax_nan(-1.0 - xk[3], xk[3] - 2.0));
   }
 }
 
 // final flags from the merged partials.  e[0..6] = ParkingConstraints.jl:133-139.  returns sum(e) == 7.
 OBCA_HD int check_finish(const ParkProblem& P, const ChkPart& c, const double* ts, int strict, double tol, int* e) {
-  const double c0 = dmax(dmax(c.c0[0] - 0.6, c.c0[1] - 0.4), dmax(dmax(c.c0[2] - 0.2, c.c0[3]), c.c0[4]));
+  const double c0 = dmax_nan(dmax_nan(c.c0[0] - 0.6, c.c0[1] - 0.4), dmax_nan(dmax_nan(c.c0[2] - 0.2, c.c0[3]), c.c0[4]));
   double c5;
   if (strict) c5 = c.c5 - 0.6;
   else c5 = c.c5 / (P.fix_time ? P.Ts : ts[0] * P.Ts) - 0.6;

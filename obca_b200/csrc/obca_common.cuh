@@ -91,6 +91,10 @@ OBCA_HD double rcp(double x) { return 1.0 / x; }
 #endif
 
 OBCA_HD double dmax(double a, double b) { return a > b ? a : b; }
+// The checkers' max: NaN wins, like Julia's maximum() in the references they restate (dmax drops a NaN in its first argument).
+// Equal to dmax whenever neither argument is NaN; commutative and associative (up to the sign of a zero), so a
+// reduction's result does not depend on its order.
+OBCA_HD double dmax_nan(double a, double b) { return a > b || a != a ? a : b; }
 OBCA_HD double dmin_(double a, double b) { return a < b ? a : b; }
 OBCA_HD double dabs(double a) { return a < 0 ? -a : a; }
 

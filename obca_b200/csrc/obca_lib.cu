@@ -293,20 +293,27 @@ __global__ void k_quad_check(const __grid_constant__ QuadProblem P, int B, const
                              const double* __restrict__ x0, const double* __restrict__ xF, const double* __restrict__ x,
                              const double* __restrict__ u, const double* __restrict__ ts, const double* __restrict__ lam,
                              int* __restrict__ feasible, double* __restrict__ worst_out) {
-  __shared__ double s_w[4];
+  __shared__ double s_w[4], s_l[4];
   const int N = P.N, NS = N + 1;
   for (int b = blockIdx.x; b < B; b += gridDim.x) {
     const int Np = Nb ? Nb[b] : N;
     const double Tsp = Tsb ? Tsb[b] : P.Ts;
-    double w = 0.0;
-    for (int k = threadIdx.x; k <= Np; k += blockDim.x)
+    double w = 0.0, wl = -1e300;      // the stages' groups; the lambda group, max(-lambda) over all columns (NaN if one is NaN)
+    for (int k = threadIdx.x; k <= Np; k += blockDim.x) {
+      double lk;
       w = fmax(w, quad_check_stage(P, Np, Tsp, k, x0 + 12 * (size_t)b, xF + 12 * (size_t)b, x + (size_t)12 * NS * b, u + (size_t)4 * N * b,
-                                   ts + (size_t)NS * b, lam + (size_t)30 * NS * b));
-    for (int off = 16; off > 0; off >>= 1) w = fmax(w, __shfl_down_sync(0xffffffffu, w, off));
-    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = w;
+                                   ts + (size_t)NS * b, lam + (size_t)30 * NS * b, &lk));
+      wl = dmax_nan(wl, lk);
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+      w = fmax(w, __shfl_down_sync(0xffffffffu, w, off));
+      wl = dmax_nan(wl, __shfl_down_sync(0xffffffffu, wl, off));
+    }
+    if ((threadIdx.x & 31) == 0) { s_w[threadIdx.x >> 5] = w; s_l[threadIdx.x >> 5] = wl; }
     __syncthreads();
     if (threadIdx.x == 0) {
-      for (int i = 1; i < (int)(blockDim.x >> 5); ++i) w = fmax(w, s_w[i]);
+      for (int i = 1; i < (int)(blockDim.x >> 5); ++i) { w = fmax(w, s_w[i]); wl = dmax_nan(wl, s_l[i]); }
+      if (wl == wl) w = fmax(w, wl);      // a NaN anywhere in lambda turns the lambda group off (:162), not the others
       feasible[b] = w <= 1e-3 ? 1 : 0;
       if (worst_out) worst_out[b] = w;
     }

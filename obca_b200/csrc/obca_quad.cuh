@@ -1111,43 +1111,70 @@ struct QuadSolver {
 // K5 (quadcopter): twin of QuadcopterNavigation/constrSatisfaction.jl:25-204, restated verbatim: tolerance 1e-3,
 // rows checked for i = 1..N only (:80), state box of the Dist variant ([-1.5, 3] on x10, :107,:119) for both
 // variants, norm row one-sided (<= 0, :166-176), quirk Q5 in the body-rate rows (:151-153).
-// x 12x(N+1), u 4xN, ts (N+1), lambda 30x(N+1) column-major.  Returns the worst violation per stage in `v`
-// (<= 1e-3 everywhere  <=>  the reference returns true).  N, Ts: the problem's own horizon and sampling time (P.N is the
+// x 12x(N+1), u 4xN, ts (N+1), lambda 30x(N+1) column-major.  N, Ts: the problem's own horizon and sampling time (P.N is the
 // layout's horizon of a batch, P.Ts its shared sampling time).
+// The reference tests groups: maximum(group) > tol, minimum(group) < -tol, norm(group, Inf) > tol.  A group that holds a NaN has a
+// NaN maximum and never fails, but the other groups still decide.  So each group is reduced with dmax_nan and a NaN group
+// contributes nothing.  Returns the largest contribution of stage k's groups: the start (k = 0) or end (k = N) state, and for
+// k < N the four box groups (1.0 when violated: they fail at any violation), the 13 dynamics rows with the timeScale difference,
+// the 5 norm rows and the 5 distance rows.  The lambda group (:162) spans every column of lambda; *lam gets column k's part of
+// it, max(-lambda[:, k]) with NaN propagated, and the caller adds max(-lambda) over all columns unless it is NaN.
+// (<= 1e-3 everywhere  <=>  the reference returns true.)
 // ------------------------------------------------------------------------------------------------------------
 OBCA_HD double quad_check_stage(const QuadProblem& P, int N, double Ts, int k, const double* x0, const double* xF, const double* x,
-                                const double* u, const double* ts, const double* lam) {
+                                const double* u, const double* ts, const double* lam, double* lamk) {
   double worst = 0.0;
-  if (k == 0)
-    for (int i = 0; i < QNX; ++i) worst = dmax(worst, dabs(x[i] - x0[i]));                          // :56-61
+  const double* lk = lam + (size_t)30 * k;
+  double ln = -lk[0];
+  for (int r = 1; r < 30; ++r) ln = dmax_nan(ln, -lk[r]);
+  *lamk = ln;
+  const double* xk = x + (size_t)QNX * k;
+  if (k == 0) {
+    double g = dabs(xk[0] - x0[0]);
+    for (int i = 1; i < QNX; ++i) g = dmax_nan(g, dabs(xk[i] - x0[i]));                          // :56-61
+    if (g == g) worst = dmax(worst, g);
+  }
   if (k == N) {
-    for (int i = 0; i < QNX; ++i) worst = dmax(worst, dabs(x[(size_t)QNX * N + i] - xF[i]));       // :63-68
-    for (int r = 0; r < 30; ++r) worst = dmax(worst, -lam[(size_t)30 * N + r]);                     // :162 looks at ALL columns
+    double g = dabs(xk[0] - xF[0]);
+    for (int i = 1; i < QNX; ++i) g = dmax_nan(g, dabs(xk[i] - xF[i]));                          // :63-68
+    if (g == g) worst = dmax(worst, g);
     return worst;
   }
-  const double* xk = x + (size_t)QNX * k;
   const double* uk = u + (size_t)QNU * k;
   const double lo[QNX] = {0, 0, 0, -3, -0.2, -0.2, -1, -1, -1, -1.5, -1, -1};                       // :107
   const double hi[QNX] = {10, 10, 5, 3, 0.2, 0.2, 1, 1, 1, 3, 1, 1};                                // :119
-  // the box rows are hard (> 0 fails, :84,:97,:108,:120): scale them so that "any violation" exceeds 1e-3
-  for (int j = 0; j < QNU; ++j) {
-    if (1.2 - uk[j] > 0.0 || uk[j] - 7.8 > 0.0) worst = dmax(worst, 1.0);
-  }
-  for (int i = 0; i < QNX; ++i)
-    if (lo[i] - xk[i] > 0.0 || xk[i] - hi[i] > 0.0) worst = dmax(worst, 1.0);
+  // the box groups are hard (> 0 fails, :83,:95,:108,:120): a violated one contributes 1.0, above the tolerance
+  double gl = 1.2 - uk[0], gh = uk[0] - 7.8;
+  for (int j = 1; j < QNU; ++j) { gl = dmax_nan(gl, 1.2 - uk[j]); gh = dmax_nan(gh, uk[j] - 7.8); }
+  if (gl > 0.0 || gh > 0.0) worst = dmax(worst, 1.0);
+  gl = lo[0] - xk[0]; gh = xk[0] - hi[0];
+  for (int i = 1; i < QNX; ++i) { gl = dmax_nan(gl, lo[i] - xk[i]); gh = dmax_nan(gh, xk[i] - hi[i]); }
+  if (gl > 0.0 || gh > 0.0) worst = dmax(worst, 1.0);
   double f[QNX];
   const double c0[3] = {x[9], x[10], x[11]};                                                         // linear indexing, :151-153
   quad_dyn_f(xk, uk, ts[k], Ts, c0, f);
-  for (int i = 0; i < QNX; ++i) worst = dmax(worst, dabs(x[(size_t)QNX * (k + 1) + i] - f[i]));      // :127-153
-  worst = dmax(worst, dabs(ts[k] - ts[k + 1]));                                                      // :154
+  double g = dabs(x[(size_t)QNX * (k + 1)] - f[0]);
+  for (int i = 1; i < QNX; ++i) g = dmax_nan(g, dabs(x[(size_t)QNX * (k + 1) + i] - f[i]));         // :127-153
+  g = dmax_nan(g, dabs(ts[k] - ts[k + 1]));                                                          // :154
+  if (g == g) worst = dmax(worst, g);
+  double gn = -1e300, gd = -1e300;
   for (int o = 0; o < QNOB; ++o) {
-    const double* l = lam + (size_t)30 * k + 6 * o;
+    const double* l = lk + 6 * o;
     double bl = 0.0;
-    for (int r = 0; r < 6; ++r) { bl += P.obs[o][r] * l[r]; worst = dmax(worst, -l[r]); }            // :162 (lambda >= -1e-3)
+    for (int r = 0; r < 6; ++r) bl += P.obs[o][r] * l[r];
     const double p0 = l[0] - l[3], p1 = l[1] - l[4], p2 = l[2] - l[5];
-    worst = dmax(worst, p0 * p0 + p1 * p1 + p2 * p2 - 1.0);                                          // :171-180 (one-sided)
-    worst = dmax(worst, -(-bl + xk[0] * p0 + xk[1] * p1 + xk[2] * p2 - P.R));                        // :187-200
+    gn = dmax_nan(gn, p0 * p0 + p1 * p1 + p2 * p2 - 1.0);                                           // :171-182 (one-sided)
+    // the distance row sums A[j, c] * l[j] over all six j (A = [I; -I]) like :185-194: equal to p on finite multipliers, NaN where an
+    // infinite multiplier meets a zero of A
+    double a[3];
+    for (int c = 0; c < 3; ++c) {
+      a[c] = 0.0;
+      for (int r = 0; r < 6; ++r) a[c] += (r == c ? 1.0 : r == c + 3 ? -1.0 : 0.0) * l[r];
+    }
+    gd = dmax_nan(gd, -(-bl + xk[0] * a[0] + xk[1] * a[1] + xk[2] * a[2] - P.R));                   // :185-199
   }
+  if (gn == gn) worst = dmax(worst, gn);
+  if (gd == gd) worst = dmax(worst, gd);
   return worst;
 }
 

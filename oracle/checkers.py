@@ -65,9 +65,15 @@ def ParkingConstraints(x0, xF, N, Ts, L, ego, XYbounds, nOb, vOb, A, b, x, u, l,
     return (ok, e) if return_e else ok
 
 
+def _nanmax(*v):
+    """max that propagates NaN, like Julia's maximum (the built-in max(0.0, nan) is 0.0)."""
+    return float(np.max(np.array(v, float)))
+
+
 def strict_check(x0, xF, N, Ts, L, ego, XYbounds, nOb, vOb, A, b, x, u, l, n, timeScale, fixTime, sd, sl=None,
                  tol=5e-5):
-    """Quirk-free audit: every dynamics row, every obstacle, box bounds, |pp-1| (sd) and slack-aware distance."""
+    """Quirk-free audit: every dynamics row, every obstacle, box bounds, |pp-1| (sd) and slack-aware distance.  Returns (ok, worst);
+    a NaN in any value it reads makes worst NaN and ok 0."""
     x0 = np.asarray(x0, float).ravel(); xF = np.asarray(xF, float).ravel()
     x = np.asarray(x, float); u = np.asarray(u, float); l = np.asarray(l, float); n = np.asarray(n, float)
     ts = np.asarray(timeScale, float).ravel()
@@ -79,13 +85,13 @@ def strict_check(x0, xF, N, Ts, L, ego, XYbounds, nOb, vOb, A, b, x, u, l, n, ti
     vm = x[3, :N] + h / 2 * u[1]; th = x[2, :N] + h / 2 * x[3, :N] * np.tan(u[0]) / L
     f = np.stack([x[0, :N] + h * vm * np.cos(th), x[1, :N] + h * vm * np.sin(th), x[2, :N] + h * vm * np.tan(u[0]) / L,
                   x[3, :N] + h * u[1]])
-    worst = max(worst, np.abs(x[:, 1:] - f).max(), np.abs(x[:, 0] - x0).max(), np.abs(x[:, N] - xF).max())
-    worst = max(worst, np.abs(u[0]).max() - 0.6, np.abs(u[1]).max() - 0.4, -l.min(), -n.min())
+    worst = _nanmax(worst, np.abs(x[:, 1:] - f).max(), np.abs(x[:, 0] - x0).max(), np.abs(x[:, N] - xF).max())
+    worst = _nanmax(worst, np.abs(u[0]).max() - 0.6, np.abs(u[1]).max() - 0.4, -l.min(), -n.min())
     if not fixTime:
-        worst = max(worst, np.abs(ts - 1).max() - 0.2, np.abs(np.diff(ts)).max())
-    worst = max(worst, (np.abs(np.diff(np.concatenate([[0.0], u[0]]))) / h).max() - 0.6)
+        worst = _nanmax(worst, np.abs(ts - 1).max() - 0.2, np.abs(np.diff(ts)).max())
+    worst = _nanmax(worst, (np.abs(np.diff(np.concatenate([[0.0], u[0]]))) / h).max() - 0.6)
     xi = x[:, 1:N]
-    worst = max(worst, (XYb[0] - xi[0]).max(), (xi[0] - XYb[1]).max(), (XYb[2] - xi[1]).max(), (xi[1] - XYb[3]).max(),
+    worst = _nanmax(worst, (XYb[0] - xi[0]).max(), (xi[0] - XYb[1]).max(), (XYb[2] - xi[1]).max(), (xi[1] - XYb[3]).max(),
                 (-1 - xi[3]).max(), (xi[3] - 2).max())
     g = np.array([(ego[0] + ego[2]) / 2, (ego[1] + ego[3]) / 2, (ego[0] + ego[2]) / 2, (ego[1] + ego[3]) / 2])
     offset = (ego[0] + ego[2]) / 2 - ego[2]
@@ -94,12 +100,12 @@ def strict_check(x0, xF, N, Ts, L, ego, XYbounds, nOb, vOb, A, b, x, u, l, n, ti
     for j in range(nOb):
         Aj = A[off[j]:off[j + 1]]; lj = l[off[j]:off[j + 1]]; nj = n[4 * j:4 * j + 4]; bj = b[off[j]:off[j + 1]]
         p1 = Aj[:, 0] @ lj; p2 = Aj[:, 1] @ lj; pp = p1 ** 2 + p2 ** 2
-        worst = max(worst, (np.abs(pp - 1) if sd else pp - 1).max())
-        worst = max(worst, np.abs(nj[0] - nj[2] + c * p1 + s * p2).max(), np.abs(nj[1] - nj[3] - s * p1 + c * p2).max())
+        worst = _nanmax(worst, (np.abs(pp - 1) if sd else pp - 1).max())
+        worst = _nanmax(worst, np.abs(nj[0] - nj[2] + c * p1 + s * p2).max(), np.abs(nj[1] - nj[3] - s * p1 + c * p2).max())
         dist = -g @ nj + (x[0] + c * offset) * p1 + (x[1] + s * offset) * p2 - bj @ lj
         if sd and sl is not None:
             dist = dist + np.asarray(sl, float)[j]
-        worst = max(worst, (0.05 - dist).max())
+        worst = _nanmax(worst, (0.05 - dist).max())
     return (1 if worst <= tol else 0), worst
 
 
@@ -146,3 +152,60 @@ def constrSatisfaction(x, u, timeScale, x0, xF, Ts, lam, ob1, ob2, ob3, ob4, ob5
                        for l, b in zip(ls, bs)])
         if t2.min() < -1e-3: return False
     return True
+
+
+def quad_dynamics_rows(x, u, ts, Ts, i):
+    """The 13 dynamics rows of constrSatisfaction.jl:135-154 at stage i (0-based), quirk Q5 included: x[9..11] of stage 0 in the
+    body-rate rows.  x 12x(N+1), u 4xN, ts (N+1)."""
+    mass, g = 0.5, 9.81
+    k_F, k_M = 0.0611, 0.0015
+    I = np.array([3.9, 4.4, 4.9]) * 1e-3
+    L = 0.225
+    xl = x.ravel(order="F")
+    h = ts[i] * Ts
+    F = k_F * (u[:, i] ** 2).sum()
+    xi = x[:, i]
+    s = np.zeros(13)
+    s[0] = x[0, i + 1] - (xi[0] + h * xi[6]); s[1] = x[1, i + 1] - (xi[1] + h * xi[7]); s[2] = x[2, i + 1] - (xi[2] + h * xi[8])
+    s[3] = x[3, i + 1] - (xi[3] + h * (np.cos(xi[4]) * xi[9] + np.sin(xi[4]) * xi[11]))
+    s[4] = x[4, i + 1] - (xi[4] + h * (np.sin(xi[4]) * np.tan(xi[3]) * xi[9] + xi[10] - np.cos(xi[4]) * np.tan(xi[3]) * xi[11]))
+    s[5] = x[5, i + 1] - (xi[5] + h * (-np.sin(xi[4]) / np.cos(xi[3]) * xi[9] + np.cos(xi[4]) / np.cos(xi[3]) * xi[11]))
+    s[6] = x[6, i + 1] - (xi[6] + h / mass * (F * (np.sin(xi[3]) * np.cos(xi[4]) * np.sin(xi[5]) + np.sin(xi[4]) * np.cos(xi[5]))))
+    s[7] = x[7, i + 1] - (xi[7] + h / mass * (F * (-np.sin(xi[3]) * np.cos(xi[4]) * np.cos(xi[5]) + np.sin(xi[4]) * np.sin(xi[5]))))
+    s[8] = x[8, i + 1] - (xi[8] + h / mass * (F * (np.cos(xi[3]) * np.cos(xi[4])) - mass * g))
+    s[9] = x[9, i + 1] - (xi[9] + h / I[0] * (L * k_F * (u[1, i] ** 2 - u[3, i] ** 2) - (I[2] - I[1]) * xl[10] * xl[11]))
+    s[10] = x[10, i + 1] - (xi[10] + h / I[1] * (L * k_F * (u[2, i] ** 2 - u[0, i] ** 2) - (I[0] - I[2]) * xl[9] * xl[11]))
+    s[11] = x[11, i + 1] - (xi[11] + h / I[2] * (k_M * (u[0, i] ** 2 - u[1, i] ** 2 + u[2, i] ** 2 - u[3, i] ** 2) - (I[1] - I[0]) * xl[9] * xl[10]))
+    s[12] = ts[i] - ts[i + 1]
+    return s
+
+
+def constr_worst(x, u, timeScale, x0, xF, Ts, lam, ob1, ob2, ob3, ob4, ob5, R):
+    """The `worst` of the quadcopter checker, group by group from constrSatisfaction.jl:25-204 like constrSatisfaction above:
+    the largest contribution of its groups, where a group is what one test of the reference reads (start, end; per stage i = 1..N
+    the u lower / upper and x lower / upper boxes, which contribute 1.0 when violated, the 13 dynamics rows, the 5 norm rows, the
+    negated 5 distance rows; the negated lambda matrix, once).  A group whose value is NaN never fails in the reference and
+    contributes nothing here.  constr_worst(...) <= 1e-3 is constrSatisfaction(...)."""
+    x = np.asarray(x, float); u = np.asarray(u, float); ts = np.asarray(timeScale, float).ravel(); lam = np.asarray(lam, float)
+    x0 = np.asarray(x0, float).ravel(); xF = np.asarray(xF, float).ravel()
+    ls = [lam[6 * o:6 * o + 6] for o in range(5)]
+    bs = [np.asarray(b, float).ravel() for b in (ob1, ob2, ob3, ob4, ob5)]
+    N = x.shape[1] - 1
+    A = np.vstack([np.eye(3), -np.eye(3)])
+    lo = np.array([0, 0, 0, -3, -0.2, -0.2, -1, -1, -1, -1.5, -1, -1.0]); hi = np.array([10, 10, 5, 3, 0.2, 0.2, 1, 1, 1, 3, 1, 1.0])
+    worst = [0.0]
+    add = lambda v: worst.append(float(v)) if not np.isnan(v) else None
+    add(np.abs(x[:, 0] - x0).max())                                  # :56-61
+    add(np.abs(x[:, -1] - xF).max())                                 # :63-68
+    add(-lam.min())                                                  # :162, the whole matrix at every i
+    for i in range(N):
+        for grp in (1.2 - u[:, i], u[:, i] - 7.8, lo - x[:, i], x[:, i] - hi):      # :83, :95, :108, :120
+            if grp.max() > 0:
+                add(1.0)
+        xi = x[:, i]
+        s = quad_dynamics_rows(x, u, ts, Ts, i)
+        add(np.abs(s).max())                                         # :156
+        add(np.array([(l[0, i] - l[3, i]) ** 2 + (l[1, i] - l[4, i]) ** 2 + (l[2, i] - l[5, i]) ** 2 - 1 for l in ls]).max())   # :178
+        add(-np.array([-(b @ l[:, i]) + xi[0] * (A[:, 0] @ l[:, i]) + xi[1] * (A[:, 1] @ l[:, i]) + xi[2] * (A[:, 2] @ l[:, i]) - R
+                       for l, b in zip(ls, bs)]).min())              # :195
+    return max(worst)
