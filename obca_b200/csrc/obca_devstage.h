@@ -7,6 +7,7 @@
 
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/obca.h"
@@ -47,7 +48,7 @@ class DevLayout {
   template <class T>
   void add(T*& d, size_t n) { record(d, n, nullptr, nullptr); }
   template <class T>
-  void in(T*& d, const T* h, size_t n) { record(d, n, h, nullptr); }
+  void in(T*& d, const std::remove_const_t<T>* h, size_t n) { record(d, n, h, nullptr); }      // d may be a pointer to const
   template <class T>
   void out(T*& d, T* h, size_t n) { record(d, n, nullptr, h); }
   template <class T>

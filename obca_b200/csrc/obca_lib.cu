@@ -10,8 +10,12 @@
 //   k_qflow_gather, k_qflow_scatter              the same for obca_quadcopter_plan_solve (obca_qflow.h), with k_flow_list
 //   k_check_batch_args       the device-pointer mixed entries' check of the per-problem horizons and sampling times in device memory
 // There is NO CPU fallback: every compute entry point returns OBCA_ERR_NO_DEVICE without a CUDA device.
-// Host-pointer entries stage their arrays through one device buffer per device (DevCtx::stage), laid out, copied and scattered back
-// with the helpers of obca_devstage.h, which the GPU planners (obca_plan.cu, obca_plan3d.cu) use for their per-call buffers too.
+// Each solve and check family (parking solve, DualMultWS, parking check, quadcopter solve, quadcopter check) passes its arguments as one
+// struct to one entry function, shared by its host-pointer entries and their device-pointer twins: the refusals in one order, the device
+// context and lock once, the host staging or the wait on the caller's stream, then the family's device core, which the
+// plan -> solve -> check flows call directly.  Host-pointer entries stage their arrays through one device buffer per device
+// (DevCtx::stage), laid out, copied and scattered back with the helpers of obca_devstage.h, which the GPU planners (obca_plan.cu,
+// obca_plan3d.cu) use for their per-call buffers too.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -637,6 +641,19 @@ static int launch_phased(DevCtx& c, const ParkProblem& P, const IpmOpts& O, cons
   return 0;
 }
 
+// Elements per problem of a batch's per-problem arrays laid out for the horizon N, for the host code (staging, chunks, scratch, the
+// flows' layouts): ns = N + 1 (stages: time scales, reference path), then states, inputs, multipliers and slacks.
+struct ParkSizes { size_t ns, x, u, l, n, sl; };      // N + 1, 4 (N + 1), 2N, V (N + 1), 4 nOb (N + 1), nOb (N + 1)
+static ParkSizes park_sizes(int N, int V, int nOb) {
+  const size_t ns = (size_t)N + 1;
+  return {ns, 4 * ns, 2 * (size_t)N, V * ns, 4 * (size_t)nOb * ns, nOb * ns};
+}
+struct QuadSizes { size_t ns, x, u, l, s; };          // N + 1, 12 (N + 1), 4N, 30 (N + 1), 5 (N + 1)
+static QuadSizes quad_sizes(int N) {
+  const size_t ns = (size_t)N + 1;
+  return {ns, 12 * ns, 4 * (size_t)N, 30 * ns, 5 * ns};
+}
+
 static int solve_dev_impl(DevCtx& c, const ParkProblem& P, const IpmOpts& O, BatchPtrs bp, double* seconds) {
   // problem, options and workspace layout -> __constant__ memory (stream-ordered with the kernels below)
   const PkLay Lc = make_layout(P, nfac_for(P));
@@ -652,17 +669,17 @@ static int solve_dev_impl(DevCtx& c, const ParkProblem& P, const IpmOpts& O, Bat
   // INTEGRATION.md section 3a) stays within a few GB.  Past NSP = 128 doubles per row the chunk shrinks with the row length, so
   // that no shape needs more memory per chunk than it does at N = 127.
   const int chunk = env_int("OBCA_CHUNK", Lc.NSP > 128 ? 16384 * 128 / Lc.NSP : 16384);
-  const int NSc = P.N + 1, Vc = P.V, nObc = P.nOb;
+  const ParkSizes z = park_sizes(P.N, P.V, P.nOb);
   rc = 0;
   for (int b0 = 0; b0 < bp.B && rc == 0; b0 += chunk) {
     BatchPtrs q = bp;
     q.B = bp.B - b0 < chunk ? bp.B - b0 : chunk;
     const size_t o = (size_t)b0;
-    q.x0 += 4 * o; q.xF += 4 * o; q.rx += NSc * o; q.ry += NSc * o; q.ryaw += NSc * o; q.xWS += 4 * NSc * o; q.uWS += 2 * (size_t)P.N * o;
-    q.lWS += (size_t)Vc * NSc * o; q.nWS += (size_t)4 * nObc * NSc * o;
-    q.xp += 4 * NSc * o; q.up += 2 * (size_t)P.N * o; q.ts += NSc * o; q.lp += (size_t)Vc * NSc * o; q.np += (size_t)4 * nObc * NSc * o;
-    if (q.sl) q.sl += (size_t)nObc * NSc * o;
-    if (q.duals) q.duals += ((size_t)4 * P.N + (size_t)4 * nObc * NSc) * o;
+    q.x0 += 4 * o; q.xF += 4 * o; q.rx += z.ns * o; q.ry += z.ns * o; q.ryaw += z.ns * o; q.xWS += z.x * o; q.uWS += z.u * o;
+    q.lWS += z.l * o; q.nWS += z.n * o;
+    q.xp += z.x * o; q.up += z.u * o; q.ts += z.ns * o; q.lp += z.l * o; q.np += z.n * o;
+    if (q.sl) q.sl += z.sl * o;
+    if (q.duals) q.duals += ((size_t)4 * P.N + z.n) * o;
     if (q.Nb) q.Nb += o;
     q.exitflag += o; q.iters += o; q.kkt_err += o;
 #ifdef OBCA_FAST_BUILD   // development builds: only the config-2 instantiation
@@ -722,45 +739,12 @@ static int check_park_horizon(int N) {
   return OBCA_ERR_UNSUPPORTED;
 }
 
-// The parking solve behind the device- and host-pointer entries.  Every per-problem array is laid out for the horizon N;
-// Nb (device pointer, optional): per-problem horizons <= N, problem b uses the first Nb[b] + 1 stages of its arrays.
-static int parking_solve_dev(int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b,
-                             const double* x0, const double* xF, double Ts, double L, const double* ego,
-                             const double* XYbounds, const double* rx, const double* ry, const double* ryaw,
-                             const double* xWS, const double* uWS, const double* lWS, const double* nWS,
-                             int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up,
-                             double* ts, double* lp, double* np, double* sl, int* exitflag, int* iters,
-                             double* kkt_err, double* solve_seconds) {
-  if (B <= 0 || !vOb || !A || !b || !x0 || !xF || !ego || !XYbounds || !rx || !ry || !ryaw || !xWS || !uWS || !xp ||
-      !up || !ts || !lp || !np || !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
-  ParkProblem P;
-  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
-  int rc = check_park_horizon(N);
-  if (rc) return rc;
-  DevCtx* c;
-  rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  IpmOpts O = to_ipm(opts);
-  BatchPtrs bp;
-  bp.x0 = x0; bp.xF = xF; bp.rx = rx; bp.ry = ry; bp.ryaw = ryaw; bp.xWS = xWS; bp.uWS = uWS; bp.Nb = Nb;
-  bp.xp = xp; bp.up = up; bp.ts = ts; bp.lp = lp; bp.np = np; bp.sl = sl; bp.duals = nullptr;
-  bp.exitflag = exitflag; bp.iters = iters; bp.kkt_err = kkt_err; bp.B = B; bp.retry = opts ? opts->retry : 1;
-  bp.q4 = opts ? opts->q4 : 0;
-  CK(cudaEventRecord(c->ev0, c->st));
-  if (lWS && nWS) { bp.lWS = lWS; bp.nWS = nWS; }
-  else {
-    // the reference runs DualMultWS inside the NLP driver (ParkingSignedDist.jl:219); its result goes to a scratch of
-    // the library (never to the caller's output arrays, which stay untouched until a problem has finished)
-    const size_t NS = (size_t)N + 1, nl = (size_t)P.V * NS * B, nn = 4 * (size_t)nOb * NS * B;
-    rc = ensure((void**)&c->wsd, &c->wsd_bytes, (nl + nn) * sizeof(double));
-    if (rc) return rc;
-    rc = run_dualws(*c, P, B, Nb, rx, ry, ryaw, c->wsd, c->wsd + nl, nullptr);
-    if (rc) return rc;
-    bp.lWS = c->wsd; bp.nWS = c->wsd + nl;
-  }
-  CK(cudaEventRecord(c->evm, c->st));      // `time` = the solve alone, as in the reference (:239-241); see obca_last_times
-  return solve_dev_impl(*c, P, O, bp, solve_seconds);
+// The quadcopter solver's horizon bound, checked before any device work: a refused call launches nothing and writes no output.
+static int check_quad_horizon(int N) {
+  if (N <= QUAD_NMAX) return 0;
+  set_err("horizon too long for the quadcopter solver: N = " + std::to_string(N) + " > " + std::to_string(QUAD_NMAX) +
+          " (N + 1 <= " + std::to_string(QUAD_NMAX + 1) + " stages)");
+  return OBCA_ERR_UNSUPPORTED;
 }
 
 // The refusal of problem q's horizon n outside [2, Nmax] and of its sampling time t (not finite and > 0), for host- and device-resident
@@ -774,328 +758,19 @@ static int bad_sampling_time(int q, double t) {
   return OBCA_ERR_ARG;
 }
 
-// per-problem horizons: Nb[b] in [2, Nmax]
-static int check_horizons(int B, const int* Nb, int Nmax) {
+// per-problem horizons: Nb present and, in host memory, every Nb[q] in [2, Nmax] (in device memory: check_batch_args_dev)
+static int check_horizons(int B, const int* Nb, int Nmax, bool on_host) {
   if (!Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
-  for (int q = 0; q < B; ++q)
+  for (int q = 0; on_host && q < B; ++q)
     if (Nb[q] < 2 || Nb[q] > Nmax) return bad_horizon(q, Nb[q], Nmax);
   return 0;
 }
 
-// per-problem sampling times: finite and > 0
-static int check_sampling_times(int B, const double* Tsb) {
+// per-problem sampling times: Tsb present and, in host memory, every Tsb[q] finite and > 0 (in device memory: check_batch_args_dev)
+static int check_sampling_times(int B, const double* Tsb, bool on_host) {
   if (!Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
-  for (int q = 0; q < B; ++q)
+  for (int q = 0; on_host && q < B; ++q)
     if (!(std::isfinite(Tsb[q]) && Tsb[q] > 0.0)) return bad_sampling_time(q, Tsb[q]);
-  return 0;
-}
-
-// Host-pointer parking solve (staged through one device buffer), behind the uniform and the mixed entries.  Every per-problem array
-// is laid out for the horizon N.  mixed: Nb (host pointer) holds per-problem horizons in [2, N]; otherwise Nb is null.
-static int parking_solve_host(bool mixed, int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b,
-                              const double* x0, const double* xF, double Ts, double L, const double* ego,
-                              const double* XYbounds, const double* rx, const double* ry, const double* ryaw,
-                              const double* xWS, const double* uWS, const double* lWS, const double* nWS,
-                              int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
-                              double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
-                              double* solve_seconds) {
-  if (B <= 0 || !vOb || !A || !b || !ego || !XYbounds || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up ||
-      !ts || !lp || !np || !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
-  int rc = mixed ? check_horizons(B, Nb, N) : 0;
-  if (rc) return rc;
-  {   // the shape decides the staging sizes below: checked before anything is sized, copied or written
-    ParkProblem P;
-    if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
-  }
-  rc = check_park_horizon(N);
-  if (rc) return rc;
-  int V = 0;
-  for (int j = 0; j < nOb; ++j) V += vOb[j];
-  DevCtx* c;
-  rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  // elements per problem
-  const size_t Bs = B, NS = N + 1, n_x = 4 * NS, n_u = 2 * (size_t)N, n_l = V * NS, n_n = 4 * (size_t)nOb * NS, n_s = nOb * NS;
-  const bool have_ws = lWS && nWS;
-  double *d0, *dF, *drx, *dry, *dryaw, *dxw, *duw, *dlw, *dnw;
-  double *dxp, *dup, *dts, *dlp, *dnp, *dsl, *derr;
-  int *dflag, *diters, *dNb;
-  char* dout;
-  DevLayout outs;      // the per-problem outputs, copied back in one piece when the horizons differ
-  outs.out(dxp, xp, n_x * Bs);
-  outs.out(dup, up, n_u * Bs);
-  outs.out(dts, ts, NS * Bs);
-  outs.out(dlp, lp, n_l * Bs);
-  outs.out(dnp, np, n_n * Bs);
-  outs.out(dsl, sl, n_s * Bs);
-  outs.out(derr, kkt_err, Bs);
-  DevLayout lay;
-  lay.in(d0, x0, 4 * Bs);
-  lay.in(dF, xF, 4 * Bs);
-  lay.in(drx, rx, NS * Bs);
-  lay.in(dry, ry, NS * Bs);
-  lay.in(dryaw, ryaw, NS * Bs);
-  lay.in(dxw, xWS, n_x * Bs);
-  lay.in(duw, uWS, n_u * Bs);
-  lay.in(dlw, have_ws ? lWS : nullptr, n_l * Bs);
-  lay.in(dnw, have_ws ? nWS : nullptr, n_n * Bs);
-  lay.in(dNb, Nb, Bs);
-  lay.add(dout, outs.bytes);
-  lay.out(dflag, exitflag, Bs);
-  lay.out(diters, iters, Bs);
-  // one staging buffer per device: the whole call (copies in, solve, copies out) runs under the device lock
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
-  if (rc) return rc;
-  lay.place(c->stage);
-  outs.place(dout);
-  cudaStream_t st = c->st;
-  CK(lay.copy_in(st));
-  obca_opts o2;
-  if (opts) o2 = *opts; else obca_default_opts(&o2);
-  rc = parking_solve_dev(B, N, Nb ? dNb : nullptr, nOb, vOb, A, b, d0, dF, Ts, L, ego, XYbounds, drx, dry, dryaw, dxw, duw,
-                         have_ws ? dlw : nullptr, have_ws ? dnw : nullptr, fixTime, signed_dist, &o2, dxp, dup, dts, dlp, dnp, dsl,
-                         dflag, diters, derr, solve_seconds);
-  if (rc) return rc;
-  CK(lay.copy_out(st));
-  if (!Nb) {
-    CK(outs.copy_out(st));
-    CK(cudaStreamSynchronize(st));
-    return 0;
-  }
-  // per-problem horizons: the outputs come back through a host scratch, and only the entries of each problem's own
-  // horizon are copied into the caller's arrays (the padding past it is never written)
-  std::vector<double> h(outs.bytes / sizeof(double));
-  CK(to_host((char*)h.data(), dout, outs.bytes, st));
-  CK(cudaStreamSynchronize(st));
-  scatter_horizons(xp, outs.in_copy(dxp, h.data()), B, Nb, n_x, 4, 1);
-  scatter_horizons(up, outs.in_copy(dup, h.data()), B, Nb, n_u, 2, 0);
-  scatter_horizons(ts, outs.in_copy(dts, h.data()), B, Nb, NS, 1, 1);
-  scatter_horizons(lp, outs.in_copy(dlp, h.data()), B, Nb, n_l, V, 1);
-  scatter_horizons(np, outs.in_copy(dnp, h.data()), B, Nb, n_n, 4 * (size_t)nOb, 1);
-  scatter_horizons(sl, outs.in_copy(dsl, h.data()), B, Nb, n_s, nOb, 1);
-  memcpy(kkt_err, outs.in_copy(derr, h.data()), Bs * sizeof(double));
-  return 0;
-}
-
-// ParkingConstraints over B problems on the device's stream (device pointers, laid out for P.N; Nb, sl, e, strict may be null).
-static int check_parking_dev(DevCtx& c, const ParkProblem& P, int B, const int* Nb, const double* x0, const double* xF, const double* x,
-                             const double* u, const double* l, const double* n, const double* ts, const double* sl, int sd, int* feasible,
-                             int* e, int* strict) {
-  const int grid = B < 4 * c.sms ? B : 4 * c.sms;
-  k_check<<<grid, 128, 0, c.st>>>(P, B, Nb, x0, xF, x, u, l, n, ts, sl, sd, feasible, e, strict);
-  CK(cudaGetLastError());
-  return 0;
-}
-
-// ParkingConstraints over a batch (host pointers).  Nb (host pointer, optional): per-problem horizons <= N, with every
-// per-problem array laid out for N.
-static int check_parking(int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b, const double* x0,
-                         const double* xF, double Ts, double L, const double* ego, const double* XYbounds,
-                         const double* x, const double* u, const double* l, const double* n, const double* timeScale,
-                         const double* sl, int fixTime, int sd, const obca_opts* opts, int* feasible, int* e,
-                         int* strict) {
-  if (B <= 0 || !vOb || !A || !b || !x0 || !xF || !ego || !XYbounds || !x || !u || !l || !n || !timeScale || !feasible) {
-    set_err("null argument"); return OBCA_ERR_ARG;
-  }
-  ParkProblem P;
-  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sd)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
-  DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  const size_t Bs = B, NS = N + 1;
-  const size_t n0 = 4 * Bs, nx = 4 * NS * Bs, nu = 2 * (size_t)N * Bs, nl = (size_t)P.V * NS * Bs, nn = 4 * (size_t)nOb * NS * Bs,
-               nt = NS * Bs, ns = (size_t)nOb * NS * Bs;
-  double *d0, *dF, *dx, *du, *dl, *dn, *dt, *ds;
-  int *dfeas, *de, *dstrict, *dNb;
-  DevLayout lay;
-  lay.in(d0, x0, n0);
-  lay.in(dF, xF, n0);
-  lay.in(dx, x, nx);
-  lay.in(du, u, nu);
-  lay.in(dl, l, nl);
-  lay.in(dn, n, nn);
-  lay.in(dt, timeScale, nt);
-  lay.in(ds, sl, ns);
-  lay.in(dNb, Nb, Bs);
-  lay.out(dfeas, feasible, Bs);
-  lay.out(de, e, 7 * Bs);
-  lay.out(dstrict, strict, Bs);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
-  if (rc) return rc;
-  lay.place(c->stage);
-  cudaStream_t st = c->st;
-  CK(lay.copy_in(st));
-  rc = check_parking_dev(*c, P, B, Nb ? dNb : nullptr, d0, dF, dx, du, dl, dn, dt, sl ? ds : nullptr, sd, dfeas, de, dstrict);
-  if (rc) return rc;
-  CK(lay.copy_out(st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-
-// The quadcopter solver's horizon bound, checked before any device work: a refused call launches nothing and writes no output.
-static int check_quad_horizon(int N) {
-  if (N <= QUAD_NMAX) return 0;
-  set_err("horizon too long for the quadcopter solver: N = " + std::to_string(N) + " > " + std::to_string(QUAD_NMAX) +
-          " (N + 1 <= " + std::to_string(QUAD_NMAX + 1) + " stages)");
-  return OBCA_ERR_UNSUPPORTED;
-}
-
-// The quadcopter solve of a batch on the device's stream (every pointer of bp a device pointer, laid out for P.N), between the events
-// ev0 and ev1 of the context, with the phase counters in c.prof; the caller copies the counters back and reads the time once the stream
-// is synchronised.
-static int quad_solve_dev(DevCtx& c, const QuadProblem& P, const IpmOpts& O, QBatchPtrs bp) {
-  bp.prof = c.prof;
-  CK(cudaMemsetAsync(c.prof, 0, 8 * sizeof(unsigned long long), c.st));
-  CK(cudaEventRecord(c.ev0, c.st));
-  const int rc = P.signed_dist ? launch_quad<true>(c, P, O, bp) : launch_quad<false>(c, P, O, bp);
-  if (rc) return rc;
-  CK(cudaEventRecord(c.ev1, c.st));
-  return 0;
-}
-
-// The quadcopter solve behind the uniform and the mixed entries (host pointers, staged through one device buffer).  Every
-// per-problem array is laid out for the horizon N.  mixed: Nb, Tsb (host pointers) hold per-problem horizons in [2, N] and sampling
-// times; problem b uses the first Nb[b] + 1 stages of its arrays and nothing past them is written.  Otherwise Nb and Tsb are null.
-static int quad_solve_host(bool mixed, int B, int N, const int* Nb, const double* Tsb, const double* x0, const double* xF, double Ts,
-                           double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
-                           const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
-                           int* exitflag, int* iters, double* kkt_err, double* solve_seconds) {
-  if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
-    set_err("null argument"); return OBCA_ERR_ARG;
-  }
-  if (mixed) {
-    int rc = check_horizons(B, Nb, N);
-    if (rc) return rc;
-    rc = check_sampling_times(B, Tsb);
-    if (rc) return rc;
-  }
-  QuadProblem P;
-  if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
-  int rc = check_quad_horizon(N);
-  if (rc) return rc;
-  DevCtx* c;
-  rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  IpmOpts O = to_ipm(opts);
-  if (!opts) O.max_iter = 3000;                        // the reference sets no max_iter here (Ipopt default)
-  // elements per problem
-  const size_t Bs = B, NS = N + 1, n_x = 12 * NS, n_u = 4 * (size_t)N, n_l = 30 * NS, n_s = 5 * NS;
-  double *d0, *dF, *dW, *dTs;
-  double *dxp, *dup, *dts, *dlp, *dsl, *derr;
-  int *dflag, *diters, *dNb;
-  char* dout;
-  double* slack_out = signed_dist ? slack : nullptr;      // the Dist formulation has no slacks
-  DevLayout outs;      // the per-problem outputs, copied back in one piece when the horizons differ
-  outs.out(dxp, xp, n_x * Bs);
-  outs.out(dup, up, n_u * Bs);
-  outs.out(dts, ts, NS * Bs);
-  outs.out(dlp, lp, n_l * Bs);
-  outs.out(dsl, slack_out, n_s * Bs);
-  outs.out(derr, kkt_err, Bs);
-  DevLayout lay;
-  lay.in(d0, x0, 12 * Bs);
-  lay.in(dF, xF, 12 * Bs);
-  lay.in(dW, xWS, n_x * Bs);
-  lay.in(dNb, Nb, Bs);
-  lay.in(dTs, Tsb, Bs);
-  lay.add(dout, outs.bytes);
-  lay.out(dflag, exitflag, Bs);
-  lay.out(diters, iters, Bs);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
-  if (rc) return rc;
-  lay.place(c->stage);
-  outs.place(dout);
-  cudaStream_t st = c->st;
-  CK(lay.copy_in(st));
-  QBatchPtrs bp;
-  bp.x0 = d0; bp.xF = dF; bp.xWS = dW; bp.Nb = Nb ? dNb : nullptr; bp.Tsb = Nb ? dTs : nullptr;
-  bp.timeWS = timeWS; bp.xp = dxp; bp.up = dup; bp.ts = dts; bp.lp = dlp; bp.slack = dsl;
-  bp.exitflag = dflag; bp.iters = diters; bp.kkt_err = derr; bp.B = B;
-  rc = quad_solve_dev(*c, P, O, bp);
-  if (rc) return rc;
-  if (!Nb) CK(outs.copy_out(st));
-  CK(lay.copy_out(st));
-  CK(to_host(c->prof_host, c->prof, 8, st));
-  std::vector<double> h;
-  if (Nb) {     // the outputs come back through a host scratch; only each problem's own horizon goes to the caller's arrays
-    h.resize(outs.bytes / sizeof(double));
-    CK(to_host((char*)h.data(), dout, outs.bytes, st));
-  }
-  CK(cudaStreamSynchronize(st));
-  float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-  if (solve_seconds) *solve_seconds = ms * 1e-3;
-  if (Nb) {
-    scatter_horizons(xp, outs.in_copy(dxp, h.data()), B, Nb, n_x, 12, 1);
-    scatter_horizons(up, outs.in_copy(dup, h.data()), B, Nb, n_u, 4, 0);
-    scatter_horizons(ts, outs.in_copy(dts, h.data()), B, Nb, NS, 1, 1);
-    scatter_horizons(lp, outs.in_copy(dlp, h.data()), B, Nb, n_l, 30, 1);
-    scatter_horizons(slack_out, outs.in_copy(dsl, h.data()), B, Nb, n_s, 5, 1);
-    memcpy(kkt_err, outs.in_copy(derr, h.data()), Bs * sizeof(double));
-  }
-  return 0;
-}
-
-// constrSatisfaction over B problems on the device's stream (device pointers, laid out for P.N; Nb and Tsb together, and worst, may be
-// null).
-static int quad_check_dev(DevCtx& c, const QuadProblem& P, int B, const int* Nb, const double* Tsb, const double* x0, const double* xF,
-                          const double* x, const double* u, const double* ts, const double* lam, int* feasible, double* worst) {
-  const int grid = B < 4 * c.sms ? B : 4 * c.sms;
-  k_quad_check<<<grid, 128, 0, c.st>>>(P, B, Nb, Tsb, x0, xF, x, u, ts, lam, feasible, worst);
-  CK(cudaGetLastError());
-  return 0;
-}
-
-// constrSatisfaction over a batch (host pointers).  Nb, Tsb (host pointers, optional, together): per-problem horizons <= N
-// and sampling times, with every per-problem array laid out for N.
-static int quad_check_host(int B, int N, const int* Nb, const double* Tsb, const double* x, const double* u,
-                           const double* timeScale, const double* x0, const double* xF, double Ts, const double* lambda,
-                           const double* ob, double R, const obca_opts* opts, int* feasible, double* worst) {
-  if (B <= 0 || !x || !u || !timeScale || !x0 || !xF || !lambda || !ob || !feasible) { set_err("null argument"); return OBCA_ERR_ARG; }
-  QuadProblem P;
-  if (fill_quad_problem(P, N, Ts, R, ob, 0)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
-  DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  const size_t Bs = B, NS = N + 1;
-  const size_t n0 = 12 * Bs, nx = 12 * NS * Bs, nu = 4 * (size_t)N * Bs, nt = NS * Bs, nl = 30 * NS * Bs;
-  double *d0, *dF, *dx, *du, *dt, *dl, *dw, *dTs;
-  int *dfeas, *dNb;
-  DevLayout lay;
-  lay.in(d0, x0, n0);
-  lay.in(dF, xF, n0);
-  lay.in(dx, x, nx);
-  lay.in(du, u, nu);
-  lay.in(dt, timeScale, nt);
-  lay.in(dl, lambda, nl);
-  lay.in(dNb, Nb, Bs);
-  lay.in(dTs, Tsb, Bs);
-  lay.out(dfeas, feasible, Bs);
-  lay.out(dw, worst, Bs);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
-  if (rc) return rc;
-  lay.place(c->stage);
-  cudaStream_t st = c->st;
-  CK(lay.copy_in(st));
-  rc = quad_check_dev(*c, P, B, Nb ? dNb : nullptr, Nb ? dTs : nullptr, d0, dF, dx, du, dt, dl, dfeas, dw);
-  if (rc) return rc;
-  CK(lay.copy_out(st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-// ---- device-pointer entries, ordered after the work the caller enqueued on its stream -------------------------------------------------
-
-// The library's stream waits for what the caller enqueued on `stream` (a cudaStream_t of the context's device; null: its default stream)
-// before the call: nothing the library enqueues after this reads an input before the caller's producers have finished.
-static int wait_caller_stream(DevCtx& c, void* stream) {
-  CK(cudaEventRecord(c.evs, (cudaStream_t)stream));
-  CK(cudaStreamWaitEvent(c.st, c.evs, 0));
   return 0;
 }
 
@@ -1120,92 +795,438 @@ static int check_batch_args_dev(DevCtx& c, int B, const int* Nb, int Nmax, const
   return bad_sampling_time(q, t);
 }
 
-// obca_check_parking_dev (Nb null) and obca_check_parking_mixed_dev: the refusals of obca_check_parking[_mixed] in their order, then
-// ParkingConstraints on the caller's device arrays.
-static int check_parking_entry_dev(bool mixed, int B, int N, const int* Nb, int nOb, const int* vOb, const double* A, const double* b,
-                                   const double* x0, const double* xF, double Ts, double L, const double* ego, const double* XYbounds,
-                                   const double* x, const double* u, const double* l, const double* n, const double* timeScale,
-                                   const double* sl, int fixTime, int sd, const obca_opts* opts, int* feasible, int* e, int* strict,
-                                   void* stream) {
-  if (mixed && !Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
-  if (B <= 0 || !vOb || !A || !b || !x0 || !xF || !ego || !XYbounds || !x || !u || !l || !n || !timeScale || !feasible) {
+// Where the arrays of an entry live.  HOST: host memory, staged through the device's staging buffer.  DEV: device memory, read on the
+// library's stream without waiting for any other (obca_parking_solve_batch_dev).  STREAM: device memory, read after the work the caller
+// enqueued on its stream (the *_dev entries with a stream argument).
+enum class Arrays { HOST, DEV, STREAM };
+
+// The start of a host-pointer entry: its layout placed in the device's staging buffer, which only grows (the whole call runs under the
+// device lock), and its inputs copied in.
+static int stage_in(DevCtx& c, DevLayout& lay) {
+  const int rc = ensure((void**)&c.stage, &c.stage_bytes, lay.bytes);
+  if (rc) return rc;
+  lay.place(c.stage);
+  CK(lay.copy_in(c.st));
+  return 0;
+}
+
+// The start of a device-pointer entry, before any output is written.  STREAM: the library's stream waits for what the caller enqueued on
+// `stream` (a cudaStream_t of the context's device; null: its default stream), so that nothing the library enqueues after this reads an
+// input before the caller's producers have finished.  Then a mixed batch's device-resident horizons Nb and (not null) sampling times Tsb
+// are checked.
+static int dev_start(DevCtx& c, Arrays at, void* stream, int B, const int* Nb, int Nmax, const double* Tsb) {
+  if (at == Arrays::STREAM) {
+    CK(cudaEventRecord(c.evs, (cudaStream_t)stream));
+    CK(cudaStreamWaitEvent(c.st, c.evs, 0));
+  }
+  return Nb ? check_batch_args_dev(c, B, Nb, Nmax, Tsb) : 0;
+}
+
+// ---- the solve and check families: one argument struct, one device core and one entry function each ------------------------------------
+// Each struct holds its entries' arguments by name, in their order.  A device core takes the struct with every per-problem array in
+// device memory (the scene is in the problem it is given), checks nothing and takes no lock.  An entry function runs a whole call, with
+// the arrays where `at` says: the refusals in the entries' order (the values of host-resident Nb / Tsb directly after their presence),
+// get_ctx and the device lock, stage_in or dev_start, the core, and for host arrays the copy back.
+
+// obca_parking_solve_batch[_dev] and obca_parking_solve_mixed[_dev].  Every per-problem array is laid out for the horizon N; Nb:
+// per-problem horizons <= N (mixed entries; problem b uses the first Nb[b] + 1 stages of its arrays), else null.
+struct ParkSolve {
+  int B, N;
+  const int* Nb;
+  int nOb;
+  const int* vOb;
+  const double *A, *b, *x0, *xF;
+  double Ts, L;
+  const double *ego, *XYbounds, *rx, *ry, *ryaw, *xWS, *uWS, *lWS, *nWS;
+  int fixTime, signed_dist;
+  const obca_opts* opts;
+  double *xp, *up, *ts, *lp, *np, *sl;
+  int *exitflag, *iters;
+  double *kkt_err, *solve_seconds;
+};
+
+// The parking solve of P: DualMultWS into the library's scratch when lWS / nWS are null, then the solve.  Returns once the device's
+// stream is synchronised.
+static int parking_solve_dev(DevCtx& c, const ParkProblem& P, const ParkSolve& a) {
+  const obca_opts* opts = a.opts;
+  BatchPtrs bp;
+  bp.x0 = a.x0; bp.xF = a.xF; bp.rx = a.rx; bp.ry = a.ry; bp.ryaw = a.ryaw; bp.xWS = a.xWS; bp.uWS = a.uWS; bp.Nb = a.Nb;
+  bp.xp = a.xp; bp.up = a.up; bp.ts = a.ts; bp.lp = a.lp; bp.np = a.np; bp.sl = a.sl; bp.duals = nullptr;
+  bp.exitflag = a.exitflag; bp.iters = a.iters; bp.kkt_err = a.kkt_err; bp.B = a.B; bp.retry = opts ? opts->retry : 1;
+  bp.q4 = opts ? opts->q4 : 0;
+  CK(cudaEventRecord(c.ev0, c.st));
+  if (a.lWS && a.nWS) { bp.lWS = a.lWS; bp.nWS = a.nWS; }
+  else {
+    // the reference runs DualMultWS inside the NLP driver (ParkingSignedDist.jl:219); its result goes to a scratch of
+    // the library (never to the caller's output arrays, which stay untouched until a problem has finished)
+    const ParkSizes z = park_sizes(P.N, P.V, P.nOb);
+    const size_t nl = z.l * a.B, nn = z.n * a.B;
+    int rc = ensure((void**)&c.wsd, &c.wsd_bytes, (nl + nn) * sizeof(double));
+    if (rc) return rc;
+    rc = run_dualws(c, P, a.B, a.Nb, a.rx, a.ry, a.ryaw, c.wsd, c.wsd + nl, nullptr);
+    if (rc) return rc;
+    bp.lWS = c.wsd; bp.nWS = c.wsd + nl;
+  }
+  CK(cudaEventRecord(c.evm, c.st));      // `time` = the solve alone, as in the reference (:239-241); see obca_last_times
+  return solve_dev_impl(c, P, to_ipm(opts), bp, a.solve_seconds);
+}
+
+// mixed: Nb holds per-problem horizons in [2, N].
+static int parking_solve(const ParkSolve& a, Arrays at, bool mixed, void* stream) {
+  const bool host = at == Arrays::HOST;
+  if (a.B <= 0 || !a.vOb || !a.A || !a.b || !a.ego || !a.XYbounds || !a.x0 || !a.xF || !a.rx || !a.ry || !a.ryaw || !a.xWS || !a.uWS ||
+      !a.xp || !a.up || !a.ts || !a.lp || !a.np || !a.exitflag || !a.iters || !a.kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
+  int rc = mixed ? check_horizons(a.B, a.Nb, a.N, host) : 0;
+  if (rc) return rc;
+  // the shape decides the staging sizes below: checked before anything is sized, copied or written
+  ParkProblem P;
+  if (const int e_ = fill_problem(P, a.N, a.nOb, a.vOb, a.A, a.b, a.Ts, a.L, a.ego, a.XYbounds, a.fixTime, a.signed_dist)) {
+    set_err(shape_error(e_)); return OBCA_ERR_ARG;
+  }
+  rc = check_park_horizon(a.N);
+  if (rc) return rc;
+  DevCtx* c;
+  rc = get_ctx(a.opts ? a.opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  const size_t Bs = a.B;
+  const ParkSizes z = park_sizes(a.N, P.V, a.nOb);
+  ParkSolve d = a;      // the call on the staged arrays (host arrays)
+  char* dout = nullptr;
+  DevLayout outs;       // host arrays: the per-problem outputs, copied back in one piece when the horizons differ
+  DevLayout lay;        // host arrays: all of their staging
+  if (host) {
+    const bool have_ws = a.lWS && a.nWS;
+    outs.out(d.xp, a.xp, z.x * Bs);
+    outs.out(d.up, a.up, z.u * Bs);
+    outs.out(d.ts, a.ts, z.ns * Bs);
+    outs.out(d.lp, a.lp, z.l * Bs);
+    outs.out(d.np, a.np, z.n * Bs);
+    outs.out(d.sl, a.sl, z.sl * Bs);
+    outs.out(d.kkt_err, a.kkt_err, Bs);
+    lay.in(d.x0, a.x0, 4 * Bs);
+    lay.in(d.xF, a.xF, 4 * Bs);
+    lay.in(d.rx, a.rx, z.ns * Bs);
+    lay.in(d.ry, a.ry, z.ns * Bs);
+    lay.in(d.ryaw, a.ryaw, z.ns * Bs);
+    lay.in(d.xWS, a.xWS, z.x * Bs);
+    lay.in(d.uWS, a.uWS, z.u * Bs);
+    lay.in(d.lWS, have_ws ? a.lWS : nullptr, z.l * Bs);
+    lay.in(d.nWS, have_ws ? a.nWS : nullptr, z.n * Bs);
+    lay.in(d.Nb, a.Nb, Bs);
+    lay.add(dout, outs.bytes);
+    lay.out(d.exitflag, a.exitflag, Bs);
+    lay.out(d.iters, a.iters, Bs);
+    rc = stage_in(*c, lay);
+    outs.place(dout);
+    if (!have_ws) d.lWS = d.nWS = nullptr;
+    if (!a.Nb) d.Nb = nullptr;
+  } else {
+    rc = dev_start(*c, at, stream, a.B, a.Nb, a.N, nullptr);
+  }
+  if (!rc) rc = parking_solve_dev(*c, P, d);
+  // device arrays: the kernels write each problem's outputs over its own horizon only, so the caller's arrays need no scatter
+  if (rc || !host) return rc;
+  cudaStream_t st = c->st;
+  CK(lay.copy_out(st));
+  if (!mixed) {
+    CK(outs.copy_out(st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  // per-problem horizons: the outputs come back through a host scratch, and only the entries of each problem's own
+  // horizon are copied into the caller's arrays (the padding past it is never written)
+  std::vector<double> h(outs.bytes / sizeof(double));
+  CK(to_host((char*)h.data(), dout, outs.bytes, st));
+  CK(cudaStreamSynchronize(st));
+  scatter_horizons(a.xp, outs.in_copy(d.xp, h.data()), a.B, a.Nb, z.x, 4, 1);
+  scatter_horizons(a.up, outs.in_copy(d.up, h.data()), a.B, a.Nb, z.u, 2, 0);
+  scatter_horizons(a.ts, outs.in_copy(d.ts, h.data()), a.B, a.Nb, z.ns, 1, 1);
+  scatter_horizons(a.lp, outs.in_copy(d.lp, h.data()), a.B, a.Nb, z.l, P.V, 1);
+  scatter_horizons(a.np, outs.in_copy(d.np, h.data()), a.B, a.Nb, z.n, 4 * (size_t)a.nOb, 1);
+  scatter_horizons(a.sl, outs.in_copy(d.sl, h.data()), a.B, a.Nb, z.sl, a.nOb, 1);
+  memcpy(a.kkt_err, outs.in_copy(d.kkt_err, h.data()), Bs * sizeof(double));
+  return 0;
+}
+
+// obca_dualmultws_batch[_dev]: laid out for the horizon N.
+struct DualWs {
+  int B, N, nOb;
+  const int* vOb;
+  const double *A, *b, *ego, *rx, *ry, *ryaw;
+  const obca_opts* opts;
+  double *lp, *np, *dd;
+};
+
+static int dualmultws(const DualWs& a, Arrays at, void* stream) {
+  if (a.B <= 0 || !a.vOb || !a.A || !a.b || !a.ego || !a.rx || !a.ry || !a.ryaw || !a.lp || !a.np) {
     set_err("null argument"); return OBCA_ERR_ARG;
   }
   ParkProblem P;
-  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sd)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
+  const double xy[4] = {0, 1, 0, 1};
+  if (const int e_ = fill_problem(P, a.N, a.nOb, a.vOb, a.A, a.b, 1.0, 1.0, a.ego, xy, 0, 1)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
   DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
+  int rc = get_ctx(a.opts ? a.opts->device : 0, &c);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
-  rc = wait_caller_stream(*c, stream);
+  DualWs d = a;      // the call on the staged arrays (host arrays)
+  DevLayout lay;     // host arrays: their staging
+  if (at == Arrays::HOST) {
+    const size_t Bs = a.B;
+    const ParkSizes z = park_sizes(a.N, P.V, a.nOb);
+    lay.in(d.rx, a.rx, z.ns * Bs);
+    lay.in(d.ry, a.ry, z.ns * Bs);
+    lay.in(d.ryaw, a.ryaw, z.ns * Bs);
+    lay.out(d.lp, a.lp, z.l * Bs);
+    lay.out(d.np, a.np, z.n * Bs);
+    lay.out(d.dd, a.dd, z.sl * Bs);
+    rc = stage_in(*c, lay);
+  } else {
+    rc = dev_start(*c, at, stream, a.B, nullptr, a.N, nullptr);
+  }
+  if (!rc) rc = run_dualws(*c, P, a.B, nullptr, d.rx, d.ry, d.ryaw, d.lp, d.np, d.dd);
   if (rc) return rc;
-  rc = mixed ? check_batch_args_dev(*c, B, Nb, N, nullptr) : 0;
-  if (rc) return rc;
-  rc = check_parking_dev(*c, P, B, Nb, x0, xF, x, u, l, n, timeScale, sl, sd, feasible, e, strict);
-  if (rc) return rc;
+  CK(lay.copy_out(c->st));
   CK(cudaStreamSynchronize(c->st));
   return 0;
 }
 
-// obca_quadcopter_solve_batch_dev (Nb, Tsb null) and obca_quadcopter_solve_mixed_dev: the refusals of quad_solve_host in its order,
-// then the solve on the caller's device arrays, reported as quad_solve_host reports it.
-static int quad_solve_entry_dev(bool mixed, int B, int N, const int* Nb, const double* Tsb, const double* x0, const double* xF, double Ts,
-                                double R, const double* ob, const double* xWS, double timeWS, int signed_dist, const obca_opts* opts,
-                                double* xp, double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters, double* kkt_err,
-                                double* solve_seconds, void* stream) {
-  if (B <= 0 || !x0 || !xF || !ob || !xWS || !xp || !up || !ts || !lp || !exitflag || !iters || !kkt_err) {
+// obca_check_parking[_dev] and obca_check_parking_mixed[_dev].  Every per-problem array is laid out for the horizon N; Nb: per-problem
+// horizons <= N (mixed entries), else null.
+struct ParkCheck {
+  int B, N;
+  const int* Nb;
+  int nOb;
+  const int* vOb;
+  const double *A, *b, *x0, *xF;
+  double Ts, L;
+  const double *ego, *XYbounds, *x, *u, *l, *n, *timeScale, *sl;
+  int fixTime, sd;
+  const obca_opts* opts;
+  int *feasible, *e, *strict;
+};
+
+// ParkingConstraints over the batch on the device's stream (Nb, sl, e, strict may be null).
+static int check_parking_dev(DevCtx& c, const ParkProblem& P, const ParkCheck& a) {
+  const int grid = a.B < 4 * c.sms ? a.B : 4 * c.sms;
+  k_check<<<grid, 128, 0, c.st>>>(P, a.B, a.Nb, a.x0, a.xF, a.x, a.u, a.l, a.n, a.timeScale, a.sl, a.sd, a.feasible, a.e, a.strict);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+static int check_parking(const ParkCheck& a, Arrays at, bool mixed, void* stream) {
+  const bool host = at == Arrays::HOST;
+  int rc = mixed ? check_horizons(a.B, a.Nb, a.N, host) : 0;
+  if (rc) return rc;
+  if (a.B <= 0 || !a.vOb || !a.A || !a.b || !a.x0 || !a.xF || !a.ego || !a.XYbounds || !a.x || !a.u || !a.l || !a.n || !a.timeScale ||
+      !a.feasible) { set_err("null argument"); return OBCA_ERR_ARG; }
+  ParkProblem P;
+  if (const int e_ = fill_problem(P, a.N, a.nOb, a.vOb, a.A, a.b, a.Ts, a.L, a.ego, a.XYbounds, a.fixTime, a.sd)) {
+    set_err(shape_error(e_)); return OBCA_ERR_ARG;
+  }
+  DevCtx* c;
+  rc = get_ctx(a.opts ? a.opts->device : 0, &c);
+  if (rc) return rc;
+  std::lock_guard<std::recursive_mutex> lk(c->mu);
+  ParkCheck d = a;      // the call on the staged arrays (host arrays)
+  DevLayout lay;        // host arrays: their staging
+  if (host) {
+    const size_t Bs = a.B;
+    const ParkSizes z = park_sizes(a.N, P.V, a.nOb);
+    lay.in(d.x0, a.x0, 4 * Bs);
+    lay.in(d.xF, a.xF, 4 * Bs);
+    lay.in(d.x, a.x, z.x * Bs);
+    lay.in(d.u, a.u, z.u * Bs);
+    lay.in(d.l, a.l, z.l * Bs);
+    lay.in(d.n, a.n, z.n * Bs);
+    lay.in(d.timeScale, a.timeScale, z.ns * Bs);
+    lay.in(d.sl, a.sl, z.sl * Bs);
+    lay.in(d.Nb, a.Nb, Bs);
+    lay.out(d.feasible, a.feasible, Bs);
+    lay.out(d.e, a.e, 7 * Bs);
+    lay.out(d.strict, a.strict, Bs);
+    rc = stage_in(*c, lay);
+    if (!a.sl) d.sl = nullptr;
+    if (!a.Nb) d.Nb = nullptr;
+  } else {
+    rc = dev_start(*c, at, stream, a.B, a.Nb, a.N, nullptr);
+  }
+  if (!rc) rc = check_parking_dev(*c, P, d);
+  if (rc) return rc;
+  CK(lay.copy_out(c->st));
+  CK(cudaStreamSynchronize(c->st));
+  return 0;
+}
+
+// obca_quadcopter_solve_batch[_dev] and obca_quadcopter_solve_mixed[_dev].  Every per-problem array is laid out for the horizon N; Nb, Tsb
+// (mixed entries): per-problem horizons <= N and sampling times, problem b uses the first Nb[b] + 1 stages of its arrays and nothing past
+// them is written; otherwise both null.
+struct QuadSolve {
+  int B, N;
+  const int* Nb;
+  const double *Tsb, *x0, *xF;
+  double Ts, R;
+  const double *ob, *xWS;
+  double timeWS;
+  int signed_dist;
+  const obca_opts* opts;
+  double *xp, *up, *ts, *lp, *slack;
+  int *exitflag, *iters;
+  double *kkt_err, *solve_seconds;
+};
+
+// The quadcopter solve of P on the device's stream between the context's events ev0 and ev1, then the phase counters back to prof_host
+// (obca_last_profile).  quad_solve_seconds reads its time once the stream is synchronised.
+static int quad_solve_dev(DevCtx& c, const QuadProblem& P, const QuadSolve& a) {
+  IpmOpts O = to_ipm(a.opts);
+  if (!a.opts) O.max_iter = 3000;                        // the reference sets no max_iter here (Ipopt default)
+  QBatchPtrs bp;
+  bp.x0 = a.x0; bp.xF = a.xF; bp.xWS = a.xWS; bp.Nb = a.Nb; bp.Tsb = a.Tsb;
+  bp.timeWS = a.timeWS; bp.xp = a.xp; bp.up = a.up; bp.ts = a.ts; bp.lp = a.lp;
+  bp.slack = P.signed_dist ? a.slack : nullptr;          // the Dist formulation has no slacks
+  bp.exitflag = a.exitflag; bp.iters = a.iters; bp.kkt_err = a.kkt_err; bp.B = a.B;
+  bp.prof = c.prof;
+  CK(cudaMemsetAsync(c.prof, 0, 8 * sizeof(unsigned long long), c.st));
+  CK(cudaEventRecord(c.ev0, c.st));
+  const int rc = P.signed_dist ? launch_quad<true>(c, P, O, bp) : launch_quad<false>(c, P, O, bp);
+  if (rc) return rc;
+  CK(cudaEventRecord(c.ev1, c.st));
+  CK(to_host(c.prof_host, c.prof, 8, c.st));
+  return 0;
+}
+static int quad_solve_seconds(DevCtx& c, double* seconds) {
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c.ev0, c.ev1));
+  if (seconds) *seconds = ms * 1e-3;
+  return 0;
+}
+
+// mixed: Nb, Tsb hold per-problem horizons in [2, N] and sampling times.
+static int quad_solve(const QuadSolve& a, Arrays at, bool mixed, void* stream) {
+  const bool host = at == Arrays::HOST;
+  if (a.B <= 0 || !a.x0 || !a.xF || !a.ob || !a.xWS || !a.xp || !a.up || !a.ts || !a.lp || !a.exitflag || !a.iters || !a.kkt_err) {
     set_err("null argument"); return OBCA_ERR_ARG;
   }
-  if (mixed && !Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
-  if (mixed && !Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
+  int rc = mixed ? check_horizons(a.B, a.Nb, a.N, host) : 0;
+  if (!rc && mixed) rc = check_sampling_times(a.B, a.Tsb, host);
+  if (rc) return rc;
   QuadProblem P;
-  if (fill_quad_problem(P, N, Ts, R, ob, signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
-  int rc = check_quad_horizon(N);
+  if (fill_quad_problem(P, a.N, a.Ts, a.R, a.ob, a.signed_dist)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  rc = check_quad_horizon(a.N);
   if (rc) return rc;
   DevCtx* c;
-  rc = get_ctx(opts ? opts->device : 0, &c);
+  rc = get_ctx(a.opts ? a.opts->device : 0, &c);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
-  rc = wait_caller_stream(*c, stream);
+  const size_t Bs = a.B;
+  const QuadSizes z = quad_sizes(a.N);
+  const bool scatter = host && mixed;      // host arrays of a mixed batch come back through a host scratch, each problem's horizon only
+  QuadSolve d = a;      // the call on the staged arrays (host arrays)
+  char* dout = nullptr;
+  DevLayout outs;       // host arrays: the per-problem outputs, copied back in one piece when the horizons differ
+  DevLayout lay;        // host arrays: all of their staging
+  if (host) {
+    outs.out(d.xp, a.xp, z.x * Bs);
+    outs.out(d.up, a.up, z.u * Bs);
+    outs.out(d.ts, a.ts, z.ns * Bs);
+    outs.out(d.lp, a.lp, z.l * Bs);
+    outs.out(d.slack, a.signed_dist ? a.slack : nullptr, z.s * Bs);
+    outs.out(d.kkt_err, a.kkt_err, Bs);
+    lay.in(d.x0, a.x0, 12 * Bs);
+    lay.in(d.xF, a.xF, 12 * Bs);
+    lay.in(d.xWS, a.xWS, z.x * Bs);
+    lay.in(d.Nb, a.Nb, Bs);
+    lay.in(d.Tsb, a.Tsb, Bs);
+    lay.add(dout, outs.bytes);
+    lay.out(d.exitflag, a.exitflag, Bs);
+    lay.out(d.iters, a.iters, Bs);
+    rc = stage_in(*c, lay);
+    outs.place(dout);
+    if (!mixed) { d.Nb = nullptr; d.Tsb = nullptr; }
+  } else {
+    rc = dev_start(*c, at, stream, a.B, a.Nb, a.N, a.Tsb);
+  }
+  if (!rc) rc = quad_solve_dev(*c, P, d);
   if (rc) return rc;
-  rc = mixed ? check_batch_args_dev(*c, B, Nb, N, Tsb) : 0;
-  if (rc) return rc;
-  IpmOpts O = to_ipm(opts);
-  if (!opts) O.max_iter = 3000;                        // as quad_solve_host
-  QBatchPtrs bp;
-  bp.x0 = x0; bp.xF = xF; bp.xWS = xWS; bp.Nb = mixed ? Nb : nullptr; bp.Tsb = mixed ? Tsb : nullptr;
-  bp.timeWS = timeWS; bp.xp = xp; bp.up = up; bp.ts = ts; bp.lp = lp; bp.slack = signed_dist ? slack : nullptr;
-  bp.exitflag = exitflag; bp.iters = iters; bp.kkt_err = kkt_err; bp.B = B;
-  rc = quad_solve_dev(*c, P, O, bp);
-  if (rc) return rc;
-  CK(to_host(c->prof_host, c->prof, 8, c->st));
-  CK(cudaStreamSynchronize(c->st));
-  float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-  if (solve_seconds) *solve_seconds = ms * 1e-3;
+  cudaStream_t st = c->st;
+  if (!scatter) CK(outs.copy_out(st));
+  CK(lay.copy_out(st));
+  std::vector<double> h;
+  if (scatter) {
+    h.resize(outs.bytes / sizeof(double));
+    CK(to_host((char*)h.data(), dout, outs.bytes, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  rc = quad_solve_seconds(*c, a.solve_seconds);
+  if (rc || !scatter) return rc;
+  scatter_horizons(a.xp, outs.in_copy(d.xp, h.data()), a.B, a.Nb, z.x, 12, 1);
+  scatter_horizons(a.up, outs.in_copy(d.up, h.data()), a.B, a.Nb, z.u, 4, 0);
+  scatter_horizons(a.ts, outs.in_copy(d.ts, h.data()), a.B, a.Nb, z.ns, 1, 1);
+  scatter_horizons(a.lp, outs.in_copy(d.lp, h.data()), a.B, a.Nb, z.l, 30, 1);
+  scatter_horizons(a.signed_dist ? a.slack : nullptr, outs.in_copy(d.slack, h.data()), a.B, a.Nb, z.s, 5, 1);
+  memcpy(a.kkt_err, outs.in_copy(d.kkt_err, h.data()), Bs * sizeof(double));
   return 0;
 }
 
-// obca_check_quadcopter_dev (Nb, Tsb null) and obca_check_quadcopter_mixed_dev: the refusals of obca_check_quadcopter[_mixed] in their
-// order, then constrSatisfaction on the caller's device arrays.
-static int quad_check_entry_dev(bool mixed, int B, int N, const int* Nb, const double* Tsb, const double* x, const double* u,
-                                const double* timeScale, const double* x0, const double* xF, double Ts, const double* lambda,
-                                const double* ob, double R, const obca_opts* opts, int* feasible, double* worst, void* stream) {
-  if (mixed && !Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
-  if (mixed && !Tsb) { set_err("null argument: Tsb"); return OBCA_ERR_ARG; }
-  if (B <= 0 || !x || !u || !timeScale || !x0 || !xF || !lambda || !ob || !feasible) { set_err("null argument"); return OBCA_ERR_ARG; }
+// obca_check_quadcopter[_dev] and obca_check_quadcopter_mixed[_dev].  Every per-problem array is laid out for the horizon N; Nb, Tsb
+// (mixed entries): per-problem horizons <= N and sampling times, otherwise both null.
+struct QuadCheck {
+  int B, N;
+  const int* Nb;
+  const double *Tsb, *x, *u, *timeScale, *x0, *xF;
+  double Ts;
+  const double *lambda, *ob;
+  double R;
+  const obca_opts* opts;
+  int* feasible;
+  double* worst;
+};
+
+// constrSatisfaction over the batch on the device's stream (Nb and Tsb together, and worst, may be null).
+static int quad_check_dev(DevCtx& c, const QuadProblem& P, const QuadCheck& a) {
+  const int grid = a.B < 4 * c.sms ? a.B : 4 * c.sms;
+  k_quad_check<<<grid, 128, 0, c.st>>>(P, a.B, a.Nb, a.Tsb, a.x0, a.xF, a.x, a.u, a.timeScale, a.lambda, a.feasible, a.worst);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+static int quad_check(const QuadCheck& a, Arrays at, bool mixed, void* stream) {
+  const bool host = at == Arrays::HOST;
+  int rc = mixed ? check_horizons(a.B, a.Nb, a.N, host) : 0;
+  if (!rc && mixed) rc = check_sampling_times(a.B, a.Tsb, host);
+  if (rc) return rc;
+  if (a.B <= 0 || !a.x || !a.u || !a.timeScale || !a.x0 || !a.xF || !a.lambda || !a.ob || !a.feasible) {
+    set_err("null argument"); return OBCA_ERR_ARG;
+  }
   QuadProblem P;
-  if (fill_quad_problem(P, N, Ts, R, ob, 0)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
+  if (fill_quad_problem(P, a.N, a.Ts, a.R, a.ob, 0)) { set_err("unsupported problem shape"); return OBCA_ERR_ARG; }
   DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
+  rc = get_ctx(a.opts ? a.opts->device : 0, &c);
   if (rc) return rc;
   std::lock_guard<std::recursive_mutex> lk(c->mu);
-  rc = wait_caller_stream(*c, stream);
+  QuadCheck d = a;      // the call on the staged arrays (host arrays)
+  DevLayout lay;        // host arrays: their staging
+  if (host) {
+    const size_t Bs = a.B;
+    const QuadSizes z = quad_sizes(a.N);
+    lay.in(d.x0, a.x0, 12 * Bs);
+    lay.in(d.xF, a.xF, 12 * Bs);
+    lay.in(d.x, a.x, z.x * Bs);
+    lay.in(d.u, a.u, z.u * Bs);
+    lay.in(d.timeScale, a.timeScale, z.ns * Bs);
+    lay.in(d.lambda, a.lambda, z.l * Bs);
+    lay.in(d.Nb, a.Nb, Bs);
+    lay.in(d.Tsb, a.Tsb, Bs);
+    lay.out(d.feasible, a.feasible, Bs);
+    lay.out(d.worst, a.worst, Bs);
+    rc = stage_in(*c, lay);
+    if (!mixed) { d.Nb = nullptr; d.Tsb = nullptr; }
+  } else {
+    rc = dev_start(*c, at, stream, a.B, a.Nb, a.N, a.Tsb);
+  }
+  if (!rc) rc = quad_check_dev(*c, P, d);
   if (rc) return rc;
-  rc = mixed ? check_batch_args_dev(*c, B, Nb, N, Tsb) : 0;
-  if (rc) return rc;
-  rc = quad_check_dev(*c, P, B, Nb, Tsb, x0, xF, x, u, timeScale, lambda, feasible, worst);
-  if (rc) return rc;
+  CK(lay.copy_out(c->st));
   CK(cudaStreamSynchronize(c->st));
   return 0;
 }
@@ -1319,41 +1340,40 @@ static int parking_plan_solve(int B, const double* x0, const double* xF, const d
     return 0;
   }
   // stage 3: gather the listed poses into the inputs of the mixed solve at the horizon M, once for every formulation
-  const size_t Qs = Bq, MS = M + 1;
+  const size_t Qs = Bq;
+  const ParkSizes zm = park_sizes(M, V, nOb), zc = park_sizes(Ncap, V, nOb);      // the solve's layout, the caller's
   obca_flow::Gather g;
   g.rx = po.rx; g.ry = po.ry; g.ryaw = po.ryaw; g.xWS = po.xWS; g.uWS = po.uWS; g.x0 = d0; g.xF = dF;
   obca_flow::Outs so;
   char* dout;
   DevLayout outs;
-  outs.add(so.xp, 4 * MS * Qs);
-  outs.add(so.up, 2 * (size_t)M * Qs);
-  outs.add(so.ts, MS * Qs);
-  outs.add(so.lp, (size_t)V * MS * Qs);
-  outs.add(so.np, 4 * (size_t)nOb * MS * Qs);
-  outs.add(so.sl, (size_t)nOb * MS * Qs);
+  outs.add(so.xp, zm.x * Qs);
+  outs.add(so.up, zm.u * Qs);
+  outs.add(so.ts, zm.ns * Qs);
+  outs.add(so.lp, zm.l * Qs);
+  outs.add(so.np, zm.n * Qs);
+  outs.add(so.sl, zm.sl * Qs);
   outs.add(so.kkt_err, Qs);
   outs.add(so.exitflag, Qs);
   outs.add(so.iters, Qs);
   outs.add(so.feasible, Qs);
   outs.add(so.strict, Qs);
   DevLayout sl_;
-  sl_.add(g.mrx, MS * Qs);
-  sl_.add(g.mry, MS * Qs);
-  sl_.add(g.mryaw, MS * Qs);
-  sl_.add(g.mxWS, 4 * MS * Qs);
-  sl_.add(g.muWS, 2 * (size_t)M * Qs);
+  sl_.add(g.mrx, zm.ns * Qs);
+  sl_.add(g.mry, zm.ns * Qs);
+  sl_.add(g.mryaw, zm.ns * Qs);
+  sl_.add(g.mxWS, zm.x * Qs);
+  sl_.add(g.muWS, zm.u * Qs);
   sl_.add(g.mx0, 4 * Qs);
   sl_.add(g.mxF, 4 * Qs);
   sl_.add(dout, outs.bytes);
   DevBuf dsolve;
   CK(alloc_layout(dsolve, sl_));
   outs.place(dout);
-  const size_t items = Qs * MS;
+  const size_t items = Qs * zm.ns;
   const int threads = 256, blocks = (int)((items + threads - 1) / threads);
   k_flow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
   CK(cudaGetLastError());
-  obca_opts o2;
-  if (opts) o2 = *opts; else obca_default_opts(&o2);
   for (int f = 0; f < nf; ++f) {
     const int sd = sets[f].signed_dist;
     const obca_parking_flow_out& u = *sets[f].out;
@@ -1361,23 +1381,23 @@ static int parking_plan_solve(int B, const double* x0, const double* xF, const d
     fill_problem(PM, M, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, sd);      // the shape passed above, with 2 <= M <= Ncap
     // stage 4: the mixed solve (DualMultWS inside) into outputs that start as zeros; stage 5: ParkingConstraints on its outputs
     CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
-    rc = parking_solve_dev(Bq, M, dNb, nOb, vOb, A, b, g.mx0, g.mxF, Ts, L, ego, XYbounds, g.mrx, g.mry, g.mryaw, g.mxWS, g.muWS, nullptr,
-                           nullptr, fixTime, sd, &o2, so.xp, so.up, so.ts, so.lp, so.np, so.sl, so.exitflag, so.iters, so.kkt_err,
-                           u.solve_seconds);
+    rc = parking_solve_dev(*c, PM, {Bq, M, dNb, nOb, vOb, A, b, g.mx0, g.mxF, Ts, L, ego, XYbounds, g.mrx, g.mry, g.mryaw, g.mxWS, g.muWS,
+                                    nullptr, nullptr, fixTime, sd, opts, so.xp, so.up, so.ts, so.lp, so.np, so.sl, so.exitflag, so.iters,
+                                    so.kkt_err, u.solve_seconds});
     if (rc) return rc;
-    rc = check_parking_dev(*c, PM, Bq, dNb, g.mx0, g.mxF, so.xp, so.up, so.lp, so.np, so.ts, so.sl, sd, so.feasible, nullptr, so.strict);
+    rc = check_parking_dev(*c, PM, {Bq, M, dNb, nOb, vOb, A, b, g.mx0, g.mxF, Ts, L, ego, XYbounds, so.xp, so.up, so.lp, so.np, so.ts,
+                                    so.sl, fixTime, sd, opts, so.feasible, nullptr, so.strict});
     if (rc) return rc;
     // stage 6: the solved poses' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
     // write keeps the caller's value), then back in one pass; this staging is freed before the next formulation runs
     obca_flow::Outs d;
-    const size_t NS = Ncap + 1;
     DevLayout ol;
-    ol.inout(d.xp, u.xp, 4 * NS * Bs);
-    ol.inout(d.up, u.up, 2 * (size_t)Ncap * Bs);
-    ol.inout(d.ts, u.ts, NS * Bs);
-    ol.inout(d.lp, u.lp, (size_t)V * NS * Bs);
-    ol.inout(d.np, u.np, 4 * (size_t)nOb * NS * Bs);
-    ol.inout(d.sl, u.sl, (size_t)nOb * NS * Bs);
+    ol.inout(d.xp, u.xp, zc.x * Bs);
+    ol.inout(d.up, u.up, zc.u * Bs);
+    ol.inout(d.ts, u.ts, zc.ns * Bs);
+    ol.inout(d.lp, u.lp, zc.l * Bs);
+    ol.inout(d.np, u.np, zc.n * Bs);
+    ol.inout(d.sl, u.sl, zc.sl * Bs);
     ol.inout(d.kkt_err, u.kkt_err, Bs);
     ol.inout(d.exitflag, u.exitflag, Bs);
     ol.inout(d.iters, u.iters, Bs);
@@ -1481,24 +1501,25 @@ static int quad_plan_solve(int B, const double* x0, const double* xF, const doub
   // formulation.  The check takes the Dist bounds whatever the formulation, as obca_check_quadcopter_mixed does.
   QuadProblem PC;
   fill_quad_problem(PC, M, std::nan(""), R, ob, 0);      // the shape passed above, with 2 <= M <= Ncap
-  const size_t Qs = Bq, MS = M + 1;
+  const size_t Qs = Bq;
+  const QuadSizes zm = quad_sizes(M), zc = quad_sizes(Ncap);      // the solve's layout, the caller's
   obca_qflow::Gather g;
   g.rx = po.rx; g.ry = po.ry; g.rz = po.rz; g.x0 = d0; g.xF = dF; g.Ts = Ts;
   obca_qflow::Outs so;
   char* dout;
   DevLayout outs;
-  outs.add(so.xp, 12 * MS * Qs);
-  outs.add(so.up, 4 * (size_t)M * Qs);
-  outs.add(so.ts, MS * Qs);
-  outs.add(so.lp, 30 * MS * Qs);
-  outs.add(so.slack, 5 * MS * Qs);
+  outs.add(so.xp, zm.x * Qs);
+  outs.add(so.up, zm.u * Qs);
+  outs.add(so.ts, zm.ns * Qs);
+  outs.add(so.lp, zm.l * Qs);
+  outs.add(so.slack, zm.s * Qs);
   outs.add(so.kkt_err, Qs);
   outs.add(so.worst, Qs);
   outs.add(so.exitflag, Qs);
   outs.add(so.iters, Qs);
   outs.add(so.feasible, Qs);
   DevLayout sl_;
-  sl_.add(g.mxWS, 12 * MS * Qs);
+  sl_.add(g.mxWS, zm.x * Qs);
   sl_.add(g.mx0, 12 * Qs);
   sl_.add(g.mxF, 12 * Qs);
   sl_.add(g.mTsb, Qs);
@@ -1507,16 +1528,10 @@ static int quad_plan_solve(int B, const double* x0, const double* xF, const doub
   CK(alloc_layout(dsolve, sl_));
   outs.place(dout);
   so.Tsb = g.mTsb;
-  const size_t items = Qs * MS;
+  const size_t items = Qs * zm.ns;
   const int threads = 256, blocks = (int)((items + threads - 1) / threads);
   k_qflow_gather<<<blocks, threads, 0, st>>>(Bq, M, cap, dlist, dNb, g);
   CK(cudaGetLastError());
-  IpmOpts O = to_ipm(opts);
-  if (!opts) O.max_iter = 3000;                        // as obca_quadcopter_solve_mixed
-  QBatchPtrs bp;
-  bp.x0 = g.mx0; bp.xF = g.mxF; bp.xWS = g.mxWS; bp.Nb = dNb; bp.Tsb = g.mTsb;
-  bp.timeWS = timeWS; bp.xp = so.xp; bp.up = so.up; bp.ts = so.ts; bp.lp = so.lp; bp.slack = so.slack;
-  bp.exitflag = so.exitflag; bp.iters = so.iters; bp.kkt_err = so.kkt_err; bp.B = Bq;
   for (int f = 0; f < nf; ++f) {
     const int sd = sets[f].signed_dist;
     const obca_quadcopter_flow_out& u = *sets[f].out;
@@ -1524,22 +1539,22 @@ static int quad_plan_solve(int B, const double* x0, const double* xF, const doub
     fill_quad_problem(PM, M, std::nan(""), R, ob, sd);
     // stage 4: the mixed solve into outputs that start as zeros; stage 5: constrSatisfaction on its outputs
     CK(cudaMemsetAsync(dout, 0, outs.bytes, st));
-    rc = quad_solve_dev(*c, PM, O, bp);
+    rc = quad_solve_dev(*c, PM, {Bq, M, dNb, g.mTsb, g.mx0, g.mxF, std::nan(""), R, ob, g.mxWS, timeWS, sd, opts, so.xp, so.up, so.ts,
+                                 so.lp, so.slack, so.exitflag, so.iters, so.kkt_err, u.solve_seconds});
     if (rc) return rc;
-    CK(to_host(c->prof_host, c->prof, 8, st));
-    rc = quad_check_dev(*c, PC, Bq, dNb, g.mTsb, g.mx0, g.mxF, so.xp, so.up, so.ts, so.lp, so.feasible, so.worst);
+    rc = quad_check_dev(*c, PC, {Bq, M, dNb, g.mTsb, so.xp, so.up, so.ts, g.mx0, g.mxF, std::nan(""), so.lp, ob, R, opts, so.feasible,
+                                 so.worst});
     if (rc) return rc;
     // stage 6: the solved pairs' outputs into the caller's arrays (copied to the device first, so that every entry the call does not
     // write keeps the caller's value), then back in one pass; this staging is freed before the next formulation runs
     double* slack_out = sd ? u.slack : nullptr;      // the Dist formulation has no slacks
     obca_qflow::Outs d;
-    const size_t NS = Ncap + 1;
     DevLayout ol;
-    ol.inout(d.xp, u.xp, 12 * NS * Bs);
-    ol.inout(d.up, u.up, 4 * (size_t)Ncap * Bs);
-    ol.inout(d.ts, u.ts, NS * Bs);
-    ol.inout(d.lp, u.lp, 30 * NS * Bs);
-    ol.inout(d.slack, slack_out, slack_out ? 5 * NS * Bs : 0);
+    ol.inout(d.xp, u.xp, zc.x * Bs);
+    ol.inout(d.up, u.up, zc.u * Bs);
+    ol.inout(d.ts, u.ts, zc.ns * Bs);
+    ol.inout(d.lp, u.lp, zc.l * Bs);
+    ol.inout(d.slack, slack_out, slack_out ? zc.s * Bs : 0);
     ol.inout(d.kkt_err, u.kkt_err, Bs);
     ol.inout(d.Tsb, Tsb, Bs);
     ol.inout(d.worst, u.worst, u.worst ? Bs : 0);
@@ -1555,9 +1570,8 @@ static int quad_plan_solve(int B, const double* x0, const double* xF, const doub
     CK(cudaGetLastError());
     CK(ol.copy_out(st));
     CK(cudaStreamSynchronize(st));
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-    if (u.solve_seconds) *u.solve_seconds = ms * 1e-3;
+    rc = quad_solve_seconds(*c, u.solve_seconds);
+    if (rc) return rc;
   }
   CK(pl.copy_out(st));
   CK(cudaStreamSynchronize(st));
@@ -1602,8 +1616,8 @@ int obca_parking_solve_batch_dev(int B, int N, int nOb, const int* vOb, const do
                                  int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up,
                                  double* ts, double* lp, double* np, double* sl, int* exitflag, int* iters,
                                  double* kkt_err, double* solve_seconds) {
-  return parking_solve_dev(B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS,
-                           fixTime, signed_dist, opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds);
+  return parking_solve({B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS, fixTime, signed_dist,
+                        opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds}, Arrays::DEV, false, nullptr);
 }
 
 int obca_parking_solve_batch(int B, int N, int nOb, const int* vOb, const double* A, const double* b,
@@ -1613,8 +1627,8 @@ int obca_parking_solve_batch(int B, int N, int nOb, const int* vOb, const double
                              int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
                              double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                              double* solve_seconds) {
-  return parking_solve_host(false, B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS,
-                            fixTime, signed_dist, opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds);
+  return parking_solve({B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS, fixTime, signed_dist,
+                        opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds}, Arrays::HOST, false, nullptr);
 }
 
 int obca_parking_solve_mixed(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
@@ -1624,39 +1638,14 @@ int obca_parking_solve_mixed(int B, const int* Nb, int Nmax, int nOb, const int*
                              int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
                              double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                              double* solve_seconds) {
-  return parking_solve_host(true, B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS,
-                            fixTime, signed_dist, opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds);
+  return parking_solve({B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS, fixTime, signed_dist,
+                        opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds}, Arrays::HOST, true, nullptr);
 }
 
 int obca_dualmultws_batch(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* ego,
                           const double* rx, const double* ry, const double* ryaw, const obca_opts* opts, double* lp,
                           double* np, double* dd) {
-  if (B <= 0 || !vOb || !A || !b || !ego || !rx || !ry || !ryaw || !lp || !np) { set_err("null argument"); return OBCA_ERR_ARG; }
-  ParkProblem P;
-  double xy[4] = {0, 1, 0, 1};
-  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, 1.0, 1.0, ego, xy, 0, 1)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
-  DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  const size_t NS = N + 1, nr = NS * B, nl = (size_t)P.V * NS * B, nn = 4 * (size_t)nOb * NS * B, ndd = (size_t)nOb * NS * B;
-  double *drx, *dry, *dryaw, *dl, *dn, *ddv;
-  DevLayout lay;
-  lay.in(drx, rx, nr);
-  lay.in(dry, ry, nr);
-  lay.in(dryaw, ryaw, nr);
-  lay.out(dl, lp, nl);
-  lay.out(dn, np, nn);
-  lay.out(ddv, dd, ndd);
-  rc = ensure((void**)&c->stage, &c->stage_bytes, lay.bytes);
-  if (rc) return rc;
-  lay.place(c->stage);
-  CK(lay.copy_in(c->st));
-  rc = run_dualws(*c, P, B, nullptr, drx, dry, dryaw, dl, dn, ddv);
-  if (rc) return rc;
-  CK(lay.copy_out(c->st));
-  CK(cudaStreamSynchronize(c->st));
-  return 0;
+  return dualmultws({B, N, nOb, vOb, A, b, ego, rx, ry, ryaw, opts, lp, np, dd}, Arrays::HOST, nullptr);
 }
 
 int obca_check_parking(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* x0,
@@ -1664,8 +1653,8 @@ int obca_check_parking(int B, int N, int nOb, const int* vOb, const double* A, c
                        const double* x, const double* u, const double* l, const double* n, const double* timeScale,
                        const double* sl, int fixTime, int sd, const obca_opts* opts, int* feasible, int* e,
                        int* strict) {
-  return check_parking(B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime, sd,
-                       opts, feasible, e, strict);
+  return check_parking({B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime, sd, opts, feasible,
+                        e, strict}, Arrays::HOST, false, nullptr);
 }
 
 int obca_check_parking_mixed(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
@@ -1673,43 +1662,40 @@ int obca_check_parking_mixed(int B, const int* Nb, int Nmax, int nOb, const int*
                              const double* XYbounds, const double* x, const double* u, const double* l, const double* n,
                              const double* timeScale, const double* sl, int fixTime, int sd, const obca_opts* opts,
                              int* feasible, int* e, int* strict) {
-  const int rc = check_horizons(B, Nb, Nmax);
-  if (rc) return rc;
-  return check_parking(B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime, sd,
-                       opts, feasible, e, strict);
+  return check_parking({B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime, sd, opts, feasible,
+                        e, strict}, Arrays::HOST, true, nullptr);
 }
 
 int obca_quadcopter_solve_batch(int B, int N, const double* x0, const double* xF, double Ts, double R, const double* ob,
                                 const double* xWS, double timeWS, int signed_dist, const obca_opts* opts, double* xp,
                                 double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters,
                                 double* kkt_err, double* solve_seconds) {
-  return quad_solve_host(false, B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
-                         exitflag, iters, kkt_err, solve_seconds);
+  return quad_solve({B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack, exitflag, iters,
+                     kkt_err, solve_seconds}, Arrays::HOST, false, nullptr);
 }
 
+// The mixed quadcopter entries' batch has no sampling time of its own: Ts is NaN, so that a read of it instead of Tsb[b] could not go
+// unnoticed.
 int obca_quadcopter_solve_mixed(int B, const int* Nb, int Nmax, const double* x0, const double* xF, const double* Tsb,
                                 double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
                                 const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
                                 int* exitflag, int* iters, double* kkt_err, double* solve_seconds) {
-  // the batch has no sampling time of its own: NaN, so that a read of it instead of Tsb[b] could not go unnoticed
-  return quad_solve_host(true, B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
-                         exitflag, iters, kkt_err, solve_seconds);
+  return quad_solve({B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack, exitflag, iters,
+                     kkt_err, solve_seconds}, Arrays::HOST, true, nullptr);
 }
 
 int obca_check_quadcopter(int B, int N, const double* x, const double* u, const double* timeScale, const double* x0,
                           const double* xF, double Ts, const double* lambda, const double* ob, double R,
                           const obca_opts* opts, int* feasible, double* worst) {
-  return quad_check_host(B, N, nullptr, nullptr, x, u, timeScale, x0, xF, Ts, lambda, ob, R, opts, feasible, worst);
+  return quad_check({B, N, nullptr, nullptr, x, u, timeScale, x0, xF, Ts, lambda, ob, R, opts, feasible, worst}, Arrays::HOST, false,
+                    nullptr);
 }
 
 int obca_check_quadcopter_mixed(int B, const int* Nb, int Nmax, const double* x, const double* u, const double* timeScale,
                                 const double* x0, const double* xF, const double* Tsb, const double* lambda,
                                 const double* ob, double R, const obca_opts* opts, int* feasible, double* worst) {
-  int rc = check_horizons(B, Nb, Nmax);
-  if (rc) return rc;
-  rc = check_sampling_times(B, Tsb);
-  if (rc) return rc;
-  return quad_check_host(B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst);
+  return quad_check({B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst}, Arrays::HOST, true,
+                    nullptr);
 }
 
 int obca_parking_solve_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
@@ -1719,44 +1705,14 @@ int obca_parking_solve_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const 
                                  int fixTime, int signed_dist, const obca_opts* opts, double* xp, double* up, double* ts,
                                  double* lp, double* np, double* sl, int* exitflag, int* iters, double* kkt_err,
                                  double* solve_seconds, void* stream) {
-  // the refusals of obca_parking_solve_mixed in its order (the horizons' values are checked on the device below)
-  if (B <= 0 || !vOb || !A || !b || !ego || !XYbounds || !x0 || !xF || !rx || !ry || !ryaw || !xWS || !uWS || !xp || !up ||
-      !ts || !lp || !np || !exitflag || !iters || !kkt_err) { set_err("null argument"); return OBCA_ERR_ARG; }
-  if (!Nb) { set_err("null argument: Nb"); return OBCA_ERR_ARG; }
-  ParkProblem P;
-  if (const int e_ = fill_problem(P, Nmax, nOb, vOb, A, b, Ts, L, ego, XYbounds, fixTime, signed_dist)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
-  int rc = check_park_horizon(Nmax);
-  if (rc) return rc;
-  DevCtx* c;
-  rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  rc = wait_caller_stream(*c, stream);
-  if (rc) return rc;
-  rc = check_batch_args_dev(*c, B, Nb, Nmax, nullptr);
-  if (rc) return rc;
-  // the kernels write each problem's outputs over its own horizon only: the caller's arrays need no scatter
-  return parking_solve_dev(B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS, fixTime,
-                           signed_dist, opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds);
+  return parking_solve({B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, rx, ry, ryaw, xWS, uWS, lWS, nWS, fixTime, signed_dist,
+                        opts, xp, up, ts, lp, np, sl, exitflag, iters, kkt_err, solve_seconds}, Arrays::STREAM, true, stream);
 }
 
 int obca_dualmultws_batch_dev(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* ego,
                               const double* rx, const double* ry, const double* ryaw, const obca_opts* opts, double* lp,
                               double* np, double* dd, void* stream) {
-  if (B <= 0 || !vOb || !A || !b || !ego || !rx || !ry || !ryaw || !lp || !np) { set_err("null argument"); return OBCA_ERR_ARG; }
-  ParkProblem P;
-  double xy[4] = {0, 1, 0, 1};
-  if (const int e_ = fill_problem(P, N, nOb, vOb, A, b, 1.0, 1.0, ego, xy, 0, 1)) { set_err(shape_error(e_)); return OBCA_ERR_ARG; }
-  DevCtx* c;
-  int rc = get_ctx(opts ? opts->device : 0, &c);
-  if (rc) return rc;
-  std::lock_guard<std::recursive_mutex> lk(c->mu);
-  rc = wait_caller_stream(*c, stream);
-  if (rc) return rc;
-  rc = run_dualws(*c, P, B, nullptr, rx, ry, ryaw, lp, np, dd);
-  if (rc) return rc;
-  CK(cudaStreamSynchronize(c->st));
-  return 0;
+  return dualmultws({B, N, nOb, vOb, A, b, ego, rx, ry, ryaw, opts, lp, np, dd}, Arrays::STREAM, stream);
 }
 
 int obca_check_parking_dev(int B, int N, int nOb, const int* vOb, const double* A, const double* b, const double* x0,
@@ -1764,8 +1720,8 @@ int obca_check_parking_dev(int B, int N, int nOb, const int* vOb, const double* 
                            const double* x, const double* u, const double* l, const double* n, const double* timeScale,
                            const double* sl, int fixTime, int sd, const obca_opts* opts, int* feasible, int* e,
                            int* strict, void* stream) {
-  return check_parking_entry_dev(false, B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime,
-                                 sd, opts, feasible, e, strict, stream);
+  return check_parking({B, N, nullptr, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime, sd, opts, feasible,
+                        e, strict}, Arrays::STREAM, false, stream);
 }
 
 int obca_check_parking_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const int* vOb, const double* A, const double* b,
@@ -1773,37 +1729,38 @@ int obca_check_parking_mixed_dev(int B, const int* Nb, int Nmax, int nOb, const 
                                  const double* XYbounds, const double* x, const double* u, const double* l, const double* n,
                                  const double* timeScale, const double* sl, int fixTime, int sd, const obca_opts* opts,
                                  int* feasible, int* e, int* strict, void* stream) {
-  return check_parking_entry_dev(true, B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime,
-                                 sd, opts, feasible, e, strict, stream);
+  return check_parking({B, Nmax, Nb, nOb, vOb, A, b, x0, xF, Ts, L, ego, XYbounds, x, u, l, n, timeScale, sl, fixTime, sd, opts, feasible,
+                        e, strict}, Arrays::STREAM, true, stream);
 }
 
 int obca_quadcopter_solve_batch_dev(int B, int N, const double* x0, const double* xF, double Ts, double R, const double* ob,
                                     const double* xWS, double timeWS, int signed_dist, const obca_opts* opts, double* xp,
                                     double* up, double* ts, double* lp, double* slack, int* exitflag, int* iters,
                                     double* kkt_err, double* solve_seconds, void* stream) {
-  return quad_solve_entry_dev(false, B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
-                              exitflag, iters, kkt_err, solve_seconds, stream);
+  return quad_solve({B, N, nullptr, nullptr, x0, xF, Ts, R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack, exitflag, iters,
+                     kkt_err, solve_seconds}, Arrays::STREAM, false, stream);
 }
 
 int obca_quadcopter_solve_mixed_dev(int B, const int* Nb, int Nmax, const double* x0, const double* xF, const double* Tsb,
                                     double R, const double* ob, const double* xWS, double timeWS, int signed_dist,
                                     const obca_opts* opts, double* xp, double* up, double* ts, double* lp, double* slack,
                                     int* exitflag, int* iters, double* kkt_err, double* solve_seconds, void* stream) {
-  return quad_solve_entry_dev(true, B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack,
-                              exitflag, iters, kkt_err, solve_seconds, stream);
+  return quad_solve({B, Nmax, Nb, Tsb, x0, xF, std::nan(""), R, ob, xWS, timeWS, signed_dist, opts, xp, up, ts, lp, slack, exitflag, iters,
+                     kkt_err, solve_seconds}, Arrays::STREAM, true, stream);
 }
 
 int obca_check_quadcopter_dev(int B, int N, const double* x, const double* u, const double* timeScale, const double* x0,
                               const double* xF, double Ts, const double* lambda, const double* ob, double R,
                               const obca_opts* opts, int* feasible, double* worst, void* stream) {
-  return quad_check_entry_dev(false, B, N, nullptr, nullptr, x, u, timeScale, x0, xF, Ts, lambda, ob, R, opts, feasible, worst, stream);
+  return quad_check({B, N, nullptr, nullptr, x, u, timeScale, x0, xF, Ts, lambda, ob, R, opts, feasible, worst}, Arrays::STREAM, false,
+                    stream);
 }
 
 int obca_check_quadcopter_mixed_dev(int B, const int* Nb, int Nmax, const double* x, const double* u, const double* timeScale,
                                     const double* x0, const double* xF, const double* Tsb, const double* lambda,
                                     const double* ob, double R, const obca_opts* opts, int* feasible, double* worst, void* stream) {
-  return quad_check_entry_dev(true, B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst,
-                              stream);
+  return quad_check({B, Nmax, Nb, Tsb, x, u, timeScale, x0, xF, std::nan(""), lambda, ob, R, opts, feasible, worst}, Arrays::STREAM, true,
+                    stream);
 }
 
 int obca_parking_plan_solve_goals(int B, const double* x0, const double* xF, const double* ox, const double* oy, int n_ob, double Ts,

@@ -1,6 +1,6 @@
 """The device-pointer entries on the caller's stream and their PyTorch ops, without a GPU: each entry is declared, exported and typed as
 its host-pointer twin plus a stream; it refuses what its twin refuses, with the same code and message, before any device work; it
-stops at OBCA_ERR_NO_DEVICE without a device; the ops register, trace under FakeTensorMode with the documented shapes and dtypes, and
+stops at OBCA_ERR_NO_DEVICE without a device; the mixed twins refuse two faults in their order; the ops register, trace under FakeTensorMode with the documented shapes and dtypes, and
 refuse CPU, float32 and mixed-device tensors with ValueError."""
 import ctypes as C
 import os
@@ -117,6 +117,35 @@ def test_no_device_without_a_gpu(name):
         pytest.skip("a CUDA device is visible")
     assert _call(name) == (-2, "no CUDA device visible")
     assert _call(name, stream=C.c_void_p(1234)) == (-2, "no CUDA device visible")      # never touched before the device check
+
+
+# A bad host-resident horizon together with a second fault: the solves check their required pointers before the horizons, the
+# checkers the horizons first; every mixed entry checks the horizons' values before the shape, the horizon bound and Tsb.
+BAD_NB = np.array([80, 80, 1, 80], np.int32)
+
+
+def _bad_nb(Nmax, q=2, n=1):
+    return f"Nb[{q}] = {n} outside [2, Nmax = {Nmax}]"
+
+
+@pytest.mark.parametrize("name,over,msg", [
+    ("obca_parking_solve_mixed", dict(x0=None), "null argument"),
+    ("obca_parking_solve_mixed", dict(nOb=0), _bad_nb(80)),
+    ("obca_parking_solve_mixed", dict(vOb=np.array([5, 4, 4], np.int32)), _bad_nb(80)),
+    ("obca_parking_solve_mixed", dict(Nmax=320), _bad_nb(320)),
+    ("obca_check_parking_mixed", dict(x0=None), _bad_nb(80)),
+    ("obca_check_parking_mixed", dict(nOb=0), _bad_nb(80)),
+    ("obca_check_parking_mixed", dict(vOb=np.array([5, 4, 4], np.int32)), _bad_nb(80)),
+    ("obca_quadcopter_solve_mixed", dict(x0=None), "null argument"),
+    ("obca_quadcopter_solve_mixed", dict(Nmax=1), _bad_nb(1, q=0, n=80)),
+    ("obca_quadcopter_solve_mixed", dict(Nmax=512), _bad_nb(512)),
+    ("obca_quadcopter_solve_mixed", dict(Tsb=None), _bad_nb(100)),
+    ("obca_check_quadcopter_mixed", dict(x0=None), _bad_nb(100)),
+    ("obca_check_quadcopter_mixed", dict(Nmax=1), _bad_nb(1, q=0, n=80)),
+    ("obca_check_quadcopter_mixed", dict(Tsb=None), _bad_nb(100)),
+])
+def test_mixed_host_twin_refuses_a_bad_horizon_and_a_second_fault_in_order(name, over, msg):
+    assert _call(name, Nb=BAD_NB, **over) == (-1, msg)
 
 
 # ---- the PyTorch ops ---------------------------------------------------------------------------------------------------------------
